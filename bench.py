@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the fake-quantization hot path on B200.
+"""bench.py -- headline benchmark of the fake-quantization hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--sweep] [--train]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--sweep] [--train] [--dump-outputs DIR]
 
 A *step* is one pass of the fused uniform fake-quant forward+backward kernel
 (qd_uniform_fwd_bwd, 'complicated' min/max backward) over one 64 Mi-float32
@@ -14,13 +14,19 @@ Printed JSON line (rank 0):
   e2e        same metric through the host-buffer C-ABI call (pinned host tensors in,
              host tensors out; H2D + kernel + D2H inside the timed region)
   roofline   achieved GB/s of the kernel vs the measured HBM copy peak
-  cpu_baseline  the reference's op chain (oracle/torch_chain.py, a port: /root/reference
-             is not on the GPU box) on the host cores, bounded sample
+  cpu_baseline  the reference's op chain (oracle/torch_chain.py, a port of the reference's
+             torch ops) on the host cores, bounded sample
 With N > 1 every rank runs an independent replica (the op does not shard:
 DESIGN.md "Multi-GPU"), timing is the max over ranks.
 
 --impl reference times the reference's CPU implementation of the path
 (the op-chain port) on the host, same metric and unit.
+
+--dump-outputs DIR writes what the last timed step returned (q and gout) as
+DIR/q.npy and DIR/gout.npy, float32: the same seeded sample of DUMP_BUCKETS
+whole buckets from each, in tensor order (DIR/buckets.npy, float64, holds the
+index of every sampled bucket).  The inputs are seeded, so two builds run
+with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -40,6 +46,8 @@ LEVELS = 16
 BUCKET = 256
 BYTES_PER_ELEM = 16        # x, g read; q, gout written
 MODE_NAME = "minmax"
+DUMP_BUCKETS = 1 << 14     # 4 Mi elements per dumped array: 16 MiB each, about 34 MB in all
+H100_HBM_GBS = 3350.0      # H100 SXM data sheet HBM3 bandwidth, used when no measured peak is present
 
 
 def load_peaks():
@@ -47,7 +55,7 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return H100_HBM_GBS, "fallback: H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
 
 
 class ClockSampler(threading.Thread):
@@ -242,7 +250,7 @@ def workload_config(n_gpus):
                         f"s={LEVELS}, bucket_size={BUCKET}, {BYTES_PER_ELEM} algorithmic bytes/element",
             "elements": N_ELEMS, "levels": LEVELS, "bucket_size": BUCKET, "backward": MODE_NAME,
             "parallelism": f"replicas x{n_gpus} (op does not shard)",
-            "l2_policy": "inputs+outputs are 1 GiB per step, larger than the 126 MB L2; no flush needed"}
+            "l2_policy": "inputs+outputs are 1 GiB per step, larger than the 50 MB L2; no flush needed"}
 
 
 # ----------------------------------------------------------------------------- training legs
@@ -493,6 +501,20 @@ def cpu_model_quant_ms(sizes, levels, bucket, repeats=3):
 
 
 # ----------------------------------------------------------------------------- GPU arm
+def dump_outputs(out_dir, arrays):
+    """Writes the same seeded sample of DUMP_BUCKETS whole buckets of every array (float32) and the sampled
+    bucket indices (float64) to out_dir."""
+    import numpy as np
+    import torch
+    buckets = np.sort(np.random.default_rng(0).choice(N_ELEMS // BUCKET, DUMP_BUCKETS, replace=False))
+    pos = (buckets[:, None] * BUCKET + np.arange(BUCKET)[None, :]).reshape(-1)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "buckets.npy"), buckets.astype(np.float64))
+    for name, t in arrays.items():
+        idx = torch.from_numpy(pos).to(t.device)
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.index_select(0, idx).float().cpu().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -506,6 +528,8 @@ def main():
                     help="CIFAR10-shaped quantized-distillation steps/s (BASELINE configs 2/3/4); auto = student at every N, "
                          "WRN-16-22 at N=1 and N=8, differentiable quantization at N=1")
     ap.add_argument("--train-steps", type=int, default=40)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write a seeded sample of the last timed step's q and gout to DIR/*.npy (float32)")
     ap.add_argument("--ref-elements", type=int, default=0,
                     help="TEST HOOK for --impl reference: run the CPU arm on fewer elements (the line says so; not a bench value)")
     args = ap.parse_args()
@@ -572,6 +596,8 @@ def main():
     if world > 1:
         dist.barrier()
     ms = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"q": q, "gout": gout})
     clocks = sampler.stop()
     if world > 1:
         t = torch.tensor([ms], device=dev)
@@ -661,7 +687,7 @@ def main():
                                          "no kernel, all ranks concurrently, in the e2e leg's unit"}},
         "gpu_launches": steps,
         "roofline": {"bound": "hbm", "achieved": round(per_gpu_gbs, 1), "peak": peak, "unit": "GB/s",
-                     "frac": round(per_gpu_gbs / peak, 4), "frac_of_nominal_8000": round(per_gpu_gbs / 8000.0, 4),
+                     "frac": round(per_gpu_gbs / peak, 4), "frac_of_datasheet_3350": round(per_gpu_gbs / H100_HBM_GBS, 4),
                      "peak_source": peak_src, "traffic": None, "traffic_source": None,
                      "kernel": "qd::warp_rows_kernel<OP_UNIFORM, BWD_MINMAX, R=2, VEC>",
                      "algorithmic_bytes_per_launch": N_ELEMS * BYTES_PER_ELEM},
@@ -682,7 +708,7 @@ def main():
         out["cpu_baseline"] = {"value": round(gbs, 3), "unit": "GB/s", "cores": threads, "kind": "port",
                                "sample": f"full workload ({N_ELEMS} elements), mean of 3 passes after 1 warm-up "
                                          f"({sec * 1e3:.0f} ms per pass), oracle/torch_chain.py (the reference's torch op "
-                                         "chain; /root/reference is absent on the GPU box); thread count tuned over powers "
+                                         "chain); thread count tuned over powers "
                                          f"of two up to the usable CPUs on {TUNE_ELEMS} elements",
                                "host_cpus_visible": os.cpu_count(), "host_cpus_usable": usable_cpus()}
     which = {"none": [], "student": ["student"], "wrn": ["wrn"], "diffquant": ["diffquant"], "all": ["student", "wrn", "diffquant"],

@@ -1,5 +1,5 @@
 /*
- * qd_b200.h -- C ABI of libqd_b200.so: the B200 (sm_100a) implementation of the
+ * qd_b200.h -- C ABI of libqd_b200.so: the H100 (sm_90a) implementation of the
  * fake-quantization hot path of antspy/quantized_distillation.
  *
  * The reference has no FFI layer: its boundary for this path is the Python

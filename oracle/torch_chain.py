@@ -2,13 +2,13 @@
 
 The reference's CPU implementation of the hot path is a chain of stock torch
 tensor ops (clone, min, max, sub_, div_, mul_, round_, div_, mul_, add_, ...;
-SURVEY.md section 3.1).  /root/reference does not exist on the GPU box, so this
+SURVEY.md section 3.1).  The reference is not a dependency of this project, so this
 module restates that chain, op for op and pass for pass, with the same torch
 CPU kernels, so that ``bench.py --impl reference`` and the ``cpu_baseline`` leg
 time the same memory passes the reference makes on the host cores
 (``kind: "port"``).  The functions are device-agnostic like the reference's own code, so
 tools/plan_bench.py can also time "the reference's stock-torch op chain on the same
-B200" next to the fused kernels.  It is also a second oracle, independent of the NumPy one,
+GPU" next to the fused kernels.  It is also a second oracle, independent of the NumPy one,
 and is pinned bit-for-bit against the golden vectors in
 tests/test_oracle_golden.py::test_torch_chain_matches_golden.
 

@@ -1,4 +1,4 @@
-"""quantized_distillation_b200 -- B200 (sm_100a) implementation of the
+"""quantized_distillation_b200 -- H100 (sm_90a) implementation of the
 fake-quantization hot path of antspy/quantized_distillation.
 
     from quantized_distillation_b200 import quantization        # same names as the reference package

@@ -77,7 +77,7 @@ def lib() -> C.CDLL:
             if _lib is None:
                 if not os.path.exists(LIB_PATH):
                     raise ImportError(
-                        f"{LIB_PATH} not found: build the sm_100a extension first "
+                        f"{LIB_PATH} not found: build the sm_90a extension first "
                         "(python -c 'import __graft_entry__ as g; g.build()'). There is no CPU fallback.")
                 handle = C.CDLL(LIB_PATH)
                 for name, (res, args) in SIGNATURES.items():
@@ -129,7 +129,7 @@ def check(rc: int) -> None:
 
 def require_cuda() -> None:
     if not torch.cuda.is_available():
-        raise RuntimeError("quantized_distillation_b200 needs a CUDA device (B200, sm_100a); "
+        raise RuntimeError("quantized_distillation_b200 needs a CUDA device (H100, sm_90a); "
                            "there is no CPU implementation of the quantization ops in this package")
 
 

@@ -1,5 +1,5 @@
-"""Builds libqd_b200.so (sm_100a) in-tree with nvcc.  Used by
-__graft_entry__.build(); the built .so is git-ignored but travels to the GPU box."""
+"""Builds libqd_b200.so (sm_90a, H100) in-tree with nvcc.  Used by
+__graft_entry__.build(); the built .so is a build product and stays out of git."""
 from __future__ import annotations
 
 import os
@@ -15,14 +15,14 @@ HEADERS.append(os.path.join(ROOT, "include", "qd_b200.h"))
 OUT = os.path.join(HERE, "libqd_b200.so")
 
 # -fmad=false + explicit _rn intrinsics: one IEEE rounding per reference torch op (DESIGN.md)
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-I", os.path.join(ROOT, "include")]
 
 
 def nvcc() -> str:
     exe = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(exe):
-        raise RuntimeError("nvcc not found; the sm_100a extension cannot be built")
+        raise RuntimeError("nvcc not found; the sm_90a extension cannot be built")
     return exe
 
 

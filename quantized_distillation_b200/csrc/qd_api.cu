@@ -5,7 +5,7 @@
 //     L <= 1024                  warp path    (registers, 1 HBM pass)
 //     L <= QD_MAX_STAGED_BUCKET  staged path  (TMA chunk ring in shared memory, 1 HBM pass; CTA size by L)
 //     otherwise                  grid path    (two streaming passes)
-// Thresholds inside these ranges come from profiles/block_path_r2_{variants,small_rows}.md.
+// Thresholds inside these ranges come from tools/block_bench.py (every variant forced through the tuning hook).
 #include <cuda_runtime.h>
 
 #include <cstdarg>
@@ -133,7 +133,7 @@ extern "C" int qd_bucket_geometry(int64_t n, int64_t bucket, int64_t* rows, int6
     return QD_OK;
 }
 
-static constexpr size_t kPointsGradMaxCtas = 148 * 8;
+static constexpr size_t kPointsGradMaxCtas = 132 * 8;  // 8 CTAs per SM of a 132-SM H100 SXM; bigger parts are capped here
 static size_t points_grad_ws_bytes() { return kPointsGradMaxCtas * 256 * sizeof(double); }
 
 extern "C" size_t qd_workspace_bytes(int64_t n, int64_t bucket) {
@@ -170,10 +170,9 @@ static int launch_warp_inst(const Params& P, cudaStream_t s) {
     int64_t cap = (int64_t)di->sms * occ;
     int grid = (int)(need < cap ? need : cap);
     if constexpr (OP == OP_UNIFORM && BWD == (int)BWD_MINMAX) {
-        // r_b accumulation, measured A/B on one box (tools/headline_ab.py, 200 back-to-back launches, 64 Mi floats):
-        // fused forward+backward 173-178 us with one float64 add per element vs 184-192 us with the grouped lane sum;
-        // backward alone 158-167 us vs 139-146 us.  So the variant follows the presence of the q output
-        // (key 3: 1 forces the per-element sum, 0 the grouped one).
+        // r_b accumulation, chosen by A/B (tools/headline_ab.py, 64 Mi floats): the fused forward+backward is faster
+        // with one float64 add per element, the backward alone with the grouped lane sum.  So the variant follows the
+        // presence of the q output (key 3: 1 forces the per-element sum, 0 the grouped one).
         const bool per_element = g_tune[3] >= 0 ? (g_tune[3] == 1) : (P.q != nullptr);
         if (per_element) {
             auto kern_a = warp_rows_kernel<OP, BWD, R, VEC, true>;
@@ -246,10 +245,11 @@ static int launch_staged_inst(const Params& P, cudaStream_t s) {
     return QD_OK;
 }
 
-// CTA size and ring depth by row length, from profiles/block_path_r2_variants.md (tools/block_bench.py on B200,
-// every variant forced through the tuning hook): 64 threads below 2048 floats (a 1280-float row is five full steps of
-// a 64-thread CTA, three ragged ones of a 128-thread CTA: fused min/max 266 -> 219 us), 128 up to 3072, 256 up to
-// 12288, 512 up to 24576, 1024 beyond; two rows in flight per CTA up to 4096 floats, the chunk ring alone above.
+// CTA size and ring depth by row length (tools/block_bench.py, every variant forced through the tuning hook): 64
+// threads below 2048 floats (a 1280-float row is five full steps of a 64-thread CTA, three ragged ones of a 128-thread
+// CTA), 128 up to 3072, 256 up to 12288, 512 up to 24576, 1024 beyond; two rows in flight per CTA up to 3072 floats,
+// the chunk ring alone above (on H100 one row in flight is as fast or faster for every op at 4096 floats, and the
+// min/max backward gains most: fused 459 vs 526 us, alone 371 vs 429 us at 64 Mi floats).
 // g_tune[1] = longest row with two rows in flight per CTA, g_tune[2] = forced CTA size.
 template <int OP, int BWD>
 static int launch_staged(const Params& P, cudaStream_t s) {
@@ -271,11 +271,15 @@ static int launch_staged(const Params& P, cudaStream_t s) {
 
 template <int OP, int BWD>
 static int launch_block(const Params& P, cudaStream_t s) {
-    // the staged ring wins or ties at every row length for the ops it implements (profiles/block_path_r2_variants.md);
+    // the staged ring wins or ties at every row length for the ops it implements (tools/block_bench.py);
     // the ops it does not implement (stats / scale / stochastic) keep the round-1 warp two-pass / whole-row staging
     constexpr bool kStagedOp = (OP == OP_UNIFORM || OP == OP_NONUNIFORM);
     const bool staged_ok = kStagedOp && !P.stochastic;
-    const int64_t warp2_default = !staged_ok ? 2 * kWarpTwoPassMaxRow : 0;
+    // except the min/max backward on rows of 1025 .. 2048 floats, where the warp two-pass variant is faster on H100
+    // (64 Mi floats: fused 460 vs 527 us at 1280 floats, 464 vs 531 us at 2048; backward alone 373 vs 409, 380 vs 407)
+    constexpr bool kMinmax = OP == OP_UNIFORM && BWD == (int)BWD_MINMAX;
+    const bool minmax_warp2 = kMinmax && staged_ok && P.geo.row_len > 1024 && P.geo.row_len <= kWarp2MinmaxMaxRow;
+    const int64_t warp2_default = !staged_ok ? 2 * kWarpTwoPassMaxRow : minmax_warp2 ? kWarp2MinmaxMaxRow : 0;
     const int64_t warp2_max = g_tune[0] >= 0 ? g_tune[0] : warp2_default;
     if (P.geo.row_len <= warp2_max) return launch_block_inst<OP, BWD, false, 32>(P, s);               // warp per row, two passes
     if constexpr (kStagedOp) {
@@ -315,7 +319,7 @@ static bool rows_vectorizable(const Params& P) {
     return ptrs && (P.geo.rows == 1 || (P.geo.row_len % 4) == 0);
 }
 
-// longest row the register-resident warp path takes for (OP, BWD); set from profiles/block_path_r2_small_rows.md
+// longest row the register-resident warp path takes for (OP, BWD); set from tools/block_bench.py --small
 template <int OP, int BWD>
 static constexpr int64_t warp_path_max_row() { return 1024; }
 
@@ -325,8 +329,8 @@ static int run_rows(const Params& P, void* ws, size_t ws_bytes, cudaStream_t s) 
     // longest row of the register-resident warp path (key 4 of the tuning hook moves the border for measurements)
     const int64_t warp_max = (g_tune[4] >= 0 && g_tune[4] <= 1024) ? g_tune[4] : warp_path_max_row<OP, BWD>();
     // ragged rows of 513..1023 floats with the min/max backward: the R = 8 register kernel runs its predicated
-    // (non-FULL) variant at 128 registers there -- 425 us at 768 floats against 249 us on the staged ring
-    // (profiles/block_path_r2_small_rows.md); everything else up to 1024 floats is faster in registers
+    // (non-FULL) variant at 128 registers there and loses to the staged ring (tools/block_bench.py --small);
+    // everything else up to 1024 floats is faster in registers
     const bool ragged_minmax = OP == OP_UNIFORM && BWD == (int)BWD_MINMAX && P.geo.row_len > 512 && P.geo.row_len < 1024 && g_tune[4] < 0;
     if (P.geo.row_len <= warp_max && !ragged_minmax)
         return launch_warp<OP, (OP == OP_NONUNIFORM ? 256 : BWD)>(P, rows_vectorizable(P), s);
@@ -362,7 +366,7 @@ extern "C" int qd_scale_down(const float* x, float* xhat, float* alpha, float* b
 
 // Tiled helper kernels (inv_scale, pack, unpack): one CTA iteration = one contiguous tile of kTileGroups thread-groups,
 // every thread owns kTileU groups of it, 256 groups apart, and issues all kTileU loads before the first use -- 64 B per
-// thread in flight instead of 16 (Little: 148 SMs x 2048 threads x 16 B = 4.8 MB does not cover 6.5 TB/s x ~1 us).
+// thread in flight instead of 16 (Little: 132 SMs x 2048 threads x 16 B = 4.3 MB does not cover 3.35 TB/s x ~1.5 us).
 constexpr int kTileU = 4;
 constexpr int kTileGroups = 256 * kTileU;
 

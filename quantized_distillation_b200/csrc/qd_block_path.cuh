@@ -4,7 +4,7 @@
 // Since round 2 the deterministic uniform op (forward, every backward mode) and the centroid op run on the
 // staged chunk ring; this kernel keeps the ops the ring does not implement -- per-row statistics, x_hat in the
 // padded layout, stochastic rounding -- in two variants (the benchmark hook can still force them for the
-// other ops, which is how profiles/block_path_r2_variants.md was measured):
+// other ops, which is how tools/block_bench.py compares the variants):
 //
 // WARP TWO-PASS (GROUP = 32, rows up to 2 * kWarpTwoPassMaxRow floats): a warp streams its row once for
 // min/max (tagged L2::evict_last) and again (L2 hit) for the element-wise pass; no block barrier anywhere,
@@ -93,6 +93,7 @@ __device__ __forceinline__ double cta_sum(double v, double* scratch) {
 // row, the whole-row staging above that, up to the 49152-float shared-memory limit.
 constexpr int kStagedMaxRow = QD_MAX_STAGED_BUCKET;  // floats; longer rows would use the L2 re-read variant
 constexpr int kWarpTwoPassMaxRow = 2048;  // floats; rows up to here: one WARP per row, two passes (second from L1/L2)
+constexpr int kWarp2MinmaxMaxRow = 2048;  // floats; the min/max backward takes the two-pass variant up to here (qd_api.cu)
 
 // GROUP = 32: a warp owns the row (no block barriers at all, dozens of rows in flight per SM);
 // GROUP = kBlockCtaThreads: the whole CTA owns the row.

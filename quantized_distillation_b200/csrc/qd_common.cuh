@@ -57,16 +57,17 @@ __device__ __forceinline__ float max_nan(float a, float b) {
     asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
     return r;
 }
-// sm_100a single-instruction warp reductions (SASS: CREDUX.MIN/MAX.F32.NAN)
+// Warp-wide NaN-propagating min / max (sm_90a has no float redux.sync): xor butterfly, then lane 0's value is
+// broadcast so that every lane holds the same bits even where the two operands of a step are +0 and -0.
 __device__ __forceinline__ float warp_min(float v) {
-    float r;
-    asm volatile("redux.sync.min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(v), "r"(kFullMask));
-    return r;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = min_nan(v, __shfl_xor_sync(kFullMask, v, o));
+    return __shfl_sync(kFullMask, v, 0);
 }
 __device__ __forceinline__ float warp_max(float v) {
-    float r;
-    asm volatile("redux.sync.max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(v), "r"(kFullMask));
-    return r;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = max_nan(v, __shfl_xor_sync(kFullMask, v, o));
+    return __shfl_sync(kFullMask, v, 0);
 }
 __device__ __forceinline__ int warp_min_int(int v) { return __reduce_min_sync(kFullMask, v); }
 __device__ __forceinline__ float warp_sum(float v) {

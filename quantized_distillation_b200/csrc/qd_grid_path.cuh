@@ -8,7 +8,7 @@
 //                           order (first occurrence wins) -> alpha, beta
 //   3. grid_apply         : element-wise pass.  Chunks are visited in REVERSE
 //                           order so the tail of the tensor, still resident in
-//                           the 126 MB L2 from pass 1, is consumed first.
+//                           the 50 MB L2 from pass 1, is consumed first.
 #pragma once
 #include "qd_block_path.cuh"
 
@@ -16,7 +16,7 @@ namespace qd {
 
 constexpr int kGridCtaThreads = 512;
 constexpr int kGridChunk = 16384;  // elements per CTA work item
-constexpr int64_t kGridKeepBytes = 80ll << 20;  // tail of the tensor pinned in the 126 MB L2 between the two passes
+constexpr int64_t kGridKeepBytes = 32ll << 20;  // tail of the tensor pinned in the 50 MB L2 between the two passes
 
 struct ChunkPartial {
     float mn, mx;

@@ -27,7 +27,7 @@ extern "C" int64_t qd_internal_tuning(int key);
 namespace {
 
 // pipeline depth and chunk size: three slots of 8-16 MiB per buffer sit on the plateau of the tuning
-// sweeps (tools/e2e_variants.py: ~44 GB/s per PCIe direction; slots beyond 2 and chunks beyond 16 MiB change nothing)
+// sweeps (tools/e2e_variants.py: slots beyond 2 and chunks beyond 16 MiB changed nothing)
 constexpr int kMaxSlots = 8;
 constexpr int kSlots = 3;
 constexpr int64_t kChunkElems = 4 << 20;
@@ -103,10 +103,9 @@ int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t 
     const int64_t t_slots = qd_internal_tuning(5), t_chunk = qd_internal_tuning(6), t_path = qd_internal_tuning(7);
     const int n_slots = (t_slots >= 1 && t_slots <= kMaxSlots) ? (int)t_slots : kSlots;
     // Pinned (cudaHostAlloc'd / registered) host buffers are device-addressable under UVA: the kernel can read its
-    // inputs and write its outputs straight over PCIe.  One such launch moves ~40 GB/s each way (the staged pipeline:
-    // ~44 of the 49 GB/s two plain copies reach together) but has no pipeline to fill and drain, so it wins up to
-    // ~8 Mi elements (tools/e2e_variants.py: 53.8 vs 49.4 GB/s at 1 Mi, 69.4 vs 65.6 at 4 Mi, 77.4 vs 80.2 at 16 Mi,
-    // 80.0 vs 88.5 at 64 Mi; mixed forms -- DMA one way, the kernel the other -- lose at every size).
+    // inputs and write its outputs straight over PCIe.  Such a launch moves less per direction than the copy engines
+    // but has no pipeline to fill and drain, so it wins on small tensors; the crossover is set at 8 Mi elements
+    // (tools/e2e_variants.py measures it; mixed forms -- DMA one way, the kernel the other -- lost at every size).
     // key 7: 0 = staged pipeline, 1 = one launch on the host pointers, -1 = this rule.
     auto device_view = [](const void* p) -> void* {
         if (p == nullptr) return nullptr;

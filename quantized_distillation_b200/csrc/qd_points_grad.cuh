@@ -138,8 +138,8 @@ __global__ void __launch_bounds__(kPgThreads) points_grad_partial(const float* _
 }
 
 // one CTA per centroid: 256 threads stride over the CTA partials (a few loads each, all in flight), then a fixed
-// tree (lanes by shuffle, warps in order).  One warp per centroid on ONE CTA made this kernel 6 us (K = 4) to 18 us
-// (K = 16) of serial L2 round trips -- a quarter of the whole op at 64 Mi elements.
+// tree (lanes by shuffle, warps in order).  One warp per centroid on ONE CTA serialised the fold into L2 round trips
+// that took a visible share of the whole op at 64 Mi elements.
 __global__ void __launch_bounds__(256) points_grad_final(const double* __restrict__ partial, int nblocks, int K,
                                                          float* __restrict__ out) {
     __shared__ double s_w[8];

@@ -27,7 +27,7 @@
 
 namespace qd {
 
-constexpr int kTwoStageMaxRow = 4096;  // floats; rows up to here keep two rows in flight per CTA (measured crossover)
+constexpr int kTwoStageMaxRow = 3072;  // floats; rows up to here keep two rows in flight per CTA (measured crossover)
 
 struct StagedScratch {
     float mm[2][2][32];  // [exchange parity][min | max][warp]

@@ -1,6 +1,6 @@
 // qd_torch_fast.cpp -- optional compiled front door of the reference-shaped per-tensor API.
 //
-// The ctypes shim costs ~25 us of host time per call (torch.empty x3, views, ctypes argument marshalling); the
+// The ctypes shim costs tens of microseconds of host time per call (torch.empty x3, views, ctypes argument marshalling); the
 // training loops avoid it with the multi-tensor plans, but code that keeps the reference's per-tensor loop
 // (INTEGRATION.md, level 1) pays it once per tensor per step.  This module does the same work from C++: output
 // allocation through ATen's caching allocator, torch's current stream, ONE call into the C ABI of libqd_b200.so.

@@ -6,8 +6,8 @@
 // (r = 0..R-1), i.e. each load/store instruction of the warp covers 512
 // contiguous bytes (4 full 128-byte lines).  Rows that are not 16-byte aligned
 // (bucket % 4 != 0 or an offset base pointer) use the scalar mapping
-// (r*4+j)*32 + L, still fully coalesced.  Row reductions are single
-// CREDUX.F32 instructions (redux.sync.{min,max}.NaN.f32, sm_100a).
+// (r*4+j)*32 + L, still fully coalesced.  Row reductions are shuffle
+// butterflies of NaN-propagating min / max (warp_min / warp_max, qd_common.cuh).
 //
 // The grid is persistent: min(ceil(rows / warps_per_cta), SMs * resident CTAs)
 // CTAs, each warp walking rows with a grid stride, so consecutive warps stream
@@ -303,8 +303,8 @@ __device__ __forceinline__ void warp_compute_row(const Params& P, const Centroid
                         if (e == imin) gv[4 * r + j] = __fadd_rn(gv[4 * r + j], -rb);
                     }
             }
-            // (patching the two elements in global memory after the row store instead was measured: the dependent
-            // load-after-store stalls the warp, 177 -> 189 us on the headline workload)
+            // (patching the two elements in global memory after the row store instead was measured to be slower: the
+            // dependent load-after-store stalls the warp)
         } else if constexpr (BWD == BWD_TRUNC) {
 #pragma unroll
             for (int i = 0; i < E; ++i) gv[i] = (fabsf(v[i]) > 1.0f) ? 0.f : gv[i];
@@ -388,12 +388,14 @@ template <int OP, int AUX>
 constexpr bool kPrefetchNextRow = (OP != OP_UNIFORM) || (AUX == (int)BWD_OFF);
 
 // minimum resident CTAs per SM the register allocator must allow: 256-element rows (every
-// experiment of the reference) are tuned for 4 x 8 warps per SM (<= 64 registers); the fused
-// min/max kernel gained 3-5 % from the extra occupancy (profiles/sweep_r1_full.md)
-// (measured per kernel: the forward-only and min/max kernels gain, STE / truncated / non-uniform
-// are better with ptxas's own choice, 0 = unconstrained)
+// experiment of the reference) are tuned for 4 x 8 warps per SM (<= 64 registers) in the forward-only
+// kernel; the fused min/max kernel spills at 64 registers on sm_90a and runs 3 % faster at 3 CTAs
+// (<= 80 registers, no spill; one H100 at 400 W, 5 x 200 back-to-back launches, two interleaved rounds:
+// 398-407 -> 385-391 us per launch, identical output bits)
+// (measured per kernel: STE / truncated / non-uniform are better with ptxas's own choice, 0 = unconstrained)
 template <int OP, int AUX, int R>
-constexpr int kMinCtas = (OP == OP_UNIFORM && R == 2 && (AUX == (int)BWD_OFF || AUX == (int)BWD_MINMAX)) ? 4
+constexpr int kMinCtas = (OP == OP_UNIFORM && R == 2 && AUX == (int)BWD_OFF) ? 4
+                         : (OP == OP_UNIFORM && R == 2 && AUX == (int)BWD_MINMAX) ? 3
                          : (OP == OP_UNIFORM && R == 8 && AUX != (int)BWD_OFF) ? 2   // 1024-element rows with a gradient: cap at 128 regs
                                                                                : 0;
 

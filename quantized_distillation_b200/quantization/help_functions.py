@@ -1,4 +1,4 @@
-"""B200 counterpart of the reference's ``quantization/help_functions.py``:
+"""H100 counterpart of the reference's ``quantization/help_functions.py``:
 bucketing view, centroid initialisation, bit allocation and Huffman statistics.
 Only what the quantized-distillation / differentiable-quantization loops and the
 size accounting call is provided (the hyperspherical helpers, :8-65, are unused

@@ -1,8 +1,8 @@
-"""B200 implementation of the reference's ``quantization.quant_functions``.
+"""H100 implementation of the reference's ``quantization.quant_functions``.
 
 Same public names, argument meaning, return values and error behaviour as
 ``quantization/quant_functions.py`` of antspy/quantized_distillation (cited as
-file:line below), but every op is ONE fused sm_100a kernel behind the C ABI of
+file:line below), but every op is ONE fused sm_90a kernel behind the C ABI of
 ``include/qd_b200.h`` instead of a chain of ~12 torch launches (uniform) or a
 device->numpy->device round trip (non-uniform).
 

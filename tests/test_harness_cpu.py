@@ -1,5 +1,6 @@
 """Host-side checks of the training harness (no GPU): model shapes the hot path sees,
 loss formula, schedules, and the N>1 data-parallel plumbing on gloo with world_size 2."""
+import contextlib
 import os
 import socket
 
@@ -148,6 +149,21 @@ def _free_port():
     return port
 
 
+@contextlib.contextmanager
+def _cpu_only_children():
+    """The spawned ranks run the CPU path: started without visible GPUs, none of them picks cuda:<rank>, which a
+    machine with fewer GPUs than ranks does not have (the variable is read when a child initialises CUDA)."""
+    saved = os.environ.get("CUDA_VISIBLE_DEVICES")
+    os.environ["CUDA_VISIBLE_DEVICES"] = ""
+    try:
+        yield
+    finally:
+        if saved is None:
+            del os.environ["CUDA_VISIBLE_DEVICES"]
+        else:
+            os.environ["CUDA_VISIBLE_DEVICES"] = saved
+
+
 def _ddp_worker(rank, world, port, ret):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank))
     from quantized_distillation_b200 import distributed as D
@@ -174,7 +190,8 @@ def test_ddp_replicas_stay_identical_gloo_world2():
     port = _free_port()
     with mp.Manager() as mgr:
         ret = mgr.dict()
-        mp.spawn(_ddp_worker, args=(world, port, ret), nprocs=world, join=True)
+        with _cpu_only_children():
+            mp.spawn(_ddp_worker, args=(world, port, ret), nprocs=world, join=True)
         assert ret[0] is True and ret[1] is True
 
 
@@ -233,7 +250,8 @@ def test_flat_data_parallel_gloo_world2_matches_single_process():
     port = _free_port()
     with mp.Manager() as mgr:
         ret = mgr.dict()
-        mp.spawn(_flat_worker, args=(world, port, ret), nprocs=world, join=True)
+        with _cpu_only_children():
+            mp.spawn(_flat_worker, args=(world, port, ret), nprocs=world, join=True)
         assert ret[0] is True and ret[1] is True
         dp = ret["params"]
     torch.manual_seed(1234)

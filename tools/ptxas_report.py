@@ -52,7 +52,7 @@ def main():
             log = res.stderr
     rows, cur = [], None
     for line in log.splitlines():
-        m = re.search(r"Compiling entry function '([^']+)' for 'sm_100a'", line)
+        m = re.search(r"Compiling entry function '([^']+)' for 'sm_90a'", line)
         if m:
             cur = {"name": m.group(1), "stack": 0, "spill_st": 0, "spill_ld": 0, "regs": 0, "smem": 0, "barriers": 0}
             rows.append(cur)
@@ -72,7 +72,7 @@ def main():
     spilled = [r for r in rows if r["spill_st"] or r["spill_ld"]]
     with open(args.out, "w") as f:
         f.write("Registers / spills / static shared memory per kernel of `libqd_b200.so`, from `nvcc -Xptxas -v` "
-                "(sm_100a, the library's own flags; `tools/ptxas_report.py`, no GPU needed).\n\n")
+                "(sm_90a, the library's own flags; `tools/ptxas_report.py`, no GPU needed).\n\n")
         f.write(f"{len(rows)} kernels; {len(spilled)} with register spills "
                 f"(max {max([r['spill_st'] for r in rows] + [0])} B of spill stores); "
                 f"max registers {max(r['regs'] for r in rows)}.\n\n")

@@ -1,5 +1,5 @@
 """Instruction histogram per kernel of libqd_b200.so (cuobjdump -sass): the static evidence that the
-library is hand-written sm_100a code -- CREDUX (redux.sync float min/max, sm_100a only), UBLKCP / SYNCS
+library is hand-written sm_90a code -- FMNMX.NAN (NaN-propagating float min/max), UBLKCP / SYNCS
 (TMA bulk copies and their mbarriers), SHFL-based table search, 128-bit LDG/STG -- and how large each
 kernel is.  Runs without a GPU.
 
@@ -14,7 +14,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "quantized_distillation_b200", "libqd_b200.so")
-KEYS = ["LDG.E.128", "STG.E.128", "LDG", "STG", "LDS", "STS", "UBLKCP", "SYNCS", "CREDUX", "SHFL", "VOTE", "BAR", "FFMA", "FMUL", "FADD",
+KEYS = ["LDG.E.128", "STG.E.128", "LDG", "STG", "LDS", "STS", "UBLKCP", "SYNCS", "FMNMX", "SHFL", "VOTE", "BAR", "FFMA", "FMUL", "FADD",
         "FSETP", "FSEL", "MUFU", "FRND", "DADD", "F2F", "ATOM", "RED", "CALL", "BRA"]
 
 
@@ -51,8 +51,8 @@ def main():
         wide_st = sum(v for op, v in c.items() if op.startswith("STG") and ".128" in op)
         rows.append((names[k], total, wide_ld, wide_st, [cnt(x) for x in KEYS[2:]]))
     with open(args.out, "w") as f:
-        f.write("SASS instruction histogram of `libqd_b200.so` (static counts, `cuobjdump -sass`, sm_100a).\n"
-                "`CREDUX` = `redux.sync.{min,max}.NaN.f32` (sm_100a), `UBLKCP`/`SYNCS` = TMA bulk copy + mbarrier, "
+        f.write("SASS instruction histogram of `libqd_b200.so` (static counts, `cuobjdump -sass`, sm_90a).\n"
+                "`FMNMX` = `{min,max}.NaN.f32`, `UBLKCP`/`SYNCS` = TMA bulk copy + mbarrier, "
                 "`SHFL` in the centroid kernels = lane-table search.\n\n")
         f.write("| kernel | instr | LDG.128 | STG.128 | " + " | ".join(KEYS[2:]) + " |\n|---|---|---|---|" + "---|" * len(KEYS[2:]) + "\n")
         for name, total, wl, ws, cs in rows:
@@ -62,7 +62,7 @@ def main():
         for c in kernels.values():
             tot.update(c)
         f.write(f"\n{len(kernels)} kernels, {sum(tot.values())} instructions; library-wide: "
-                + ", ".join(f"{k} {sum(v for op, v in tot.items() if op == k or op.startswith(k + '.'))}" for k in ("CREDUX", "UBLKCP", "SYNCS", "SHFL", "MUFU")) + ".\n")
+                + ", ".join(f"{k} {sum(v for op, v in tot.items() if op == k or op.startswith(k + '.'))}" for k in ("FMNMX", "UBLKCP", "SYNCS", "SHFL", "MUFU")) + ".\n")
     print("wrote", args.out, len(kernels), "kernels")
 
 

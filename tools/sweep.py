@@ -1,12 +1,13 @@
 """Per-op / per-size throughput table (BASELINE.json config 5: synthetic weight-tensor
-sweep, uniform + non-uniform fwd/bwd, GB/s vs the B200 HBM roofline).
+sweep, uniform + non-uniform fwd/bwd, GB/s vs the H100 HBM roofline).
 
     python -m tools.sweep [--out gpurun_out/sweep.json] [--max-log2 28]
 
 Each row: CUDA-event time per launch (inputs resident in HBM, 3 warm-ups, buffers
 rotated so that consecutive launches never touch the same cache lines when the
 tensor is smaller than L2), algorithmic bytes (SURVEY.md section 8d), GB/s and the
-fraction of the measured HBM copy peak."""
+fraction of the HBM peak (measured copy peak when MEASURED_PEAKS.json is present,
+the H100 SXM data sheet's 3.35 TB/s otherwise)."""
 from __future__ import annotations
 
 import argparse
@@ -24,13 +25,13 @@ def run(dev=None, out_path=None, max_log2=28, min_log2=10, only=None):
     from quantized_distillation_b200 import _native as N
     dev = dev or torch.device("cuda", torch.cuda.current_device())
     lib = N.lib()
-    peak = 6650.0
+    peak = 3350.0
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         peak = float(json.load(open(pk))["hbm_gbs"])
     sp = N.stream_ptr(dev)
     rows = []
-    L2_BYTES = 126 << 20
+    L2_BYTES = 50 << 20
 
     def timeit(fn, nbuf, iters):
         for i in range(3):
