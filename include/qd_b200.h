@@ -166,6 +166,42 @@ int qd_unpack_dequant_nonuniform(const uint8_t* packed, int bits, const float* p
                                  const float* alpha, const float* beta, float* q, int64_t n, int64_t bucket,
                                  qd_stream_t stream);
 
+/* ---- next row f2: Huffman-coded storage (the model helpers/functions.py:226-262 only sizes) ----------
+ * Canonical code over uint8 symbols, codes of 1..QD_HUFFMAN_MAX_LENGTH bits (built on the host: codec.py).
+ * Stream: a tensor's symbols are cut into chunks of QD_HUFFMAN_CHUNK; each chunk's codes are written MSB-first
+ * into 32-bit words (stored little-endian), starting on a fresh word; chunk_offsets[c] (uint32, one per chunk)
+ * is the word at which chunk c starts.  A single-symbol code has length 0: no stream, every element is that
+ * symbol.  The table is DEVICE memory in this layout (13328 bytes): */
+#define QD_HUFFMAN_CHUNK 1024
+#define QD_HUFFMAN_MAX_LENGTH 57 /* a 64-bit window at any bit of a word, minus the in-word offset slack */
+#define QD_HUFFMAN_LUT_BITS 11
+typedef struct {
+    uint64_t code[256];    /* codeword of each symbol, right-aligned */
+    uint64_t first[64];    /* first codeword of length l, right-aligned (canonical order) */
+    uint32_t length[256];  /* code length of each symbol, 0 when absent */
+    uint32_t count[64];    /* codewords of length l */
+    uint32_t index[64];    /* position in symbols[] of the first codeword of length l */
+    uint32_t symbols[256]; /* symbols in canonical order (length, then symbol) */
+    uint32_t lut[1 << QD_HUFFMAN_LUT_BITS]; /* next 11 stream bits -> (length << 16) | symbol; length 0: longer code */
+    uint32_t max_length;   /* longest code; 0: single-symbol code, every element is symbols[0] */
+    uint32_t reserved[3];
+} qd_huffman_table;
+/* Encoder: pass 1 (per-chunk word counts), a one-CTA exclusive scan into chunk_offsets[ceil(n/C)] and
+ * *total_words (device uint64), pass 2 (one warp per chunk) writes words_out.  The caller allocates
+ * words_capacity words from its own bound (code bits of the tensor's histogram / 32 + one word per chunk) and
+ * trims to *total_words after a synchronise; chunks that would end beyond the capacity are not written. */
+int qd_huffman_encode(const uint8_t* idx_u8, int64_t n, const qd_huffman_table* table, uint32_t* words_out,
+                      int64_t words_capacity, uint32_t* chunk_offsets, uint64_t* total_words, qd_stream_t stream);
+/* Decoder fused with the dequantization of qd_unpack_dequant_*: q is bit-identical to the output of the op that
+ * produced the levels.  words may be NULL when num_words is 0 (single-symbol code). */
+int qd_huffman_decode_dequant_uniform(const uint32_t* words, int64_t num_words, const uint32_t* chunk_offsets,
+                                      const qd_huffman_table* table, const float* alpha, const float* beta, float* q,
+                                      int64_t n, int64_t bucket, int levels, qd_stream_t stream);
+int qd_huffman_decode_dequant_nonuniform(const uint32_t* words, int64_t num_words, const uint32_t* chunk_offsets,
+                                         const qd_huffman_table* table, const float* points, int num_points,
+                                         const float* alpha, const float* beta, float* q, int64_t n, int64_t bucket,
+                                         qd_stream_t stream);
+
 /* ---- next row f1: one launch over every parameter tensor of a model ------
  * (replaces the per-tensor loop of cnn_models/conv_forward_model.py:236-247).
  * A plan owns a device-side table of (src, dst, n, levels); pointers must stay

@@ -7,9 +7,12 @@ bit-packed codes (1/2/4/8 bits) + (alpha, beta) per bucket, produced and decoded
 and decoding reproduces the fake-quantized float tensor bit for bit."""
 from __future__ import annotations
 
+import json
 import math
-from dataclasses import dataclass
+import struct
+from dataclasses import dataclass, field
 
+import numpy as np
 import torch
 
 from . import _native as N
@@ -101,6 +104,435 @@ def decode(pt: PackedTensor) -> torch.Tensor:
         N.check(N.lib().qd_unpack_dequant_nonuniform(N.ptr(pt.packed), pt.bits, N.ptr(pt.points), pt.points.numel(),
                                                      N.ptr(pt.alpha), N.ptr(pt.beta), N.ptr(out), n, b, sp))
     return out.view(pt.shape)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Huffman-coded model container.  The code is the one the size accounting uses (huffman_code_of_histogram over
+# the level histogram of every quantized tensor), made canonical; the stream and table layout are declared in
+# include/qd_b200.h and produced / consumed by csrc/qd_huffman.cuh.
+HUFFMAN_CHUNK = 1024            # symbols per independently decodable chunk (QD_HUFFMAN_CHUNK)
+HUFFMAN_MAX_LENGTH = 57         # QD_HUFFMAN_MAX_LENGTH
+HUFFMAN_LUT_BITS = 11           # QD_HUFFMAN_LUT_BITS
+HUFFMAN_TABLE_BYTES = 13328     # sizeof(qd_huffman_table)
+FILE_MAGIC = b"QDHUFF\x00\x00"
+FILE_VERSION = 1
+_PREFIX = struct.Struct("<8sIIQ")   # magic, version, reserved (0), JSON header length
+_ALIGN = 16
+
+
+def huffman_code_lengths(counts) -> dict:
+    """{symbol: code length} of the reference's Huffman code for a level histogram (counts[symbol]).  A
+    single-symbol histogram gives length 0.  Codes longer than HUFFMAN_MAX_LENGTH bits raise ValueError."""
+    _, code = qhf.huffman_code_of_histogram(np.asarray(counts, dtype=np.int64))
+    lengths = {int(sym): len(bits) for sym, bits in code}
+    check_code_lengths(lengths)
+    return lengths
+
+
+def check_code_lengths(lengths: dict) -> None:
+    """Raises ValueError unless `lengths` is a complete prefix code the stream format can carry."""
+    if not lengths:
+        raise ValueError("empty code")
+    if any(not (0 <= int(s) < 256) for s in lengths):
+        raise ValueError("symbols must be in [0, 256)")
+    if len(lengths) == 1:
+        if next(iter(lengths.values())) != 0:
+            raise ValueError("a single-symbol code has length 0")
+        return
+    longest = max(lengths.values())
+    if longest > HUFFMAN_MAX_LENGTH:
+        raise ValueError(f"longest Huffman code is {longest} bits; the stream format supports at most {HUFFMAN_MAX_LENGTH}")
+    if min(lengths.values()) < 1:
+        raise ValueError("code lengths must be >= 1 when there are several symbols")
+    if sum(1 << (longest - l) for l in lengths.values()) != 1 << longest:
+        raise ValueError("code lengths violate Kraft equality: not a complete prefix code")
+
+
+def canonical_codes(lengths: dict) -> dict:
+    """{symbol: codeword}: codewords assigned in (length, symbol) order, each the previous one plus one, shifted
+    to its length.  Lengths (hence the size) are those of the input."""
+    codes, code, prev = {}, 0, None
+    for sym, l in sorted(lengths.items(), key=lambda kv: (kv[1], kv[0])):
+        if prev is not None:
+            code = (code + 1) << (l - prev)
+        codes[sym] = code
+        prev = l
+    return codes
+
+
+def huffman_table(lengths: dict) -> np.ndarray:
+    """The qd_huffman_table bytes (include/qd_b200.h) of a canonical code."""
+    check_code_lengths(lengths)
+    code = np.zeros(256, "<u8")
+    first = np.zeros(64, "<u8")
+    length = np.zeros(256, "<u4")
+    count = np.zeros(64, "<u4")
+    index = np.zeros(64, "<u4")
+    symbols = np.zeros(256, "<u4")
+    lut = np.zeros(1 << HUFFMAN_LUT_BITS, "<u4")
+    codes = canonical_codes(lengths)
+    for pos, (sym, l) in enumerate(sorted(lengths.items(), key=lambda kv: (kv[1], kv[0]))):
+        code[sym], length[sym], symbols[pos] = codes[sym], l, sym
+        if count[l] == 0:
+            first[l], index[l] = codes[sym], pos
+        count[l] += 1
+        if 1 <= l <= HUFFMAN_LUT_BITS:
+            lo = codes[sym] << (HUFFMAN_LUT_BITS - l)
+            lut[lo:lo + (1 << (HUFFMAN_LUT_BITS - l))] = (l << 16) | sym
+    tail = np.array([max(lengths.values()), 0, 0, 0], "<u4")
+    out = np.concatenate([a.view(np.uint8) for a in (code, first, length, count, index, symbols, lut, tail)])
+    assert out.nbytes == HUFFMAN_TABLE_BYTES
+    return out
+
+
+@dataclass
+class HuffmanTensor:
+    """One parameter of a CompressedModel: a Huffman stream + (alpha, beta) per bucket, or float32 as is."""
+    name: str
+    shape: tuple
+    words: torch.Tensor = None          # int32 storage of the uint32 stream words
+    chunk_offsets: torch.Tensor = None  # int32 storage of uint32[ceil(n / HUFFMAN_CHUNK)]
+    alpha: torch.Tensor = None          # float32[rows]
+    beta: torch.Tensor = None
+    points: torch.Tensor = None         # non-uniform: this tensor's centroids
+    raw: torch.Tensor = None            # unquantized tensor (float32)
+    code_bits: int = 0                  # bits of the codes alone (no chunk padding)
+
+    @property
+    def numel(self) -> int:
+        return int(math.prod(self.shape))
+
+    @property
+    def quantized(self) -> bool:
+        return self.raw is None
+
+
+@dataclass
+class CompressedModel:
+    """A model whose quantized parameters are Huffman-coded (compress_model, load_compressed)."""
+    kind: str                       # "uniform" | "nonuniform"
+    levels: object                  # uniform: s; non-uniform: None
+    bucket_size: object
+    code_lengths: dict              # symbol -> code length (canonical code)
+    tensors: list
+    chunk: int = HUFFMAN_CHUNK
+    _tables: dict = field(default_factory=dict, repr=False)
+
+    def table(self, device) -> torch.Tensor:
+        key = str(device)
+        if key not in self._tables:
+            self._tables[key] = torch.from_numpy(huffman_table(self.code_lengths)).to(device)
+        return self._tables[key]
+
+    def size_breakdown(self) -> dict:
+        """Bytes of the saved file by what they hold.  code_bits / 8 + scale_bytes + unquantized_bytes is what
+        get_size_quantized_model accounts for; the rest is the price of the format."""
+        header, sections, data_bytes = _layout(self)
+        q = [t for t in self.tensors if t.quantized]
+        code_bits = sum(t.code_bits for t in q)
+        section_bytes = sum(nb for _, _, nb, _ in sections)
+        return {
+            "code_bits": code_bits,
+            "padding_bits": sum(t.words.numel() for t in q) * 32 - code_bits,
+            "chunk_index_bytes": sum(t.chunk_offsets.numel() * 4 for t in q),
+            "scale_bytes": sum((t.alpha.numel() + t.beta.numel()) * 4 for t in q),
+            "unquantized_bytes": sum(t.raw.numel() * 4 for t in self.tensors if not t.quantized),
+            "header_bytes": _PREFIX.size + len(header),
+            "alignment_bytes": _align(_PREFIX.size + len(header)) - _PREFIX.size - len(header) + data_bytes - section_bytes,
+            "file_bytes": _align(_PREFIX.size + len(header)) + data_bytes,
+        }
+
+
+def _align(x: int) -> int:
+    return (x + _ALIGN - 1) // _ALIGN * _ALIGN
+
+
+def _sections_of(t: HuffmanTensor):
+    if not t.quantized:
+        return [("raw", t.raw)]
+    return [("words", t.words), ("chunk_offsets", t.chunk_offsets), ("alpha", t.alpha), ("beta", t.beta)]
+
+
+def _layout(cm: CompressedModel):
+    """(JSON header bytes, [(tensor index, section name, nbytes, offset)], data bytes); offsets are relative to
+    the first 16-byte boundary after the header."""
+    sections, entries, off = [], [], 0
+    for i, t in enumerate(cm.tensors):
+        e = {"name": t.name, "shape": list(t.shape), "dtype": "float32", "quantized": t.quantized, "sections": {}}
+        if t.quantized:
+            e["code_bits"] = int(t.code_bits)
+            if t.points is not None:
+                e["points"] = [float(v) for v in t.points.detach().cpu().numpy().astype(np.float32)]
+        for name, tensor in _sections_of(t):
+            nb = tensor.numel() * 4
+            e["sections"][name] = [off, nb]
+            sections.append((i, name, nb, off))
+            off = _align(off + nb)
+        entries.append(e)
+    header = {"chunk": cm.chunk, "kind": cm.kind, "levels": cm.levels, "bucket": cm.bucket_size,
+              "code": [[int(s), int(l)] for s, l in sorted(cm.code_lengths.items())], "tensors": entries, "data_bytes": off}
+    return json.dumps(header, separators=(",", ":")).encode("utf-8"), sections, off
+
+
+def _selected(named, quantize_first_and_last_layer):
+    """Indices of the quantized parameters: all, or all but the first and the last, exactly as
+    get_size_quantized_model selects them."""
+    return set(range(len(named))) if quantize_first_and_last_layer is True else set(range(1, len(named) - 1))
+
+
+def compress_model(model, numBits=None, bucket_size=256, quantize_first_and_last_layer=True, *, points=None,
+                   rule="nearest") -> CompressedModel:
+    """Huffman-codes a model's quantized parameters.  Uniform: ``numBits`` (s = 2**numBits levels,
+    uniformQuantization).  Non-uniform: ``points`` -- one ascending list of centroids for every tensor, or one
+    list per quantized tensor (the differentiable-quantization output) -- with nonUniformQuantization's
+    ``rule``.  One level histogram over all quantized tensors gives the code, so the stored code bits equal
+    get_huffman_encoding_mean_bit_length x the number of quantized weights."""
+    N.require_cuda()
+    if (numBits is None) == (points is None):
+        raise ValueError("give numBits (uniform) or points (non-uniform), not both")
+    named = list(model.named_parameters())
+    sel = _selected(named, quantize_first_and_last_layer)
+    order = [i for i in range(len(named)) if i in sel]
+    uniform = points is None
+    if uniform:
+        s = 2 ** int(numBits)
+        if not 2 <= s <= 256:
+            raise ValueError("the Huffman codec stores uint8 levels: numBits must be in [1, 8]")
+        bins = s
+    else:
+        per_tensor = len(points) > 0 and (torch.is_tensor(points[0]) or isinstance(points[0], (list, tuple, np.ndarray)))
+        pts_list = list(points) if per_tensor else [points] * len(order)
+        if len(pts_list) != len(order):
+            raise ValueError(f"{len(pts_list)} point lists for {len(order)} quantized tensors")
+        bins = 256
+    dev = next((p.device for _, p in named if p.is_cuda), torch.device("cuda", torch.cuda.current_device()))
+    b = 0 if bucket_size is None else int(bucket_size)
+    sp = N.stream_ptr(dev)
+    counts = torch.zeros(len(order), 256, dtype=torch.int64, device=dev)
+    tensors, idxs = [], []
+    with torch.cuda.device(dev):
+        for i, (name, p) in enumerate(named):
+            if i not in sel:
+                tensors.append(HuffmanTensor(name, tuple(p.shape), raw=p.detach().to(dev, torch.float32).contiguous().view(-1).clone()))
+                continue
+            k = len(idxs)
+            x = p.detach().to(dev, torch.float32).contiguous().view(-1)
+            n = x.numel()
+            rows = _rows(n, bucket_size)
+            alpha = torch.empty(rows, device=dev)
+            beta = torch.empty(rows, device=dev)
+            idx = torch.empty(n, dtype=torch.uint8, device=dev)
+            ws = N.workspace(n, b, dev)
+            pts = None
+            if uniform:
+                N.check(N.lib().qd_uniform_fwd(N.ptr(x), None, N.ptr(idx), N.ptr(alpha), N.ptr(beta), None, None, n, b, s, None, 0.0,
+                                               0, 0, 0, N.ptr(ws), ws.numel(), sp))
+            else:
+                pts = torch.as_tensor(pts_list[k], dtype=torch.float32).detach().to(dev).contiguous().view(-1)
+                N.check(N.lib().qd_nonuniform_fwd(N.ptr(x), N.ptr(pts), pts.numel(), N.RULE_MIDPOINT if rule == "midpoint" else N.RULE_NEAREST,
+                                                  None, N.ptr(idx), None, N.ptr(alpha), N.ptr(beta), n, b, None, 0.0, N.ptr(ws), ws.numel(), sp))
+            N.check(N.lib().qd_index_histogram(N.ptr(idx), n, bins, N.ptr(counts[k]), sp))
+            idxs.append(idx)
+            tensors.append(HuffmanTensor(name, tuple(p.shape), alpha=alpha, beta=beta, points=pts))
+        if not idxs:
+            raise ValueError("no parameter is selected for quantization")
+        lengths = huffman_code_lengths(counts.sum(0).cpu().numpy())
+        cm = CompressedModel("uniform" if uniform else "nonuniform", s if uniform else None, bucket_size, lengths, tensors)
+        table = cm.table(dev)
+        len_vec = torch.zeros(256, dtype=torch.int64)
+        for sym, l in lengths.items():
+            len_vec[sym] = l
+        code_bits = (counts.cpu() * len_vec).sum(1).tolist()
+        quantized = [t for t in tensors if t.quantized]
+        totals, bufs = torch.zeros(len(idxs), dtype=torch.int64, device=dev), []
+        for k, (t, idx) in enumerate(zip(quantized, idxs)):
+            n = idx.numel()
+            chunks = -(-n // HUFFMAN_CHUNK)
+            capacity = -(-int(code_bits[k]) // 32) + chunks
+            if capacity - chunks > 1 << 32:
+                raise ValueError(f"{t.name}: its Huffman stream would exceed 2^32 words")
+            capacity = min(capacity, 1 << 32)
+            words = torch.empty(max(capacity, 1), dtype=torch.int32, device=dev)
+            offs = torch.empty(chunks, dtype=torch.int32, device=dev)
+            N.check(N.lib().qd_huffman_encode(N.ptr(idx), n, N.ptr(table), N.ptr(words), capacity, N.ptr(offs), N.ptr(totals[k:k + 1]), sp))
+            t.chunk_offsets, t.code_bits = offs, int(code_bits[k])
+            bufs.append((words, capacity))
+        for (t, (words, capacity)), total in zip(zip(quantized, bufs), totals.cpu().tolist()):
+            if total > capacity:
+                raise ValueError(f"{t.name}: its Huffman stream would exceed 2^32 words")
+            t.words = words[:total]
+    return cm
+
+
+def _device_of(cm: CompressedModel, device=None):
+    N.require_cuda()
+    if device is not None:
+        return torch.device(device)
+    for t in cm.tensors:
+        for x in (t.words, t.raw):
+            if x is not None and x.is_cuda:
+                return x.device
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def decompress_tensor(cm: CompressedModel, which, out: torch.Tensor = None, device=None) -> torch.Tensor:
+    """Decodes one tensor (index or name) of a CompressedModel to float32 on the GPU: the fake-quantized tensor
+    bit for bit, or the stored tensor when it was kept unquantized.  ``out``: contiguous float32 CUDA tensor of
+    the same number of elements to decode into."""
+    t = cm.tensors[which] if isinstance(which, int) else next(x for x in cm.tensors if x.name == which)
+    dev = out.device if out is not None else _device_of(cm, device)
+    if out is None:
+        out = torch.empty(t.shape, dtype=torch.float32, device=dev)
+    if out.dtype != torch.float32 or not out.is_cuda or not out.is_contiguous() or out.numel() != t.numel:
+        raise ValueError("out must be a contiguous float32 CUDA tensor with as many elements as the stored one")
+    with torch.cuda.device(dev):
+        if not t.quantized:
+            out.view(-1).copy_(t.raw.view(-1))
+            return out
+        words, offs = t.words.to(dev), t.chunk_offsets.to(dev)
+        alpha, beta = t.alpha.to(dev), t.beta.to(dev)
+        b = 0 if cm.bucket_size is None else int(cm.bucket_size)
+        sp = N.stream_ptr(dev)
+        args = (N.ptr(words) if words.numel() else None, words.numel(), N.ptr(offs), N.ptr(cm.table(dev)))
+        if cm.kind == "uniform":
+            N.check(N.lib().qd_huffman_decode_dequant_uniform(*args, N.ptr(alpha), N.ptr(beta), N.ptr(out), t.numel, b, int(cm.levels), sp))
+        else:
+            pts = t.points.to(dev)
+            N.check(N.lib().qd_huffman_decode_dequant_nonuniform(*args, N.ptr(pts), pts.numel(), N.ptr(alpha), N.ptr(beta), N.ptr(out),
+                                                                 t.numel, b, sp))
+    return out
+
+
+def decompress_(cm: CompressedModel, model) -> None:
+    """Writes every parameter of ``model`` in place from ``cm`` (existing parameter handles stay valid)."""
+    named = list(model.named_parameters())
+    if len(named) != len(cm.tensors):
+        raise ValueError(f"model has {len(named)} parameters, the compressed model {len(cm.tensors)}")
+    for (name, p), t in zip(named, cm.tensors):
+        if tuple(p.shape) != tuple(t.shape):
+            raise ValueError(f"{name}: shape {tuple(p.shape)} != stored {tuple(t.shape)} ({t.name})")
+    with torch.no_grad():
+        for k, (_, p) in enumerate(named):
+            d = p.data
+            if d.is_cuda and d.dtype == torch.float32 and d.is_contiguous():
+                decompress_tensor(cm, k, out=d)
+            else:
+                d.copy_(decompress_tensor(cm, k, device=d.device if d.is_cuda else None))
+
+
+def save_compressed(cm: CompressedModel, path) -> int:
+    """Writes the container: magic, version, JSON header, 16-byte-aligned little-endian sections.  Returns the
+    file size in bytes."""
+    header, sections, data_bytes = _layout(cm)
+    start = _align(_PREFIX.size + len(header))
+    buf = bytearray(start + data_bytes)
+    buf[:_PREFIX.size] = _PREFIX.pack(FILE_MAGIC, FILE_VERSION, 0, len(header))
+    buf[_PREFIX.size:_PREFIX.size + len(header)] = header
+    for i, name, nb, off in sections:
+        tensor = dict(_sections_of(cm.tensors[i]))[name]
+        buf[start + off:start + off + nb] = tensor.detach().contiguous().cpu().numpy().astype("<i4" if tensor.dtype == torch.int32 else "<f4",
+                                                                                            copy=False).tobytes()
+    with open(path, "wb") as f:
+        f.write(buf)
+    return len(buf)
+
+
+def _bad(msg):
+    raise ValueError(f"not a valid Huffman-coded model file: {msg}")
+
+
+def load_compressed(path, device=None) -> CompressedModel:
+    """Reads and validates a file written by save_compressed.  device=None keeps every section in host memory
+    (reading and validating needs no GPU); decoding then moves them to the GPU."""
+    with open(path, "rb") as f:
+        buf = f.read()
+    if len(buf) < _PREFIX.size:
+        _bad("shorter than its prefix")
+    magic, version, _, hlen = _PREFIX.unpack_from(buf)
+    if magic != FILE_MAGIC:
+        _bad("bad magic")
+    if version != FILE_VERSION:
+        _bad(f"format version {version}, this reader knows {FILE_VERSION}")
+    if _PREFIX.size + hlen > len(buf):
+        _bad("header runs past the end of the file")
+    try:
+        h = json.loads(buf[_PREFIX.size:_PREFIX.size + hlen].decode("utf-8"))
+        kind, levels, bucket, chunk = h["kind"], h["levels"], h["bucket"], h["chunk"]
+        code = {int(s): int(l) for s, l in h["code"]}
+        entries, data_bytes = h["tensors"], int(h["data_bytes"])
+    except (ValueError, KeyError, TypeError) as e:
+        _bad(f"unreadable header ({e})")
+    start = _align(_PREFIX.size + hlen)
+    if start + data_bytes != len(buf):
+        _bad(f"{len(buf)} bytes, the header describes {start + data_bytes}")
+    if chunk != HUFFMAN_CHUNK:
+        _bad(f"chunk of {chunk} symbols, this reader decodes {HUFFMAN_CHUNK}")
+    if kind not in ("uniform", "nonuniform"):
+        _bad(f"unknown kind {kind!r}")
+    if kind == "uniform" and not (isinstance(levels, int) and 2 <= levels <= 256):
+        _bad("uniform levels must be in [2, 256]")
+    if bucket is not None and not (isinstance(bucket, int) and bucket > 0):
+        _bad("bucket must be a positive integer or null")
+    if len(code) != len(h["code"]):
+        _bad("a symbol appears twice in the code")
+    try:
+        check_code_lengths(code)
+    except ValueError as e:
+        _bad(str(e))
+    if kind == "uniform" and max(code) >= levels:
+        _bad("a code symbol is not a level")
+
+    def section(e, name, dtype, count):
+        try:
+            off, nb = (int(v) for v in e["sections"][name])
+        except (KeyError, TypeError, ValueError):
+            _bad(f"{e.get('name')}: section {name} missing")
+        if off < 0 or off % _ALIGN or nb != count * 4 or off + nb > data_bytes:
+            _bad(f"{e.get('name')}: section {name} out of range")
+        return torch.from_numpy(np.frombuffer(buf, dtype=dtype, count=count, offset=start + off).copy())
+
+    tensors = []
+    for e in entries:
+        try:
+            name, shape, quantized = str(e["name"]), tuple(int(d) for d in e["shape"]), bool(e["quantized"])
+        except (KeyError, TypeError, ValueError):
+            _bad("tensor entry without name / shape / quantized")
+        if e.get("dtype") != "float32" or any(d < 0 for d in shape):
+            _bad(f"{name}: bad dtype or shape")
+        n = int(math.prod(shape))
+        if not quantized:
+            tensors.append(HuffmanTensor(name, shape, raw=section(e, "raw", "<f4", n)))
+            continue
+        if n == 0:
+            _bad(f"{name}: empty quantized tensor")
+        chunks = -(-n // HUFFMAN_CHUNK)
+        rows = _rows(n, bucket)
+        words_nb = e.get("sections", {}).get("words", [0, -1])[1]
+        if not isinstance(words_nb, int) or words_nb < 0 or words_nb % 4:
+            _bad(f"{name}: section words out of range")
+        words = section(e, "words", "<i4", words_nb // 4)
+        offs = section(e, "chunk_offsets", "<i4", chunks)
+        o = offs.numpy().view(np.uint32).astype(np.int64)
+        if o[0] != 0 or np.any(np.diff(o) < 0) or o[-1] > words.numel():
+            _bad(f"{name}: chunk offsets out of range")
+        pts = None
+        if kind == "nonuniform":
+            try:
+                pts = torch.tensor([float(v) for v in e["points"]], dtype=torch.float32)
+            except (KeyError, TypeError, ValueError):
+                _bad(f"{name}: non-uniform tensor without points")
+            # the code is model-wide: a tensor with fewer points than another never emits the higher symbols
+            if not 1 <= pts.numel() <= 256:
+                _bad(f"{name}: {pts.numel()} points, expected 1 to 256")
+        tensors.append(HuffmanTensor(name, shape, words=words, chunk_offsets=offs,
+                                     alpha=section(e, "alpha", "<f4", rows), beta=section(e, "beta", "<f4", rows), points=pts,
+                                     code_bits=int(e.get("code_bits", 0))))
+    if device is not None:                       # everything is validated before anything reaches the GPU
+        for t in tensors:
+            for f_ in ("words", "chunk_offsets", "alpha", "beta", "points", "raw"):
+                if getattr(t, f_) is not None:
+                    setattr(t, f_, getattr(t, f_).to(device))
+    return CompressedModel(kind, levels, bucket, code, tensors)
 
 
 def get_size_reduction(effective_number_bits, bucket_size=256, full_precision_bits=32):

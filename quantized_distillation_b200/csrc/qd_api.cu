@@ -19,6 +19,7 @@
 #include "qd_abs_path.cuh"
 #include "qd_block_path.cuh"
 #include "qd_grid_path.cuh"
+#include "qd_huffman.cuh"
 #include "qd_plan.cuh"
 #include "qd_points_grad.cuh"
 #include "qd_select.cuh"
@@ -972,6 +973,73 @@ extern "C" int qd_unpack_dequant_nonuniform(const uint8_t* packed, int bits, con
     else if (bits == 4) unpack_dequant_kernel<false, 4><<<grid, 256, 0, st>>>(packed, points, num_points, alpha, beta, q, geo, 0.f);
     else if (bits == 2) unpack_dequant_kernel<false, 2><<<grid, 256, 0, st>>>(packed, points, num_points, alpha, beta, q, geo, 0.f);
     else unpack_dequant_kernel<false, 1><<<grid, 256, 0, st>>>(packed, points, num_points, alpha, beta, q, geo, 0.f);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+// ------------------------------------------------------------------ f2: Huffman-coded storage (qd_huffman.cuh)
+extern "C" int qd_huffman_encode(const uint8_t* idx_u8, int64_t n, const qd_huffman_table* table, uint32_t* words_out,
+                                 int64_t words_capacity, uint32_t* chunk_offsets, uint64_t* total_words, qd_stream_t stream) {
+    if (idx_u8 == nullptr || table == nullptr || chunk_offsets == nullptr || total_words == nullptr || n <= 0)
+        return fail(QD_ERR_INVALID_ARG, "NULL argument or n <= 0");
+    if (words_capacity < 0 || (words_capacity > 0 && words_out == nullptr)) return fail(QD_ERR_INVALID_ARG, "bad words_out / capacity");
+    DevInfo* di;
+    int rc = dev_info(&di);
+    if (rc) return rc;
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const int64_t chunks = (n + kHuffChunk - 1) / kHuffChunk;
+    const int64_t cap = (int64_t)di->sms * 8;
+    const int64_t need1 = (chunks + 7) / 8;
+    huff_chunk_words_kernel<<<(int)(need1 < cap ? need1 : cap), 256, 0, s>>>(idx_u8, n, table, chunk_offsets, chunks);
+    huff_scan_kernel<<<1, 1024, 0, s>>>(chunk_offsets, chunks, reinterpret_cast<unsigned long long*>(total_words));
+    const int64_t need2 = (chunks + kHuffEncWarps - 1) / kHuffEncWarps;
+    if (words_capacity > 0)
+        huff_encode_kernel<<<(int)(need2 < cap ? need2 : cap), kHuffEncWarps * 32, 0, s>>>(
+            idx_u8, n, table, chunk_offsets, reinterpret_cast<const unsigned long long*>(total_words), chunks, words_out, words_capacity);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+static int huff_decode_common(const uint32_t* words, int64_t num_words, const uint32_t* chunk_offsets, const qd_huffman_table* table,
+                              const float* alpha, const float* beta, float* q, int64_t n, int64_t bucket, Geometry* geo, int* grid) {
+    if (chunk_offsets == nullptr || table == nullptr || alpha == nullptr || beta == nullptr || q == nullptr)
+        return fail(QD_ERR_INVALID_ARG, "NULL argument");
+    if (num_words < 0 || (num_words > 0 && words == nullptr)) return fail(QD_ERR_INVALID_ARG, "bad words / num_words");
+    if (geometry_of(n, bucket, geo)) return fail(QD_ERR_INVALID_ARG, "bad geometry");
+    DevInfo* di;
+    int rc = dev_info(&di);
+    if (rc) return rc;
+    const int64_t need = ((n + kHuffChunk - 1) / kHuffChunk + kHuffDecThreads - 1) / kHuffDecThreads;
+    const int64_t cap = (int64_t)di->sms * 16;
+    *grid = (int)(need < cap ? need : cap);
+    return QD_OK;
+}
+
+extern "C" int qd_huffman_decode_dequant_uniform(const uint32_t* words, int64_t num_words, const uint32_t* chunk_offsets,
+                                                 const qd_huffman_table* table, const float* alpha, const float* beta, float* q,
+                                                 int64_t n, int64_t bucket, int levels, qd_stream_t stream) {
+    Geometry geo;
+    int grid = 0;
+    if (levels < 2 || levels > 256) return fail(QD_ERR_INVALID_ARG, "levels must be in [2, 256]");
+    int rc = huff_decode_common(words, num_words, chunk_offsets, table, alpha, beta, q, n, bucket, &geo, &grid);
+    if (rc) return rc;
+    huff_decode_dequant_kernel<true><<<grid, kHuffDecThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        words, num_words, chunk_offsets, table, nullptr, 0, alpha, beta, q, geo, (float)(levels - 1), (n + kHuffChunk - 1) / kHuffChunk);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+extern "C" int qd_huffman_decode_dequant_nonuniform(const uint32_t* words, int64_t num_words, const uint32_t* chunk_offsets,
+                                                    const qd_huffman_table* table, const float* points, int num_points,
+                                                    const float* alpha, const float* beta, float* q, int64_t n, int64_t bucket,
+                                                    qd_stream_t stream) {
+    Geometry geo;
+    int grid = 0;
+    if (points == nullptr || num_points < 1 || num_points > 256) return fail(QD_ERR_INVALID_ARG, "num_points must be in [1, 256]");
+    int rc = huff_decode_common(words, num_words, chunk_offsets, table, alpha, beta, q, n, bucket, &geo, &grid);
+    if (rc) return rc;
+    huff_decode_dequant_kernel<false><<<grid, kHuffDecThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        words, num_words, chunk_offsets, table, points, num_points, alpha, beta, q, geo, 0.f, (n + kHuffChunk - 1) / kHuffChunk);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }

@@ -14,7 +14,8 @@ import torch
 from .. import _native as N
 
 __all__ = ("create_bucket_tensor", "assign_bits_automatically", "initialize_quantization_points", "huffman_encode",
-           "get_huffman_encoding_mean_bit_length", "index_histogram", "order_statistics", "gradient_norms")
+           "get_huffman_encoding_mean_bit_length", "huffman_code_of_histogram", "index_histogram", "order_statistics",
+           "gradient_norms")
 
 
 def create_bucket_tensor(tensor, bucket_size, fill_values="last"):
@@ -223,8 +224,18 @@ def get_huffman_encoding_mean_bit_length(model_param_iter, quantization_function
         index_histogram(bins_u8, max(nbins, 1), counts[:256])
     counts = counts.cpu().numpy()
     assert total_length == int(counts.sum())                                              # :227
+    frequency, code = huffman_code_of_histogram(counts)
+    return sum(frequency[sym] * len(bits) for sym, bits in code)
+
+
+def huffman_code_of_histogram(counts):
+    """(frequency, code) of a level histogram the way the reference builds them (help_functions.py:226-231):
+    ``frequency[level] = count / total`` over the non-zero bins, then ``huffman_encode`` on that dict.  The
+    size accounting above and the Huffman codec (codec.py) both take their code from here, so float ties
+    break identically and the stored stream has exactly the accounted length."""
+    counts = np.asarray(counts)
+    total_length = int(counts.sum())
     frequency = defaultdict(int)
     for val in np.nonzero(counts)[0]:
         frequency[int(val)] = counts[val] / total_length
-    code = huffman_encode(frequency)
-    return sum(frequency[sym] * len(bits) for sym, bits in code)
+    return frequency, huffman_encode(frequency)

@@ -23,6 +23,7 @@ if ROOT not in sys.path:
 def run(dev=None, out_path=None, max_log2=28, min_log2=10, only=None):
     import torch
     from quantized_distillation_b200 import _native as N
+    from quantized_distillation_b200 import codec
     dev = dev or torch.device("cuda", torch.cuda.current_device())
     lib = N.lib()
     peak = 3350.0
@@ -109,6 +110,27 @@ def run(dev=None, out_path=None, max_log2=28, min_log2=10, only=None):
                 ops["pack_2bit"] = (1.25, lambda i: N.check(lib.qd_pack_indices(N.ptr(idx[i]), N.ptr(packed2), n, 2, sp)))
                 ops["unpack_dequant_nonuniform_4bit"] = (4.5, lambda i: N.check(lib.qd_unpack_dequant_nonuniform(
                     N.ptr(packed), 4, N.ptr(pts16), 16, N.ptr(alpha), N.ptr(beta), N.ptr(qs[i]), n, bucket, sp)))
+                # Huffman codec on the 16 levels of the weight-like xs[0]: the stream is made once, outside the timed
+                # loop, and the algorithmic bytes come from its actual length (+ one uint32 offset per chunk)
+                hidx, ha, hb = torch.empty(n, dtype=torch.uint8, device=dev), torch.empty(rws, device=dev), torch.empty(rws, device=dev)
+                N.check(lib.qd_uniform_fwd(N.ptr(xs[0]), None, N.ptr(hidx), N.ptr(ha), N.ptr(hb), None, None, n, bucket, 16, None, 0.0,
+                                           0, 0, 0, N.ptr(ws), ws.numel(), sp))
+                hcounts = torch.bincount(hidx, minlength=256).cpu().numpy()
+                hlen = codec.huffman_code_lengths(hcounts)
+                htab = torch.from_numpy(codec.huffman_table(hlen)).to(dev)
+                hchunks = -(-n // codec.HUFFMAN_CHUNK)
+                hcap = -(-int(sum(int(hcounts[s_]) * l_ for s_, l_ in hlen.items())) // 32) + hchunks
+                hwords = torch.empty(hcap, dtype=torch.int32, device=dev)
+                hoffs = torch.empty(hchunks, dtype=torch.int32, device=dev)
+                htot = torch.zeros(1, dtype=torch.int64, device=dev)
+                N.check(lib.qd_huffman_encode(N.ptr(hidx), n, N.ptr(htab), N.ptr(hwords), hcap, N.ptr(hoffs), N.ptr(htot), sp))
+                hn = int(htot.item())
+                hstream = (hn + hchunks) * 4 / n          # stream + chunk index bytes per element
+                ops["huffman_encode_16lvl"] = (2 + hstream, lambda i: N.check(lib.qd_huffman_encode(
+                    N.ptr(hidx), n, N.ptr(htab), N.ptr(hwords), hcap, N.ptr(hoffs), N.ptr(htot), sp)))
+                ops["huffman_decode_dequant_uniform_16lvl"] = (4 + hstream, lambda i: N.check(lib.qd_huffman_decode_dequant_uniform(
+                    N.ptr(hwords), hn, N.ptr(hoffs), N.ptr(htab), N.ptr(ha), N.ptr(hb), N.ptr(qs[i]),
+                    n, bucket, 16, sp)))
                 ops["uniform_fwd_bwd_minmax"] = (16, lambda i: N.check(lib.qd_uniform_fwd_bwd(
                     N.ptr(xs[i]), N.ptr(gs[i]), N.ptr(qs[i]), N.ptr(gos[i]), n, bucket, 16, N.BWD_MINMAX, N.ptr(ws), ws.numel(), sp)))
                 ops["uniform_bwd_minmax"] = (12, lambda i: N.check(lib.qd_uniform_bwd(
