@@ -201,6 +201,28 @@ int qd_huffman_decode_dequant_nonuniform(const uint32_t* words, int64_t num_word
                                          const qd_huffman_table* table, const float* points, int num_points,
                                          const float* alpha, const float* beta, float* q, int64_t n, int64_t bucket,
                                          qd_stream_t stream);
+/* Whole model in one launch: every chunk of every tensor, with the model-wide table, levels and bucket; q of each
+ * tensor is bit-identical to the per-tensor entry points above.  The host array is validated, then copied into
+ * `workspace` (device, 16-byte aligned, >= qd_huffman_model_workspace_bytes(count) bytes, private to the stream
+ * until the launch has run) with a stream-ordered copy; the call neither allocates nor synchronises, and the host
+ * array may be reused as soon as it returns. */
+typedef struct {                 /* one quantized tensor of a model; every pointer is DEVICE memory */
+    const uint32_t* words;       /* may be NULL when num_words == 0 (single-symbol code) */
+    const uint32_t* chunk_offsets;
+    const float* alpha;
+    const float* beta;
+    const float* points;         /* non-uniform: this tensor's points; NULL for uniform */
+    float* q;                    /* n floats, contiguous; 4-byte alignment is enough */
+    int64_t num_words;
+    int64_t n;                   /* >= 1 */
+    int32_t num_points;          /* non-uniform: 1..256; uniform: 0 */
+    int32_t reserved;            /* 0 */
+} qd_huffman_tensor;
+size_t qd_huffman_model_workspace_bytes(int count);
+int qd_huffman_decode_dequant_model(const qd_huffman_tensor* tensors /* HOST array */, int count,
+                                    const qd_huffman_table* table, int64_t bucket,
+                                    int levels /* uniform: s in [2,256]; 0: non-uniform */,
+                                    void* workspace, size_t workspace_bytes, qd_stream_t stream);
 
 /* ---- next row f1: one launch over every parameter tensor of a model ------
  * (replaces the per-tensor loop of cnn_models/conv_forward_model.py:236-247).

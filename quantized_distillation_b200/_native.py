@@ -47,6 +47,8 @@ SIGNATURES = {
     "qd_huffman_encode": (C.c_int, [_p, _i64, _p, _p, _i64, _p, _p, _p]),
     "qd_huffman_decode_dequant_uniform": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _i64, _i64, _i32, _p]),
     "qd_huffman_decode_dequant_nonuniform": (C.c_int, [_p, _i64, _p, _p, _p, _i32, _p, _p, _p, _i64, _i64, _p]),
+    "qd_huffman_model_workspace_bytes": (_sz, [_i32]),
+    "qd_huffman_decode_dequant_model": (C.c_int, [_p, _i32, _p, _i64, _i32, _p, _sz, _p]),
     "qd_plan_create": (C.c_int, [C.POINTER(_p), _i32, _p, _p, _p, _p, _i64]),
     "qd_plan_destroy": (C.c_int, [_p]),
     "qd_plan_set_shadow": (C.c_int, [_p, _p]),

@@ -115,9 +115,16 @@ HUFFMAN_MAX_LENGTH = 57         # QD_HUFFMAN_MAX_LENGTH
 HUFFMAN_LUT_BITS = 11           # QD_HUFFMAN_LUT_BITS
 HUFFMAN_TABLE_BYTES = 13328     # sizeof(qd_huffman_table)
 FILE_MAGIC = b"QDHUFF\x00\x00"
-FILE_VERSION = 1
+FILE_VERSION = 1                # parameters only
+FILE_VERSION_BUFFERS = 2        # parameters + persistent buffers: a version-1 reader refuses it rather than drop them
 _PREFIX = struct.Struct("<8sIIQ")   # magic, version, reserved (0), JSON header length
 _ALIGN = 16
+# dtypes a stored buffer may have, by their name in the header
+_BUFFER_DTYPES = {"float32": torch.float32, "int64": torch.int64}
+# qd_huffman_tensor (include/qd_b200.h): one entry of the whole-model decode
+_MODEL_TENSOR = np.dtype([("words", "<u8"), ("chunk_offsets", "<u8"), ("alpha", "<u8"), ("beta", "<u8"), ("points", "<u8"),
+                          ("q", "<u8"), ("num_words", "<i8"), ("n", "<i8"), ("num_points", "<i4"), ("reserved", "<i4")])
+assert _MODEL_TENSOR.itemsize == 72
 
 
 def huffman_code_lengths(counts) -> dict:
@@ -217,6 +224,10 @@ class CompressedModel:
     tensors: list
     chunk: int = HUFFMAN_CHUNK
     _tables: dict = field(default_factory=dict, repr=False)
+    # persistent buffers (BatchNorm running statistics, ...) as [(name, tensor)] in state_dict() order; None: not stored
+    buffers: list = None
+    # a loaded file's data region: every section is a view into it, so it reaches a device in one copy
+    _data: torch.Tensor = field(default=None, init=False, repr=False, compare=False)
 
     def table(self, device) -> torch.Tensor:
         key = str(device)
@@ -226,17 +237,18 @@ class CompressedModel:
 
     def size_breakdown(self) -> dict:
         """Bytes of the saved file by what they hold.  code_bits / 8 + scale_bytes + unquantized_bytes is what
-        get_size_quantized_model accounts for; the rest is the price of the format."""
+        get_size_quantized_model accounts for; the rest is the price of the format (and the stored buffers)."""
         header, sections, data_bytes = _layout(self)
         q = [t for t in self.tensors if t.quantized]
         code_bits = sum(t.code_bits for t in q)
-        section_bytes = sum(nb for _, _, nb, _ in sections)
+        section_bytes = sum(nb for _, nb, _ in sections)
         return {
             "code_bits": code_bits,
             "padding_bits": sum(t.words.numel() for t in q) * 32 - code_bits,
             "chunk_index_bytes": sum(t.chunk_offsets.numel() * 4 for t in q),
             "scale_bytes": sum((t.alpha.numel() + t.beta.numel()) * 4 for t in q),
             "unquantized_bytes": sum(t.raw.numel() * 4 for t in self.tensors if not t.quantized),
+            "buffer_bytes": sum(b.numel() * b.element_size() for _, b in self.buffers or []),
             "header_bytes": _PREFIX.size + len(header),
             "alignment_bytes": _align(_PREFIX.size + len(header)) - _PREFIX.size - len(header) + data_bytes - section_bytes,
             "file_bytes": _align(_PREFIX.size + len(header)) + data_bytes,
@@ -253,11 +265,19 @@ def _sections_of(t: HuffmanTensor):
     return [("words", t.words), ("chunk_offsets", t.chunk_offsets), ("alpha", t.alpha), ("beta", t.beta)]
 
 
+def _dtype_name(tensor) -> str:
+    name = str(tensor.dtype).replace("torch.", "")
+    if name not in _BUFFER_DTYPES:
+        raise ValueError(f"buffers of dtype {tensor.dtype} cannot be stored (float32 and int64 can)")
+    return name
+
+
 def _layout(cm: CompressedModel):
-    """(JSON header bytes, [(tensor index, section name, nbytes, offset)], data bytes); offsets are relative to
-    the first 16-byte boundary after the header."""
+    """(JSON header bytes, [(tensor, nbytes, offset)], data bytes); offsets are relative to the first 16-byte
+    boundary after the header.  The buffers' sections follow the parameters' and their key exists only in a
+    version-2 header, so a file without buffers is laid out exactly as version 1 always was."""
     sections, entries, off = [], [], 0
-    for i, t in enumerate(cm.tensors):
+    for t in cm.tensors:
         e = {"name": t.name, "shape": list(t.shape), "dtype": "float32", "quantized": t.quantized, "sections": {}}
         if t.quantized:
             e["code_bits"] = int(t.code_bits)
@@ -266,12 +286,26 @@ def _layout(cm: CompressedModel):
         for name, tensor in _sections_of(t):
             nb = tensor.numel() * 4
             e["sections"][name] = [off, nb]
-            sections.append((i, name, nb, off))
+            sections.append((tensor, nb, off))
             off = _align(off + nb)
         entries.append(e)
+    buffers = []
+    for name, b in cm.buffers or []:
+        nb = b.numel() * b.element_size()
+        buffers.append({"name": name, "shape": list(b.shape), "dtype": _dtype_name(b), "section": [off, nb]})
+        sections.append((b, nb, off))
+        off = _align(off + nb)
     header = {"chunk": cm.chunk, "kind": cm.kind, "levels": cm.levels, "bucket": cm.bucket_size,
               "code": [[int(s), int(l)] for s, l in sorted(cm.code_lengths.items())], "tensors": entries, "data_bytes": off}
+    if cm.buffers is not None:
+        header["buffers"] = buffers
     return json.dumps(header, separators=(",", ":")).encode("utf-8"), sections, off
+
+
+def _persistent_buffers(model):
+    """[(name, tensor)] of the buffers model.state_dict() holds, in its order."""
+    params = {id(p) for p in model.parameters()}
+    return [(k, v) for k, v in model.state_dict(keep_vars=True).items() if torch.is_tensor(v) and id(v) not in params]
 
 
 def _selected(named, quantize_first_and_last_layer):
@@ -281,12 +315,19 @@ def _selected(named, quantize_first_and_last_layer):
 
 
 def compress_model(model, numBits=None, bucket_size=256, quantize_first_and_last_layer=True, *, points=None,
-                   rule="nearest") -> CompressedModel:
+                   rule="nearest", include_buffers=False) -> CompressedModel:
     """Huffman-codes a model's quantized parameters.  Uniform: ``numBits`` (s = 2**numBits levels,
     uniformQuantization).  Non-uniform: ``points`` -- one ascending list of centroids for every tensor, or one
     list per quantized tensor (the differentiable-quantization output) -- with nonUniformQuantization's
     ``rule``.  One level histogram over all quantized tensors gives the code, so the stored code bits equal
-    get_huffman_encoding_mean_bit_length x the number of quantized weights."""
+    get_huffman_encoding_mean_bit_length x the number of quantized weights.  ``include_buffers``: also store the
+    persistent buffers (state_dict() order, float32 or int64, e.g. BatchNorm running statistics) as they are, so
+    that decompress_ into a freshly built network gives back the whole eval-mode model."""
+    buffers = None
+    if include_buffers:
+        buffers = _persistent_buffers(model)
+        for _, b in buffers:
+            _dtype_name(b)
     N.require_cuda()
     if (numBits is None) == (points is None):
         raise ValueError("give numBits (uniform) or points (non-uniform), not both")
@@ -337,7 +378,8 @@ def compress_model(model, numBits=None, bucket_size=256, quantize_first_and_last
         if not idxs:
             raise ValueError("no parameter is selected for quantization")
         lengths = huffman_code_lengths(counts.sum(0).cpu().numpy())
-        cm = CompressedModel("uniform" if uniform else "nonuniform", s if uniform else None, bucket_size, lengths, tensors)
+        cm = CompressedModel("uniform" if uniform else "nonuniform", s if uniform else None, bucket_size, lengths, tensors,
+                             buffers=None if buffers is None else [(name, b.detach().to(dev).clone()) for name, b in buffers])
         table = cm.table(dev)
         len_vec = torch.zeros(256, dtype=torch.int64)
         for sym, l in lengths.items():
@@ -403,21 +445,104 @@ def decompress_tensor(cm: CompressedModel, which, out: torch.Tensor = None, devi
     return out
 
 
+def _mover(cm: CompressedModel, dev):
+    """tensor -> the same tensor on ``dev``.  Sections of a file loaded to the host are views into its data region,
+    which goes to ``dev`` in one copy (on first use); any other tensor moves by itself (no copy when it is there)."""
+    host = cm._data if cm._data is not None and not cm._data.is_cuda else None
+    region = []
+
+    def move(x):
+        if x is None:
+            return None
+        if host is not None and not x.is_cuda and x.untyped_storage().data_ptr() == host.untyped_storage().data_ptr():
+            if not region:
+                region.append(host.to(dev))
+            off = x.data_ptr() - host.data_ptr()
+            return region[0][off:off + x.numel() * x.element_size()].view(x.dtype).view(x.shape)
+        return x.to(dev)
+    return move
+
+
+def _model_decode_args(cm: CompressedModel, items, dev, move):
+    """Arguments of one qd_huffman_decode_dequant_model call that decodes every (quantized tensor, out) of
+    ``items`` on ``dev`` (the current device); out: contiguous float32 on ``dev``.  Also returns the device tensors
+    the call reads, which must outlive its enqueueing."""
+    desc = np.zeros(len(items), _MODEL_TENSOR)
+    keep = []
+    if cm.kind != "uniform":                     # every tensor's points in one upload
+        src = items[0][0].points.device
+        flat = move(torch.cat([t.points.reshape(-1).to(src, torch.float32) for t, _ in items]))
+        keep.append(flat)
+    at = 0
+    for i, (t, out) in enumerate(items):
+        words, offs, alpha, beta = (move(x) for x in (t.words, t.chunk_offsets, t.alpha, t.beta))
+        keep += [words, offs, alpha, beta]
+        points, k = 0, 0
+        if cm.kind != "uniform":
+            k = t.points.numel()
+            points = flat[at:at + k].data_ptr()
+            at += k
+        desc[i] = (N.ptr(words) if words.numel() else 0, N.ptr(offs), N.ptr(alpha), N.ptr(beta), points, N.ptr(out), words.numel(),
+                   t.numel, k, 0)
+    ws = torch.empty(int(N.lib().qd_huffman_model_workspace_bytes(len(items))), dtype=torch.uint8, device=dev)
+    keep += [desc, ws]
+    table = cm.table(dev)
+    args = (desc.ctypes.data, len(items), N.ptr(table), 0 if cm.bucket_size is None else int(cm.bucket_size),
+            int(cm.levels) if cm.kind == "uniform" else 0, N.ptr(ws), ws.numel(), N.stream_ptr(dev))
+    return args, keep
+
+
 def decompress_(cm: CompressedModel, model) -> None:
-    """Writes every parameter of ``model`` in place from ``cm`` (existing parameter handles stay valid)."""
+    """Writes every parameter of ``model`` in place from ``cm`` (existing parameter handles stay valid), and its
+    persistent buffers when ``cm`` stores them.  Everything is checked before anything is written.  Per device, the
+    quantized tensors decode in one launch, straight into parameters that are contiguous float32 on that device."""
     named = list(model.named_parameters())
     if len(named) != len(cm.tensors):
         raise ValueError(f"model has {len(named)} parameters, the compressed model {len(cm.tensors)}")
     for (name, p), t in zip(named, cm.tensors):
         if tuple(p.shape) != tuple(t.shape):
             raise ValueError(f"{name}: shape {tuple(p.shape)} != stored {tuple(t.shape)} ({t.name})")
+    bufs = []
+    if cm.buffers is not None:
+        bufs = _persistent_buffers(model)
+        if len(bufs) != len(cm.buffers):
+            raise ValueError(f"model has {len(bufs)} persistent buffers, the compressed model {len(cm.buffers)}")
+        for (name, b), (stored, s) in zip(bufs, cm.buffers):
+            if tuple(b.shape) != tuple(s.shape) or b.dtype != s.dtype:
+                raise ValueError(f"buffer {name}: {b.dtype} {tuple(b.shape)} != stored {s.dtype} {tuple(s.shape)} ({stored})")
+    default = _device_of(cm)
+    groups = {}                                  # device -> parameter indices (host parameters decode on `default`)
+    for k, (_, p) in enumerate(named):
+        groups.setdefault(p.device if p.is_cuda else default, []).append(k)
+    for _, b in bufs:
+        if b.is_cuda:
+            groups.setdefault(b.device, [])
     with torch.no_grad():
-        for k, (_, p) in enumerate(named):
-            d = p.data
-            if d.is_cuda and d.dtype == torch.float32 and d.is_contiguous():
-                decompress_tensor(cm, k, out=d)
-            else:
-                d.copy_(decompress_tensor(cm, k, device=d.device if d.is_cuda else None))
+        for dev, ks in groups.items():
+            with torch.cuda.device(dev):
+                move = _mover(cm, dev)
+                items, temps = [], []
+                for k in ks:
+                    t, d = cm.tensors[k], named[k][1].data
+                    if not t.quantized:
+                        d.copy_((move(t.raw) if d.is_cuda else t.raw).view_as(d))
+                    elif d.device == dev and d.dtype == torch.float32 and d.is_contiguous():
+                        items.append((t, d))
+                    else:
+                        out = torch.empty(t.numel, dtype=torch.float32, device=dev)
+                        items.append((t, out))
+                        temps.append((d, out))
+                if items:
+                    args, keep = _model_decode_args(cm, items, dev, move)
+                    N.check(N.lib().qd_huffman_decode_dequant_model(*args))
+                for d, out in temps:
+                    d.copy_(out.view_as(d))
+                for (_, b), (_, s) in zip(bufs, cm.buffers or []):
+                    if b.is_cuda and b.device == dev:
+                        b.copy_(move(s))
+        for (_, b), (_, s) in zip(bufs, cm.buffers or []):
+            if not b.is_cuda:
+                b.copy_(s)
 
 
 def save_compressed(cm: CompressedModel, path) -> int:
@@ -426,12 +551,12 @@ def save_compressed(cm: CompressedModel, path) -> int:
     header, sections, data_bytes = _layout(cm)
     start = _align(_PREFIX.size + len(header))
     buf = bytearray(start + data_bytes)
-    buf[:_PREFIX.size] = _PREFIX.pack(FILE_MAGIC, FILE_VERSION, 0, len(header))
+    version = FILE_VERSION if cm.buffers is None else FILE_VERSION_BUFFERS
+    buf[:_PREFIX.size] = _PREFIX.pack(FILE_MAGIC, version, 0, len(header))
     buf[_PREFIX.size:_PREFIX.size + len(header)] = header
-    for i, name, nb, off in sections:
-        tensor = dict(_sections_of(cm.tensors[i]))[name]
-        buf[start + off:start + off + nb] = tensor.detach().contiguous().cpu().numpy().astype("<i4" if tensor.dtype == torch.int32 else "<f4",
-                                                                                            copy=False).tobytes()
+    little = {torch.int32: "<i4", torch.float32: "<f4", torch.int64: "<i8"}
+    for tensor, nb, off in sections:
+        buf[start + off:start + off + nb] = tensor.detach().contiguous().cpu().numpy().astype(little[tensor.dtype], copy=False).tobytes()
     with open(path, "wb") as f:
         f.write(buf)
     return len(buf)
@@ -442,17 +567,18 @@ def _bad(msg):
 
 
 def load_compressed(path, device=None) -> CompressedModel:
-    """Reads and validates a file written by save_compressed.  device=None keeps every section in host memory
-    (reading and validating needs no GPU); decoding then moves them to the GPU."""
+    """Reads and validates a file written by save_compressed (version 1, or 2 with buffers).  Every section is a
+    view into one tensor holding the file's data region.  device=None keeps it in host memory (reading and
+    validating needs no GPU; decompress_ moves it to the GPU in one copy); a device gets it in one copy here."""
     with open(path, "rb") as f:
-        buf = f.read()
+        buf = bytearray(f.read())
     if len(buf) < _PREFIX.size:
         _bad("shorter than its prefix")
     magic, version, _, hlen = _PREFIX.unpack_from(buf)
     if magic != FILE_MAGIC:
         _bad("bad magic")
-    if version != FILE_VERSION:
-        _bad(f"format version {version}, this reader knows {FILE_VERSION}")
+    if version not in (FILE_VERSION, FILE_VERSION_BUFFERS):
+        _bad(f"format version {version}, this reader knows {FILE_VERSION} and {FILE_VERSION_BUFFERS}")
     if _PREFIX.size + hlen > len(buf):
         _bad("header runs past the end of the file")
     try:
@@ -463,8 +589,12 @@ def load_compressed(path, device=None) -> CompressedModel:
     except (ValueError, KeyError, TypeError) as e:
         _bad(f"unreadable header ({e})")
     start = _align(_PREFIX.size + hlen)
-    if start + data_bytes != len(buf):
+    if data_bytes < 0 or start + data_bytes != len(buf):
         _bad(f"{len(buf)} bytes, the header describes {start + data_bytes}")
+    if ("buffers" in h) != (version == FILE_VERSION_BUFFERS):
+        _bad(f"a version-{version} file {'must not list' if version == FILE_VERSION else 'must list its'} buffers")
+    region = torch.from_numpy(np.frombuffer(buf, np.uint8, count=data_bytes, offset=start)) if data_bytes else \
+        torch.empty(0, dtype=torch.uint8)
     if chunk != HUFFMAN_CHUNK:
         _bad(f"chunk of {chunk} symbols, this reader decodes {HUFFMAN_CHUNK}")
     if kind not in ("uniform", "nonuniform"):
@@ -482,6 +612,9 @@ def load_compressed(path, device=None) -> CompressedModel:
     if kind == "uniform" and max(code) >= levels:
         _bad("a code symbol is not a level")
 
+    def view(off, nb, dtype, shape):
+        return region[off:off + nb].view(dtype).view(shape)
+
     def section(e, name, dtype, count):
         try:
             off, nb = (int(v) for v in e["sections"][name])
@@ -489,7 +622,7 @@ def load_compressed(path, device=None) -> CompressedModel:
             _bad(f"{e.get('name')}: section {name} missing")
         if off < 0 or off % _ALIGN or nb != count * 4 or off + nb > data_bytes:
             _bad(f"{e.get('name')}: section {name} out of range")
-        return torch.from_numpy(np.frombuffer(buf, dtype=dtype, count=count, offset=start + off).copy())
+        return view(off, nb, dtype, (count,))
 
     tensors = []
     for e in entries:
@@ -501,7 +634,7 @@ def load_compressed(path, device=None) -> CompressedModel:
             _bad(f"{name}: bad dtype or shape")
         n = int(math.prod(shape))
         if not quantized:
-            tensors.append(HuffmanTensor(name, shape, raw=section(e, "raw", "<f4", n)))
+            tensors.append(HuffmanTensor(name, shape, raw=section(e, "raw", torch.float32, n)))
             continue
         if n == 0:
             _bad(f"{name}: empty quantized tensor")
@@ -510,8 +643,8 @@ def load_compressed(path, device=None) -> CompressedModel:
         words_nb = e.get("sections", {}).get("words", [0, -1])[1]
         if not isinstance(words_nb, int) or words_nb < 0 or words_nb % 4:
             _bad(f"{name}: section words out of range")
-        words = section(e, "words", "<i4", words_nb // 4)
-        offs = section(e, "chunk_offsets", "<i4", chunks)
+        words = section(e, "words", torch.int32, words_nb // 4)
+        offs = section(e, "chunk_offsets", torch.int32, chunks)
         o = offs.numpy().view(np.uint32).astype(np.int64)
         if o[0] != 0 or np.any(np.diff(o) < 0) or o[-1] > words.numel():
             _bad(f"{name}: chunk offsets out of range")
@@ -525,14 +658,49 @@ def load_compressed(path, device=None) -> CompressedModel:
             if not 1 <= pts.numel() <= 256:
                 _bad(f"{name}: {pts.numel()} points, expected 1 to 256")
         tensors.append(HuffmanTensor(name, shape, words=words, chunk_offsets=offs,
-                                     alpha=section(e, "alpha", "<f4", rows), beta=section(e, "beta", "<f4", rows), points=pts,
-                                     code_bits=int(e.get("code_bits", 0))))
+                                     alpha=section(e, "alpha", torch.float32, rows), beta=section(e, "beta", torch.float32, rows),
+                                     points=pts, code_bits=int(e.get("code_bits", 0))))
+    buffers = None
+    if version == FILE_VERSION_BUFFERS:
+        if not isinstance(h["buffers"], list):
+            _bad("buffers is not a list")
+        buffers, names = [], set()
+        for e in h["buffers"]:
+            try:
+                name, shape, dtype = str(e["name"]), tuple(int(d) for d in e["shape"]), e["dtype"]
+                off, nb = (int(v) for v in e["section"])
+            except (KeyError, TypeError, ValueError):
+                _bad("buffer entry without name / shape / dtype / section")
+            if dtype not in _BUFFER_DTYPES:
+                _bad(f"buffer {name}: unknown dtype {dtype!r}")
+            if any(d < 0 for d in shape):
+                _bad(f"buffer {name}: bad shape")
+            if name in names:
+                _bad(f"buffer {name} appears twice")
+            names.add(name)
+            tdtype = _BUFFER_DTYPES[dtype]
+            size = int(math.prod(shape)) * tdtype.itemsize
+            if nb != size:
+                _bad(f"buffer {name}: {nb} bytes, its shape and dtype need {size}")
+            if off < 0 or off % _ALIGN or off + nb > data_bytes:
+                _bad(f"buffer {name}: section out of range")
+            buffers.append((name, view(off, nb, tdtype, shape)))
+    cm = CompressedModel(kind, levels, bucket, code, tensors, buffers=buffers)
+    cm._data = region
     if device is not None:                       # everything is validated before anything reaches the GPU
+        move = _mover(cm, torch.device(device))
+        pts = [t.points for t in tensors if t.points is not None]
+        flat = torch.cat(pts).to(device) if pts else None          # every tensor's points in one upload too
+        at = 0
         for t in tensors:
-            for f_ in ("words", "chunk_offsets", "alpha", "beta", "points", "raw"):
-                if getattr(t, f_) is not None:
-                    setattr(t, f_, getattr(t, f_).to(device))
-    return CompressedModel(kind, levels, bucket, code, tensors)
+            for f_ in ("words", "chunk_offsets", "alpha", "beta", "raw"):
+                setattr(t, f_, move(getattr(t, f_)))
+            if t.points is not None:
+                t.points, at = flat[at:at + t.points.numel()], at + t.points.numel()
+        if buffers is not None:
+            cm.buffers = [(name, move(b)) for name, b in buffers]
+        cm._data = move(region)
+    return cm
 
 
 def get_size_reduction(effective_number_bits, bucket_size=256, full_precision_bits=32):

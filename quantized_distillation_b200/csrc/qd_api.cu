@@ -1044,6 +1044,59 @@ extern "C" int qd_huffman_decode_dequant_nonuniform(const uint32_t* words, int64
     return QD_OK;
 }
 
+// workspace of the model decode: the tensor array, then cta_start[count + 1] (int32)
+static_assert(sizeof(qd_huffman_tensor) == 72 && sizeof(qd_huffman_tensor) % alignof(int32_t) == 0,
+              "qd_huffman_tensor layout is shared with codec.py");
+
+extern "C" size_t qd_huffman_model_workspace_bytes(int count) {
+    return count < 1 ? 0 : (size_t)count * sizeof(qd_huffman_tensor) + ((size_t)count + 1) * sizeof(int32_t);
+}
+
+extern "C" int qd_huffman_decode_dequant_model(const qd_huffman_tensor* tensors, int count, const qd_huffman_table* table,
+                                               int64_t bucket, int levels, void* workspace, size_t workspace_bytes,
+                                               qd_stream_t stream) {
+    if (tensors == nullptr || count < 1 || table == nullptr) return fail(QD_ERR_INVALID_ARG, "NULL tensors / table or count < 1");
+    if (bucket < 0) return fail(QD_ERR_INVALID_ARG, "bucket must be >= 0");
+    if (levels != 0 && (levels < 2 || levels > 256)) return fail(QD_ERR_INVALID_ARG, "levels must be in [2, 256] (uniform) or 0 (non-uniform)");
+    const size_t need = qd_huffman_model_workspace_bytes(count);
+    if (workspace == nullptr || (reinterpret_cast<uintptr_t>(workspace) & 15) || workspace_bytes < need)
+        return fail(QD_ERR_WORKSPACE, "workspace must be 16-byte aligned and hold %zu bytes (got %zu)", need, workspace_bytes);
+    const bool uniform = levels != 0;
+    // host image of the workspace, consumed by the pageable copy before it returns (kept per thread: no allocation once grown)
+    thread_local std::vector<unsigned char> image;
+    image.resize(need);
+    int32_t* cta_start = reinterpret_cast<int32_t*>(image.data() + (size_t)count * sizeof(qd_huffman_tensor));
+    int64_t ctas = 0;
+    for (int i = 0; i < count; ++i) {
+        const qd_huffman_tensor& t = tensors[i];
+        if (t.chunk_offsets == nullptr || t.alpha == nullptr || t.beta == nullptr || t.q == nullptr)
+            return fail(QD_ERR_INVALID_ARG, "tensor %d: NULL argument", i);
+        if (t.num_words < 0 || (t.num_words > 0 && t.words == nullptr)) return fail(QD_ERR_INVALID_ARG, "tensor %d: bad words / num_words", i);
+        if (t.n < 1) return fail(QD_ERR_INVALID_ARG, "tensor %d: n must be >= 1", i);
+        if (t.reserved != 0) return fail(QD_ERR_INVALID_ARG, "tensor %d: reserved must be 0", i);
+        if (uniform && (t.points != nullptr || t.num_points != 0))
+            return fail(QD_ERR_INVALID_ARG, "tensor %d: a uniform model has no points (points NULL, num_points 0)", i);
+        if (!uniform && (t.points == nullptr || t.num_points < 1 || t.num_points > 256))
+            return fail(QD_ERR_INVALID_ARG, "tensor %d: num_points must be in [1, 256]", i);
+        cta_start[i] = (int32_t)ctas;
+        ctas += ((t.n + kHuffChunk - 1) / kHuffChunk + kHuffDecThreads - 1) / kHuffDecThreads;
+        if (ctas > INT32_MAX) return fail(QD_ERR_INVALID_ARG, "the model has more than 2^31 - 1 blocks of %d chunks", kHuffDecThreads);
+    }
+    cta_start[count] = (int32_t)ctas;
+    memcpy(image.data(), tensors, (size_t)count * sizeof(qd_huffman_tensor));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    QD_CUDA(cudaMemcpyAsync(workspace, image.data(), need, cudaMemcpyHostToDevice, st));
+    const qd_huffman_tensor* dev_tensors = static_cast<const qd_huffman_tensor*>(workspace);
+    const int32_t* dev_start = reinterpret_cast<const int32_t*>(static_cast<const unsigned char*>(workspace) + (size_t)count * sizeof(qd_huffman_tensor));
+    if (uniform)
+        huff_decode_dequant_model_kernel<true><<<(unsigned)ctas, kHuffDecThreads, 0, st>>>(dev_tensors, dev_start, count, table, bucket,
+                                                                                           (float)(levels - 1));
+    else
+        huff_decode_dequant_model_kernel<false><<<(unsigned)ctas, kHuffDecThreads, 0, st>>>(dev_tensors, dev_start, count, table, bucket, 0.f);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
 // ------------------------------------------------------------------ plans (f1)
 struct qd_plan {
     int count = 0;

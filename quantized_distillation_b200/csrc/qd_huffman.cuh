@@ -208,12 +208,11 @@ __device__ __forceinline__ uint32_t huff_decode_one(const HuffDecodeShared& s, i
     return sym;
 }
 
+// the code (model-wide) and the unit table (per tensor: level / S, or the tensor's points) into shared memory; the
+// caller synchronises the CTA before decoding
 template <bool UNIFORM>
-__global__ void __launch_bounds__(kHuffDecThreads) huff_decode_dequant_kernel(
-    const uint32_t* __restrict__ words, int64_t num_words, const uint32_t* __restrict__ offs,
-    const qd_huffman_table* __restrict__ tab, const float* __restrict__ points, int K, const float* __restrict__ alpha,
-    const float* __restrict__ beta, float* __restrict__ q, Geometry geo, float S, int64_t chunks) {
-    __shared__ HuffDecodeShared s;
+__device__ __forceinline__ void huff_load_tables(HuffDecodeShared& s, const qd_huffman_table* __restrict__ tab, float S,
+                                                 const float* __restrict__ points, int K) {
     for (int i = threadIdx.x; i < (1 << kHuffLutBits); i += blockDim.x) s.lut[i] = tab->lut[i];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) {
         s.symbols[i] = tab->symbols[i];
@@ -225,55 +224,99 @@ __global__ void __launch_bounds__(kHuffDecThreads) huff_decode_dequant_kernel(
         s.count[i] = tab->count[i];
         s.index[i] = tab->index[i];
     }
+}
+
+// Decodes chunks [c0, c0 + kHuffDecThreads) of one tensor (c0 < chunks), one chunk per thread.  Every thread of the
+// CTA calls it with the same arguments (the staging rounds synchronise the CTA).
+__device__ __forceinline__ void huff_decode_chunks(HuffDecodeShared& s, int max_len, const uint32_t* __restrict__ words,
+                                                   int64_t num_words, const uint32_t* __restrict__ offs,
+                                                   const float* __restrict__ alpha, const float* __restrict__ beta,
+                                                   float* __restrict__ q, int64_t n, int64_t L, bool single_row, int64_t chunks,
+                                                   int64_t c0) {
+    const bool qvec = (reinterpret_cast<uintptr_t>(q) & 15) == 0;
+    const int64_t c = c0 + threadIdx.x;
+    const int64_t e0 = c * kHuffChunk;
+    const int m = c < chunks ? (int)(n - e0 < kHuffChunk ? n - e0 : kHuffChunk) : 0;
+    const int m_cta = (int)(n - c0 * kHuffChunk < kHuffChunk ? n - c0 * kHuffChunk : kHuffChunk);  // first chunk is the longest
+    int64_t wi = c < chunks ? (int64_t)offs[c] : 0;
+    unsigned long long buf = 0ull;
+    int nb = 0;
+    for (int r = 0; r < m_cta; r += kHuffDecRound) {
+        const int cnt = m - r;
+#pragma unroll 1
+        for (int g = 0; g < kHuffDecRound / 4; ++g) {
+            uint32_t acc = 0u;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                if (g * 4 + k < cnt) {
+                    const uint32_t sym = max_len == 0 ? s.symbols[0] : huff_decode_one(s, max_len, words, num_words, wi, buf, nb);
+                    acc |= (sym & 0xffu) << (8 * k);
+                }
+            }
+            s.stage[threadIdx.x * kHuffStageStride + g] = acc;
+        }
+        __syncthreads();
+#pragma unroll 2
+        for (int i = threadIdx.x; i < kHuffDecThreads * (kHuffDecRound / 4); i += kHuffDecThreads) {
+            const int cl = i / (kHuffDecRound / 4), part = i % (kHuffDecRound / 4);
+            const int64_t e = (c0 + cl) * kHuffChunk + r + part * 4;
+            if (c0 + cl >= chunks || e >= n || r + part * 4 >= kHuffChunk) continue;
+            const uint32_t codes = s.stage[cl * kHuffStageStride + part];
+            if (qvec && e + 4 <= n && (single_row || L % 4 == 0)) {
+                const int64_t row = single_row ? 0 : e / L;
+                const float a = __ldg(alpha + row), b = __ldg(beta + row);
+                st_stream4(q + e, make_float4(from_unit(s.unit[codes & 0xffu], a, b), from_unit(s.unit[(codes >> 8) & 0xffu], a, b),
+                                              from_unit(s.unit[(codes >> 16) & 0xffu], a, b), from_unit(s.unit[codes >> 24], a, b)));
+            } else {
+                for (int j = 0; j < 4 && e + j < n; ++j) {
+                    const int64_t row = single_row ? 0 : (e + j) / L;
+                    q[e + j] = from_unit(s.unit[(codes >> (8 * j)) & 0xffu], __ldg(alpha + row), __ldg(beta + row));
+                }
+            }
+        }
+        __syncthreads();
+    }
+}
+
+// one tensor: a grid-stride loop over its chunks, kHuffDecThreads chunks per CTA step
+template <bool UNIFORM>
+__global__ void __launch_bounds__(kHuffDecThreads) huff_decode_dequant_kernel(
+    const uint32_t* __restrict__ words, int64_t num_words, const uint32_t* __restrict__ offs,
+    const qd_huffman_table* __restrict__ tab, const float* __restrict__ points, int K, const float* __restrict__ alpha,
+    const float* __restrict__ beta, float* __restrict__ q, Geometry geo, float S, int64_t chunks) {
+    __shared__ HuffDecodeShared s;
+    huff_load_tables<UNIFORM>(s, tab, S, points, K);
     const int max_len = (int)tab->max_length;
     __syncthreads();
-    const int64_t n = geo.n, L = geo.row_len;
-    const bool single_row = geo.rows == 1;
-    const bool qvec = (reinterpret_cast<uintptr_t>(q) & 15) == 0;
-    for (int64_t c0 = (int64_t)blockIdx.x * kHuffDecThreads; c0 < chunks; c0 += (int64_t)gridDim.x * kHuffDecThreads) {
-        const int64_t c = c0 + threadIdx.x;
-        const int64_t e0 = c * kHuffChunk;
-        const int m = c < chunks ? (int)(n - e0 < kHuffChunk ? n - e0 : kHuffChunk) : 0;
-        const int m_cta = (int)(n - c0 * kHuffChunk < kHuffChunk ? n - c0 * kHuffChunk : kHuffChunk);  // first chunk is the longest
-        int64_t wi = c < chunks ? (int64_t)offs[c] : 0;
-        unsigned long long buf = 0ull;
-        int nb = 0;
-        for (int r = 0; r < m_cta; r += kHuffDecRound) {
-            const int cnt = m - r;
-#pragma unroll 1
-            for (int g = 0; g < kHuffDecRound / 4; ++g) {
-                uint32_t acc = 0u;
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    if (g * 4 + k < cnt) {
-                        const uint32_t sym = max_len == 0 ? s.symbols[0] : huff_decode_one(s, max_len, words, num_words, wi, buf, nb);
-                        acc |= (sym & 0xffu) << (8 * k);
-                    }
-                }
-                s.stage[threadIdx.x * kHuffStageStride + g] = acc;
-            }
-            __syncthreads();
-#pragma unroll 2
-            for (int i = threadIdx.x; i < kHuffDecThreads * (kHuffDecRound / 4); i += kHuffDecThreads) {
-                const int cl = i / (kHuffDecRound / 4), part = i % (kHuffDecRound / 4);
-                const int64_t e = (c0 + cl) * kHuffChunk + r + part * 4;
-                if (c0 + cl >= chunks || e >= n || r + part * 4 >= kHuffChunk) continue;
-                const uint32_t codes = s.stage[cl * kHuffStageStride + part];
-                if (qvec && e + 4 <= n && (single_row || L % 4 == 0)) {
-                    const int64_t row = single_row ? 0 : e / L;
-                    const float a = __ldg(alpha + row), b = __ldg(beta + row);
-                    st_stream4(q + e, make_float4(from_unit(s.unit[codes & 0xffu], a, b), from_unit(s.unit[(codes >> 8) & 0xffu], a, b),
-                                                  from_unit(s.unit[(codes >> 16) & 0xffu], a, b), from_unit(s.unit[codes >> 24], a, b)));
-                } else {
-                    for (int j = 0; j < 4 && e + j < n; ++j) {
-                        const int64_t row = single_row ? 0 : (e + j) / L;
-                        q[e + j] = from_unit(s.unit[(codes >> (8 * j)) & 0xffu], __ldg(alpha + row), __ldg(beta + row));
-                    }
-                }
-            }
-            __syncthreads();
-        }
+    for (int64_t c0 = (int64_t)blockIdx.x * kHuffDecThreads; c0 < chunks; c0 += (int64_t)gridDim.x * kHuffDecThreads)
+        huff_decode_chunks(s, max_len, words, num_words, offs, alpha, beta, q, geo.n, geo.row_len, geo.rows == 1, chunks, c0);
+}
+
+// A whole model in one launch.  Tensor t owns CTAs [cta_start[t], cta_start[t + 1]), ceil(chunks_t / kHuffDecThreads)
+// of them, so every CTA serves one tensor (found by binary search) and loads that tensor's unit table once.  The
+// tensor's fields live in registers rather than kernel parameters: 10 CTAs per SM (<= 51 registers) keep them without
+// spills, where ptxas's default budget for 128 threads (40) spills.
+template <bool UNIFORM>
+__global__ void __launch_bounds__(kHuffDecThreads, 10) huff_decode_dequant_model_kernel(
+    const qd_huffman_tensor* __restrict__ tensors, const int32_t* __restrict__ cta_start, int count,
+    const qd_huffman_table* __restrict__ tab, int64_t bucket, float S) {
+    __shared__ HuffDecodeShared s;
+    const int b = (int)blockIdx.x;
+    int lo = 0, hi = count;                       // cta_start[lo] <= b < cta_start[hi]
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(cta_start + mid) <= b) lo = mid;
+        else hi = mid;
     }
+    const qd_huffman_tensor& t = tensors[lo];
+    huff_load_tables<UNIFORM>(s, tab, S, t.points, t.num_points);
+    const int max_len = (int)tab->max_length;
+    __syncthreads();
+    const int64_t n = t.n;
+    const int64_t L = (bucket == 0 || n < bucket) ? n : bucket;   // geometry_of; one row exactly when L == n
+    const int64_t chunks = (n + kHuffChunk - 1) / kHuffChunk;
+    huff_decode_chunks(s, max_len, t.words, t.num_words, t.chunk_offsets, t.alpha, t.beta, t.q, n, L, L == n, chunks,
+                       (int64_t)(b - __ldg(cta_start + lo)) * kHuffDecThreads);
 }
 
 }  // namespace qd
