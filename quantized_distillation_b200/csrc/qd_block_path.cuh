@@ -93,7 +93,7 @@ __device__ __forceinline__ double cta_sum(double v, double* scratch) {
 // row, the whole-row staging above that, up to the 49152-float shared-memory limit.
 constexpr int kStagedMaxRow = QD_MAX_STAGED_BUCKET;  // floats; longer rows would use the L2 re-read variant
 constexpr int kWarpTwoPassMaxRow = 2048;  // floats; rows up to here: one WARP per row, two passes (second from L1/L2)
-constexpr int kWarp2MinmaxMaxRow = 2048;  // floats; the min/max backward takes the two-pass variant up to here (qd_api.cu)
+constexpr int kWarp2MinmaxMaxRow = 2048;  // floats; the min/max backward takes the two-pass variant up to here (qd_quant.cu)
 
 // GROUP = 32: a warp owns the row (no block barriers at all, dozens of rows in flight per SM);
 // GROUP = kBlockCtaThreads: the whole CTA owns the row.

@@ -1,0 +1,386 @@
+// qd_codec.cu -- stored-model codecs: histogram of level indices, fixed-width 1/2/4/8-bit packing and its fused
+// unpack + dequantization, and the Huffman-coded stream (qd_huffman.cuh) per tensor and per model.
+#include <cstring>
+#include <vector>
+
+#include "qd_huffman.cuh"
+#include "qd_launch.h"
+
+using namespace qd;
+
+// Calls f(std::integral_constant<int, BITS>{}) for a code width `bits` already checked to be 1, 2, 4 or 8.
+template <class F>
+static void with_bits(int bits, F&& f) {
+    if (bits == 8) f(std::integral_constant<int, 8>{});
+    else if (bits == 4) f(std::integral_constant<int, 4>{});
+    else if (bits == 2) f(std::integral_constant<int, 2>{});
+    else f(std::integral_constant<int, 1>{});
+}
+
+static bool bits_ok(int bits) { return bits == 1 || bits == 2 || bits == 4 || bits == 8; }
+
+// ------------------------------------------------------------------ f2: histogram of indices
+__global__ void __launch_bounds__(256) index_histogram_kernel(const uint8_t* __restrict__ idx, int64_t n, int bins,
+                                                             unsigned long long* __restrict__ counts) {
+    __shared__ unsigned int s_h[8][256];
+    for (int i = threadIdx.x; i < 8 * 256; i += 256) (&s_h[0][0])[i] = 0u;
+    __syncthreads();
+    unsigned int* h = s_h[threadIdx.x >> 5];
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    const bool vec = (reinterpret_cast<uintptr_t>(idx) & 15) == 0;
+    const int64_t nv = vec ? (n >> 4) : 0;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += stride) {
+        uint4 w = reinterpret_cast<const uint4*>(idx)[i];
+        unsigned int ws[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+        for (int a = 0; a < 4; ++a)
+#pragma unroll
+            for (int b = 0; b < 4; ++b) atomicAdd(&h[(ws[a] >> (8 * b)) & 0xffu], 1u);
+    }
+    for (int64_t i = nv * 16 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) atomicAdd(&h[idx[i]], 1u);
+    __syncthreads();
+    for (int b = threadIdx.x; b < bins; b += 256) {
+        unsigned long long s = 0;
+        for (int w = 0; w < 8; ++w) s += s_h[w][b];
+        if (s) atomicAdd(&counts[b], s);
+    }
+}
+
+extern "C" int qd_index_histogram(const uint8_t* idx_u8, int64_t n, int num_bins, int64_t* counts, qd_stream_t stream) {
+    if (idx_u8 == nullptr || counts == nullptr || n <= 0) return fail(QD_ERR_INVALID_ARG, "NULL argument or n <= 0");
+    if (num_bins < 1 || num_bins > 256) return fail(QD_ERR_INVALID_ARG, "num_bins must be in [1, 256]");
+    int grid;
+    int rc = capped_grid((n / 16 + 255) / 256 + 1, 4, &grid);
+    if (rc) return rc;
+    index_histogram_kernel<<<grid, 256, 0, as_stream(stream)>>>(idx_u8, n, num_bins, reinterpret_cast<unsigned long long*>(counts));
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+// ------------------------------------------------------------------ f2: packed codec
+// one thread-group = 16 consecutive codes in (one 128-bit load), 2*BITS bytes out (one store of that width); BITS is a
+// template parameter so that every shift, mask and access width is a compile-time constant
+template <int BITS>
+__device__ __forceinline__ uint32_t squeeze4(uint32_t w) {  // four codes in four bytes -> 4*BITS bits
+    constexpr unsigned mask = (1u << BITS) - 1u;
+    return (w & mask) | (((w >> 8) & mask) << BITS) | (((w >> 16) & mask) << (2 * BITS)) | (((w >> 24) & mask) << (3 * BITS));
+}
+
+template <int BITS>
+__global__ void __launch_bounds__(256) pack_kernel(const uint8_t* __restrict__ idx, uint8_t* __restrict__ packed, int64_t n) {
+    const int64_t groups = (n + 15) / 16;
+    const int64_t full = n / 16;   // groups with all sixteen codes present
+    const int64_t tiles = (groups + kTileGroups - 1) / kTileGroups;
+    const int64_t out_bytes = (n * BITS + 7) / 8;
+    const bool in_vec = (reinterpret_cast<uintptr_t>(idx) & 15) == 0;
+    const bool out_vec = (reinterpret_cast<uintptr_t>(packed) & 15) == 0;
+    for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int64_t g0 = tile * kTileGroups + threadIdx.x;
+        uint4 c[kTileU];
+#pragma unroll
+        for (int u = 0; u < kTileU; ++u) {
+            const int64_t g = g0 + u * 256;
+            if (in_vec && g < full) {
+                c[u] = __ldcs(reinterpret_cast<const uint4*>(idx) + g);
+            } else {
+                uint32_t w[4] = {0u, 0u, 0u, 0u};
+                if (g < groups)
+                    for (int j = 0; j < 16; ++j)
+                        if (g * 16 + j < n) w[j >> 2] |= (uint32_t)idx[g * 16 + j] << (8 * (j & 3));
+                c[u] = make_uint4(w[0], w[1], w[2], w[3]);
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < kTileU; ++u) {
+            const int64_t g = g0 + u * 256;
+            if (g >= groups) continue;
+            // 16*BITS output bits, low codes first, as two 64-bit halves (the second one is only used for BITS = 8)
+            unsigned long long lo, hi = 0;
+            if constexpr (BITS == 8) {
+                lo = (unsigned long long)c[u].x | ((unsigned long long)c[u].y << 32);
+                hi = (unsigned long long)c[u].z | ((unsigned long long)c[u].w << 32);
+            } else {
+                lo = (unsigned long long)squeeze4<BITS>(c[u].x) | ((unsigned long long)squeeze4<BITS>(c[u].y) << (4 * BITS)) |
+                     ((unsigned long long)squeeze4<BITS>(c[u].z) << (8 * BITS)) | ((unsigned long long)squeeze4<BITS>(c[u].w) << (12 * BITS));
+            }
+            uint8_t* dst = packed + g * (2 * BITS);
+            if (out_vec && g < full) {
+                if constexpr (BITS == 8) __stcs(reinterpret_cast<uint4*>(dst), make_uint4((uint32_t)lo, (uint32_t)(lo >> 32), (uint32_t)hi, (uint32_t)(hi >> 32)));
+                else if constexpr (BITS == 4) __stcs(reinterpret_cast<unsigned long long*>(dst), lo);
+                else if constexpr (BITS == 2) __stcs(reinterpret_cast<uint32_t*>(dst), (uint32_t)lo);
+                else __stcs(reinterpret_cast<uint16_t*>(dst), (uint16_t)lo);
+            } else {
+                for (int b = 0; b < 2 * BITS; ++b)
+                    if (g * (2 * BITS) + b < out_bytes) dst[b] = (uint8_t)((b < 8 ? lo >> (8 * b) : hi >> (8 * (b - 8))));
+            }
+        }
+    }
+}
+
+extern "C" int qd_pack_indices(const uint8_t* idx_u8, uint8_t* packed, int64_t n, int bits, qd_stream_t stream) {
+    if (idx_u8 == nullptr || packed == nullptr || n <= 0) return fail(QD_ERR_INVALID_ARG, "NULL argument or n <= 0");
+    if (!bits_ok(bits)) return fail(QD_ERR_INVALID_ARG, "bits must be 1, 2, 4 or 8");
+    int grid;
+    int rc = capped_grid(((n + 15) / 16 + kTileGroups - 1) / kTileGroups, 8, &grid);
+    if (rc) return rc;
+    with_bits(bits, [&](auto b) { pack_kernel<b><<<grid, 256, 0, as_stream(stream)>>>(idx_u8, packed, n); });
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+// one thread-group = FOUR consecutive elements: their codes are one aligned load of 4*BITS bits (a nibble for BITS = 1),
+// the four dequantized values leave as one 128-bit store (a warp writes 512 contiguous bytes).  The unit value of a
+// code comes from a 256-entry table in shared memory: c/S for the uniform scheme (the reference's division, done once
+// per code instead of once per element), the centroid for the non-uniform one.
+template <int BITS>
+__device__ __forceinline__ uint32_t load_codes4(const uint8_t* __restrict__ packed, int64_t e0, int64_t in_bytes, bool ivec) {
+    if constexpr (BITS == 8) {
+        if (ivec && e0 + 4 <= in_bytes) return __ldcs(reinterpret_cast<const uint32_t*>(packed + e0));
+        uint32_t word = 0;
+        for (int b = 0; b < 4; ++b)
+            if (e0 + b < in_bytes) word |= (uint32_t)packed[e0 + b] << (8 * b);
+        return word;
+    } else if constexpr (BITS == 4) {
+        const int64_t b0 = e0 >> 1;
+        if (ivec && b0 + 2 <= in_bytes) return __ldcs(reinterpret_cast<const uint16_t*>(packed + b0));
+        uint32_t word = packed[b0];
+        if (b0 + 1 < in_bytes) word |= (uint32_t)packed[b0 + 1] << 8;
+        return word;
+    } else if constexpr (BITS == 2) {
+        return packed[e0 >> 2];
+    } else {
+        return (uint32_t)packed[e0 >> 3] >> (unsigned)(e0 & 4);
+    }
+}
+
+// codes of group g (four elements) when the packed pointer is 4-byte aligned and the group is complete
+template <int BITS>
+__device__ __forceinline__ uint32_t load_codes4_fast(const uint8_t* __restrict__ packed, int64_t g) {
+    if constexpr (BITS == 8) return __ldcs(reinterpret_cast<const uint32_t*>(packed) + g);
+    else if constexpr (BITS == 4) return __ldcs(reinterpret_cast<const uint16_t*>(packed) + g);
+    else if constexpr (BITS == 2) return __ldcs(packed + g);
+    else return (uint32_t)__ldcs(packed + (g >> 1)) >> (unsigned)((g & 1) * 4);
+}
+
+template <bool UNIFORM, int BITS>
+__global__ void __launch_bounds__(256, 4) unpack_dequant_kernel(const uint8_t* __restrict__ packed,
+                                                            const float* __restrict__ points, int K,
+                                                            const float* __restrict__ alpha, const float* __restrict__ beta,
+                                                            float* __restrict__ q, Geometry geo, float S) {
+    __shared__ float s_unit[256];
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) {
+        if (UNIFORM) s_unit[i] = ((float)i <= S) ? level_to_unit((float)i, S) : 0.f;
+        else s_unit[i] = (i < K) ? points[i] : 0.f;
+    }
+    __syncthreads();
+    const int64_t L = geo.row_len;
+    const int64_t groups = (geo.n + 3) / 4;
+    constexpr unsigned mask = (1u << BITS) - 1u;
+    const bool single = geo.rows == 1;
+    // fast tiles: complete tiles of kTileGroups groups, aligned pointers, the four elements of a group in one row, and
+    // a row cursor that fits 32 bits (rows x row length beyond that only exist for buckets of < 32 floats on > 8 G
+    // elements; they take the general loop below)
+    const bool fast_ok = ((reinterpret_cast<uintptr_t>(q) & 15) == 0) && ((reinterpret_cast<uintptr_t>(packed) & 3) == 0) &&
+                         (single || (L % 4 == 0 && L < (1ll << 30) && geo.rows < (1ll << 31)));
+    const int64_t full_tiles = fast_ok ? geo.n / (kTileGroups * 4) : 0;
+    if (full_tiles > (int64_t)blockIdx.x) {
+        const uint32_t L32 = single ? 1u : (uint32_t)L;
+        const int64_t e_first = ((int64_t)blockIdx.x * kTileGroups + threadIdx.x) * 4;
+        int row = single ? 0 : (int)(e_first / L);
+        uint32_t rem = single ? 0u : (uint32_t)(e_first % L);
+        const int du_rows = single ? 0 : (int)((256 * 4) / L);
+        const uint32_t du_rem = single ? 0u : (uint32_t)((256 * 4) % L);
+        const int64_t dt = (int64_t)gridDim.x * kTileGroups * 4;
+        const int dt_rows = single ? 0 : (int)(dt / L);
+        const uint32_t dt_rem = single ? 0u : (uint32_t)(dt % L);
+        // Everything a tile READS (codes, alpha, beta of its kTileU groups) is fetched one tile ahead: the stores of a
+        // tile are asm volatile (no load moves across them), and under a store-dominated stream a read round trip is
+        // several microseconds -- without the prefetch every group of four stores waited for its own alpha/beta read.
+        struct Fetched { uint32_t w[kTileU]; float a[kTileU], b[kTileU]; };
+        auto fetch = [&](int64_t tile, int r, uint32_t m, Fetched& f) {
+            const int64_t g0 = tile * kTileGroups + threadIdx.x;
+#pragma unroll
+            for (int u = 0; u < kTileU; ++u) f.w[u] = load_codes4_fast<BITS>(packed, g0 + u * 256);
+#pragma unroll
+            for (int u = 0; u < kTileU; ++u) {
+                f.a[u] = __ldg(alpha + r);
+                f.b[u] = __ldg(beta + r);
+                r += du_rows;
+                m += du_rem;
+                if (m >= L32) { m -= L32; ++r; }
+            }
+        };
+        Fetched cur;
+        fetch(blockIdx.x, row, rem, cur);
+        for (int64_t tile = blockIdx.x; tile < full_tiles; tile += gridDim.x) {
+            Fetched nxt = cur;
+            row += dt_rows;
+            rem += dt_rem;
+            if (rem >= L32) { rem -= L32; ++row; }
+            if (tile + gridDim.x < full_tiles) fetch(tile + gridDim.x, row, rem, nxt);
+            float* dst = q + (tile * kTileGroups + threadIdx.x) * 4;
+#pragma unroll
+            for (int u = 0; u < kTileU; ++u) {
+                float o[4];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) o[j] = from_unit(s_unit[(cur.w[u] >> (j * BITS)) & mask], cur.a[u], cur.b[u]);
+                st_stream4(dst + u * 1024, make_float4(o[0], o[1], o[2], o[3]));
+            }
+            cur = nxt;
+        }
+    }
+    // general loop: the last partial tile, unaligned pointers, ragged buckets
+    const int64_t in_bytes = (geo.n * BITS + 7) / 8;
+    const bool ivec = (reinterpret_cast<uintptr_t>(packed) & 3) == 0;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t g = full_tiles * kTileGroups + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += stride) {
+        const int64_t e0 = g * 4;
+        const uint32_t w = load_codes4<BITS>(packed, e0, in_bytes, ivec);
+        for (int j = 0; j < 4; ++j) {
+            if (e0 + j >= geo.n) break;
+            const int64_t r = single ? 0 : (e0 + j) / L;
+            q[e0 + j] = from_unit(s_unit[(w >> (j * BITS)) & mask], alpha[r], beta[r]);
+        }
+    }
+}
+
+// Checks the arguments both unpacks share and launches unpack_dequant_kernel<UNIFORM, bits>.
+template <bool UNIFORM>
+static int unpack_dequant(const uint8_t* packed, int bits, const float* points, int K, const float* alpha, const float* beta,
+                          float* q, int64_t n, int64_t bucket, float S, qd_stream_t stream) {
+    Geometry geo;
+    if (packed == nullptr || alpha == nullptr || beta == nullptr || q == nullptr) return fail(QD_ERR_INVALID_ARG, "NULL argument");
+    if (!bits_ok(bits)) return fail(QD_ERR_INVALID_ARG, "bits must be 1, 2, 4 or 8");
+    if (geometry_of(n, bucket, &geo)) return fail(QD_ERR_INVALID_ARG, "bad geometry");
+    int grid;   // one resident wave (__launch_bounds__(256, 4))
+    int rc = capped_grid(((n + 3) / 4 + kTileGroups - 1) / kTileGroups, 4, &grid);
+    if (rc) return rc;
+    with_bits(bits, [&](auto b) {
+        unpack_dequant_kernel<UNIFORM, b><<<grid, 256, 0, as_stream(stream)>>>(packed, points, K, alpha, beta, q, geo, S);
+    });
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+extern "C" int qd_unpack_dequant_uniform(const uint8_t* packed, int bits, const float* alpha, const float* beta, float* q,
+                                         int64_t n, int64_t bucket, int levels, qd_stream_t stream) {
+    if (levels < 2 || levels > (1 << bits)) return fail(QD_ERR_INVALID_ARG, "levels must be in [2, 2^bits]");
+    return unpack_dequant<true>(packed, bits, nullptr, 0, alpha, beta, q, n, bucket, (float)(levels - 1), stream);
+}
+
+extern "C" int qd_unpack_dequant_nonuniform(const uint8_t* packed, int bits, const float* points, int num_points,
+                                            const float* alpha, const float* beta, float* q, int64_t n, int64_t bucket,
+                                            qd_stream_t stream) {
+    if (points == nullptr || num_points < 1 || num_points > (1 << bits)) return fail(QD_ERR_INVALID_ARG, "num_points must be in [1, 2^bits]");
+    return unpack_dequant<false>(packed, bits, points, num_points, alpha, beta, q, n, bucket, 0.f, stream);
+}
+
+// ------------------------------------------------------------------ f2: Huffman-coded storage (qd_huffman.cuh)
+extern "C" int qd_huffman_encode(const uint8_t* idx_u8, int64_t n, const qd_huffman_table* table, uint32_t* words_out,
+                                 int64_t words_capacity, uint32_t* chunk_offsets, uint64_t* total_words, qd_stream_t stream) {
+    if (idx_u8 == nullptr || table == nullptr || chunk_offsets == nullptr || total_words == nullptr || n <= 0)
+        return fail(QD_ERR_INVALID_ARG, "NULL argument or n <= 0");
+    if (words_capacity < 0 || (words_capacity > 0 && words_out == nullptr)) return fail(QD_ERR_INVALID_ARG, "bad words_out / capacity");
+    DevInfo* di;
+    int rc = dev_info(&di);
+    if (rc) return rc;
+    cudaStream_t s = as_stream(stream);
+    const int64_t chunks = (n + kHuffChunk - 1) / kHuffChunk;
+    huff_chunk_words_kernel<<<di->grid((chunks + 7) / 8, 8), 256, 0, s>>>(idx_u8, n, table, chunk_offsets, chunks);
+    huff_scan_kernel<<<1, 1024, 0, s>>>(chunk_offsets, chunks, reinterpret_cast<unsigned long long*>(total_words));
+    if (words_capacity > 0)
+        huff_encode_kernel<<<di->grid((chunks + kHuffEncWarps - 1) / kHuffEncWarps, 8), kHuffEncWarps * 32, 0, s>>>(
+            idx_u8, n, table, chunk_offsets, reinterpret_cast<const unsigned long long*>(total_words), chunks, words_out, words_capacity);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+// Checks the arguments both per-tensor decodes share and launches huff_decode_dequant_kernel<UNIFORM>.
+template <bool UNIFORM>
+static int huff_decode_dequant(const uint32_t* words, int64_t num_words, const uint32_t* chunk_offsets, const qd_huffman_table* table,
+                               const float* points, int K, const float* alpha, const float* beta, float* q, int64_t n,
+                               int64_t bucket, float S, qd_stream_t stream) {
+    Geometry geo;
+    if (chunk_offsets == nullptr || table == nullptr || alpha == nullptr || beta == nullptr || q == nullptr)
+        return fail(QD_ERR_INVALID_ARG, "NULL argument");
+    if (num_words < 0 || (num_words > 0 && words == nullptr)) return fail(QD_ERR_INVALID_ARG, "bad words / num_words");
+    if (geometry_of(n, bucket, &geo)) return fail(QD_ERR_INVALID_ARG, "bad geometry");
+    const int64_t chunks = (n + kHuffChunk - 1) / kHuffChunk;
+    int grid;
+    int rc = capped_grid((chunks + kHuffDecThreads - 1) / kHuffDecThreads, 16, &grid);
+    if (rc) return rc;
+    huff_decode_dequant_kernel<UNIFORM><<<grid, kHuffDecThreads, 0, as_stream(stream)>>>(
+        words, num_words, chunk_offsets, table, points, K, alpha, beta, q, geo, S, chunks);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+extern "C" int qd_huffman_decode_dequant_uniform(const uint32_t* words, int64_t num_words, const uint32_t* chunk_offsets,
+                                                 const qd_huffman_table* table, const float* alpha, const float* beta, float* q,
+                                                 int64_t n, int64_t bucket, int levels, qd_stream_t stream) {
+    if (levels < 2 || levels > 256) return fail(QD_ERR_INVALID_ARG, "levels must be in [2, 256]");
+    return huff_decode_dequant<true>(words, num_words, chunk_offsets, table, nullptr, 0, alpha, beta, q, n, bucket,
+                                     (float)(levels - 1), stream);
+}
+
+extern "C" int qd_huffman_decode_dequant_nonuniform(const uint32_t* words, int64_t num_words, const uint32_t* chunk_offsets,
+                                                    const qd_huffman_table* table, const float* points, int num_points,
+                                                    const float* alpha, const float* beta, float* q, int64_t n, int64_t bucket,
+                                                    qd_stream_t stream) {
+    if (points == nullptr || num_points < 1 || num_points > 256) return fail(QD_ERR_INVALID_ARG, "num_points must be in [1, 256]");
+    return huff_decode_dequant<false>(words, num_words, chunk_offsets, table, points, num_points, alpha, beta, q, n, bucket, 0.f,
+                                      stream);
+}
+
+// workspace of the model decode: the tensor array, then cta_start[count + 1] (int32)
+static_assert(sizeof(qd_huffman_tensor) == 72 && sizeof(qd_huffman_tensor) % alignof(int32_t) == 0,
+              "qd_huffman_tensor layout is shared with codec.py");
+
+extern "C" size_t qd_huffman_model_workspace_bytes(int count) {
+    return count < 1 ? 0 : (size_t)count * sizeof(qd_huffman_tensor) + ((size_t)count + 1) * sizeof(int32_t);
+}
+
+extern "C" int qd_huffman_decode_dequant_model(const qd_huffman_tensor* tensors, int count, const qd_huffman_table* table,
+                                               int64_t bucket, int levels, void* workspace, size_t workspace_bytes,
+                                               qd_stream_t stream) {
+    if (tensors == nullptr || count < 1 || table == nullptr) return fail(QD_ERR_INVALID_ARG, "NULL tensors / table or count < 1");
+    if (bucket < 0) return fail(QD_ERR_INVALID_ARG, "bucket must be >= 0");
+    if (levels != 0 && (levels < 2 || levels > 256)) return fail(QD_ERR_INVALID_ARG, "levels must be in [2, 256] (uniform) or 0 (non-uniform)");
+    const size_t need = qd_huffman_model_workspace_bytes(count);
+    if (workspace == nullptr || (reinterpret_cast<uintptr_t>(workspace) & 15) || workspace_bytes < need)
+        return fail(QD_ERR_WORKSPACE, "workspace must be 16-byte aligned and hold %zu bytes (got %zu)", need, workspace_bytes);
+    const bool uniform = levels != 0;
+    // host image of the workspace, consumed by the pageable copy before it returns (kept per thread: no allocation once grown)
+    thread_local std::vector<unsigned char> image;
+    image.resize(need);
+    int32_t* cta_start = reinterpret_cast<int32_t*>(image.data() + (size_t)count * sizeof(qd_huffman_tensor));
+    int64_t ctas = 0;
+    for (int i = 0; i < count; ++i) {
+        const qd_huffman_tensor& t = tensors[i];
+        if (t.chunk_offsets == nullptr || t.alpha == nullptr || t.beta == nullptr || t.q == nullptr)
+            return fail(QD_ERR_INVALID_ARG, "tensor %d: NULL argument", i);
+        if (t.num_words < 0 || (t.num_words > 0 && t.words == nullptr)) return fail(QD_ERR_INVALID_ARG, "tensor %d: bad words / num_words", i);
+        if (t.n < 1) return fail(QD_ERR_INVALID_ARG, "tensor %d: n must be >= 1", i);
+        if (t.reserved != 0) return fail(QD_ERR_INVALID_ARG, "tensor %d: reserved must be 0", i);
+        if (uniform && (t.points != nullptr || t.num_points != 0))
+            return fail(QD_ERR_INVALID_ARG, "tensor %d: a uniform model has no points (points NULL, num_points 0)", i);
+        if (!uniform && (t.points == nullptr || t.num_points < 1 || t.num_points > 256))
+            return fail(QD_ERR_INVALID_ARG, "tensor %d: num_points must be in [1, 256]", i);
+        cta_start[i] = (int32_t)ctas;
+        ctas += ((t.n + kHuffChunk - 1) / kHuffChunk + kHuffDecThreads - 1) / kHuffDecThreads;
+        if (ctas > INT32_MAX) return fail(QD_ERR_INVALID_ARG, "the model has more than 2^31 - 1 blocks of %d chunks", kHuffDecThreads);
+    }
+    cta_start[count] = (int32_t)ctas;
+    memcpy(image.data(), tensors, (size_t)count * sizeof(qd_huffman_tensor));
+    cudaStream_t st = as_stream(stream);
+    QD_CUDA(cudaMemcpyAsync(workspace, image.data(), need, cudaMemcpyHostToDevice, st));
+    const qd_huffman_tensor* dev_tensors = static_cast<const qd_huffman_tensor*>(workspace);
+    const int32_t* dev_start = reinterpret_cast<const int32_t*>(static_cast<const unsigned char*>(workspace) + (size_t)count * sizeof(qd_huffman_tensor));
+    if (uniform)
+        huff_decode_dequant_model_kernel<true><<<(unsigned)ctas, kHuffDecThreads, 0, st>>>(dev_tensors, dev_start, count, table, bucket,
+                                                                                           (float)(levels - 1));
+    else
+        huff_decode_dequant_model_kernel<false><<<(unsigned)ctas, kHuffDecThreads, 0, st>>>(dev_tensors, dev_start, count, table, bucket, 0.f);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}

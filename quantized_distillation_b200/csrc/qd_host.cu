@@ -11,18 +11,10 @@
 #include <cstdlib>
 #include <mutex>
 
-#include "qd_b200.h"
+#include "qd_launch.h"
 
-// message of the calling thread (qd_last_error), defined in qd_api.cu
-extern "C" int qd_internal_fail(int code, const char* fmt, ...);
-// measurement hook (qd_debug_set_tuning): key 5 = slots, key 6 = chunk elements, key 7 = staging path (see run_host)
-extern "C" int64_t qd_internal_tuning(int key);
-
-#define QDH_CUDA(call)                                                                                   \
-    do {                                                                                                 \
-        cudaError_t e_ = (call);                                                                         \
-        if (e_ != cudaSuccess) return qd_internal_fail(QD_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(e_)); \
-    } while (0)
+using qd::fail;
+using qd::tuning;
 
 namespace {
 
@@ -73,14 +65,14 @@ int ensure_ctx(int device, int slots, int64_t chunk_elems, HostCtx** out) {
         c.chunk_cap = 0;
         for (int i = 0; i < slots; ++i) {
             Slot& s = c.slot[i];
-            if (s.stream == nullptr) QDH_CUDA(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
+            if (s.stream == nullptr) QD_CUDA(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
             const size_t bytes = (size_t)chunk_elems * sizeof(float);
-            QDH_CUDA(cudaMalloc(&s.x, bytes));
-            QDH_CUDA(cudaMalloc(&s.g, bytes));
-            QDH_CUDA(cudaMalloc(&s.q, bytes));
-            QDH_CUDA(cudaMalloc(&s.gout, bytes));
+            QD_CUDA(cudaMalloc(&s.x, bytes));
+            QD_CUDA(cudaMalloc(&s.g, bytes));
+            QD_CUDA(cudaMalloc(&s.q, bytes));
+            QD_CUDA(cudaMalloc(&s.gout, bytes));
             s.ws_bytes = qd_workspace_bytes(chunk_elems, 0);
-            QDH_CUDA(cudaMalloc(&s.ws, s.ws_bytes));
+            QD_CUDA(cudaMalloc(&s.ws, s.ws_bytes));
         }
         c.slots = slots;
         c.chunk_cap = chunk_elems;
@@ -92,15 +84,16 @@ int ensure_ctx(int device, int slots, int64_t chunk_elems, HostCtx** out) {
 int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t n, int64_t bucket, int levels, int mode,
              int device) {
     if (hx == nullptr || hq == nullptr || n <= 0 || bucket < 0)
-        return qd_internal_fail(QD_ERR_INVALID_ARG, "host entry point: NULL buffer, n <= 0 or bucket < 0 (n=%lld bucket=%lld)", (long long)n, (long long)bucket);
+        return fail(QD_ERR_INVALID_ARG, "host entry point: NULL buffer, n <= 0 or bucket < 0 (n=%lld bucket=%lld)", (long long)n, (long long)bucket);
     const bool bwd = hg != nullptr;
-    if (bwd && hgout == nullptr) return qd_internal_fail(QD_ERR_INVALID_ARG, "gout_host is NULL");
-    if (device < 0 || device >= 64) return qd_internal_fail(QD_ERR_INVALID_ARG, "device ordinal %d out of range", device);
+    if (bwd && hgout == nullptr) return fail(QD_ERR_INVALID_ARG, "gout_host is NULL");
+    if (device < 0 || device >= 64) return fail(QD_ERR_INVALID_ARG, "device ordinal %d out of range", device);
     DeviceGuard guard;
-    QDH_CUDA(cudaGetDevice(&guard.prev));
-    QDH_CUDA(cudaSetDevice(device));
+    QD_CUDA(cudaGetDevice(&guard.prev));
+    QD_CUDA(cudaSetDevice(device));
     std::lock_guard<std::mutex> lk(g_mu[device]);
-    const int64_t t_slots = qd_internal_tuning(5), t_chunk = qd_internal_tuning(6), t_path = qd_internal_tuning(7);
+    // tuning keys: 5 = slots, 6 = chunk elements, 7 = staging path (below)
+    const int64_t t_slots = tuning(5), t_chunk = tuning(6), t_path = tuning(7);
     const int n_slots = (t_slots >= 1 && t_slots <= kMaxSlots) ? (int)t_slots : kSlots;
     // Pinned (cudaHostAlloc'd / registered) host buffers are device-addressable under UVA: the kernel can read its
     // inputs and write its outputs straight over PCIe.  Such a launch moves less per direction than the copy engines
@@ -143,25 +136,25 @@ int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t 
             c->big_cap = 0;
             c->big_x = c->big_g = c->big_q = c->big_gout = nullptr;
             c->big_ws = nullptr;
-            QDH_CUDA(cudaMalloc(&c->big_x, bytes));
-            QDH_CUDA(cudaMalloc(&c->big_g, bytes));
-            QDH_CUDA(cudaMalloc(&c->big_q, bytes));
-            QDH_CUDA(cudaMalloc(&c->big_gout, bytes));
-            QDH_CUDA(cudaMalloc(&c->big_ws, c->big_ws_bytes));
+            QD_CUDA(cudaMalloc(&c->big_x, bytes));
+            QD_CUDA(cudaMalloc(&c->big_g, bytes));
+            QD_CUDA(cudaMalloc(&c->big_q, bytes));
+            QD_CUDA(cudaMalloc(&c->big_gout, bytes));
+            QD_CUDA(cudaMalloc(&c->big_ws, c->big_ws_bytes));
             c->big_cap = n;
         }
         cudaStream_t s = c->slot[0].stream;
         const size_t bytes = (size_t)n * sizeof(float);
-        QDH_CUDA(cudaMemcpyAsync(c->big_x, hx, bytes, cudaMemcpyHostToDevice, s));
-        if (bwd) QDH_CUDA(cudaMemcpyAsync(c->big_g, hg, bytes, cudaMemcpyHostToDevice, s));
+        QD_CUDA(cudaMemcpyAsync(c->big_x, hx, bytes, cudaMemcpyHostToDevice, s));
+        if (bwd) QD_CUDA(cudaMemcpyAsync(c->big_g, hg, bytes, cudaMemcpyHostToDevice, s));
         rc = bwd ? qd_uniform_fwd_bwd(c->big_x, c->big_g, c->big_q, c->big_gout, n, bucket, levels, mode, c->big_ws,
                                       c->big_ws_bytes, s)
                  : qd_uniform_fwd(c->big_x, c->big_q, nullptr, nullptr, nullptr, nullptr, nullptr, n, bucket, levels,
                                   nullptr, 0.f, 0, 0, 0, c->big_ws, c->big_ws_bytes, s);
         if (rc) return rc;
-        QDH_CUDA(cudaMemcpyAsync(hq, c->big_q, bytes, cudaMemcpyDeviceToHost, s));
-        if (bwd) QDH_CUDA(cudaMemcpyAsync(hgout, c->big_gout, bytes, cudaMemcpyDeviceToHost, s));
-        QDH_CUDA(cudaStreamSynchronize(s));
+        QD_CUDA(cudaMemcpyAsync(hq, c->big_q, bytes, cudaMemcpyDeviceToHost, s));
+        if (bwd) QD_CUDA(cudaMemcpyAsync(hgout, c->big_gout, bytes, cudaMemcpyDeviceToHost, s));
+        QD_CUDA(cudaStreamSynchronize(s));
         return QD_OK;
     }
 
@@ -178,8 +171,8 @@ int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t 
                  : qd_uniform_fwd(dev_x, dev_q, nullptr, nullptr, nullptr, nullptr, nullptr, n, bucket, levels, nullptr, 0.f, 0,
                                   0, 0, s.ws, s.ws_bytes, s.stream);
         if (rc) return rc;
-        QDH_CUDA(cudaStreamSynchronize(s.stream));
-        QDH_CUDA(cudaGetLastError());
+        QD_CUDA(cudaStreamSynchronize(s.stream));
+        QD_CUDA(cudaGetLastError());
         return QD_OK;
     }
     const int64_t rows_per_chunk = chunk_elems / row_len;
@@ -192,17 +185,17 @@ int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t 
         // a chunk shorter than the bucket must still be bucketed like the tail of the
         // full tensor: with rows >= 2 overall the tail row is "padded", never a short
         // single row -- both cases give the same min/max, so passing bucket is exact.
-        QDH_CUDA(cudaMemcpyAsync(s.x, hx + off, bytes, cudaMemcpyHostToDevice, s.stream));
-        if (bwd) QDH_CUDA(cudaMemcpyAsync(s.g, hg + off, bytes, cudaMemcpyHostToDevice, s.stream));
+        QD_CUDA(cudaMemcpyAsync(s.x, hx + off, bytes, cudaMemcpyHostToDevice, s.stream));
+        if (bwd) QD_CUDA(cudaMemcpyAsync(s.g, hg + off, bytes, cudaMemcpyHostToDevice, s.stream));
         rc = bwd ? qd_uniform_fwd_bwd(s.x, s.g, s.q, s.gout, len, bucket, levels, mode, s.ws, s.ws_bytes, s.stream)
                  : qd_uniform_fwd(s.x, s.q, nullptr, nullptr, nullptr, nullptr, nullptr, len, bucket, levels, nullptr,
                                   0.f, 0, 0, 0, s.ws, s.ws_bytes, s.stream);
         if (rc) return rc;
-        QDH_CUDA(cudaMemcpyAsync(hq + off, s.q, bytes, cudaMemcpyDeviceToHost, s.stream));
-        if (bwd) QDH_CUDA(cudaMemcpyAsync(hgout + off, s.gout, bytes, cudaMemcpyDeviceToHost, s.stream));
+        QD_CUDA(cudaMemcpyAsync(hq + off, s.q, bytes, cudaMemcpyDeviceToHost, s.stream));
+        if (bwd) QD_CUDA(cudaMemcpyAsync(hgout + off, s.gout, bytes, cudaMemcpyDeviceToHost, s.stream));
     }
-    for (int i = 0; i < n_slots; ++i) QDH_CUDA(cudaStreamSynchronize(c->slot[i].stream));
-    QDH_CUDA(cudaGetLastError());
+    for (int i = 0; i < n_slots; ++i) QD_CUDA(cudaStreamSynchronize(c->slot[i].stream));
+    QD_CUDA(cudaGetLastError());
     return QD_OK;
 }
 
@@ -214,6 +207,6 @@ extern "C" int qd_uniform_fwd_host(const float* x_host, float* q_host, int64_t n
 
 extern "C" int qd_uniform_fwd_bwd_host(const float* x_host, const float* g_host, float* q_host, float* gout_host,
                                        int64_t n, int64_t bucket, int levels, int mode, int device) {
-    if (g_host == nullptr) return qd_internal_fail(QD_ERR_INVALID_ARG, "g_host is NULL");
+    if (g_host == nullptr) return fail(QD_ERR_INVALID_ARG, "g_host is NULL");
     return run_host(x_host, g_host, q_host, gout_host, n, bucket, levels, mode, device);
 }

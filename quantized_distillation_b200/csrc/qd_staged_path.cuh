@@ -35,7 +35,7 @@ struct StagedScratch {
     double acc[2][32];   // r_b partials
 };
 
-// T threads per CTA, chosen by row length (qd_api.cu): short rows want MANY small CTAs per SM (cheap
+// T threads per CTA, chosen by row length (qd_quant.cu): short rows want MANY small CTAs per SM (cheap
 // barriers, many rows in flight), rows that fill the shared memory of an SM want one large CTA (all
 // the warps the SM can hold).  Registers are capped at 64 so that 2048 / T CTAs fit.
 template <int OP, int BWD, int STAGES, int T>

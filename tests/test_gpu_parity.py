@@ -312,7 +312,7 @@ def test_fused_fwd_bwd_capi(Q):
             N.check(N.lib().qd_uniform_bwd(N.ptr(x), N.ptr(g), N.ptr(go2), n, b, 16, mode, N.ptr(ws), ws.numel(), N.stream_ptr()))
             if mode == N.BWD_MINMAX:
                 # the fused pass and the stand-alone backward may add the terms of r_b in a different order (each uses
-                # the faster one, qd_api.cu): same positions, both inside the a5 tolerance of the oracle
+                # the faster one, qd_quant.cu): same positions, both inside the a5 tolerance of the oracle
                 ref, info = O.uniform_bwd_minmax(x.cpu().numpy(), g.cpu().numpy(), 16, b)
                 for out in (go, go2):
                     assert_minmax_gradient(out.cpu().numpy(), g.cpu().numpy(), ref, info["argmax"], info["argmin"], info["abs_sum"],

@@ -1,5 +1,5 @@
 """Registers, spills and static shared memory per kernel of libqd_b200.so as ptxas reports them (`-Xptxas -v`): compiles
-the two translation units into a scratch file (the in-tree library is not touched) and tabulates the log.  Runs
+the library's translation units into a scratch file (the in-tree library is not touched) and tabulates the log.  Runs
 without a GPU.
 
     python tools/ptxas_report.py [--out profiles/ptxas_r2.md]
