@@ -46,9 +46,11 @@ extern "C" size_t qd_workspace_bytes(int64_t n, int64_t bucket) {
 template <int OP, int BWD, int R, bool VEC>
 static int launch_warp_inst(const Params& P, cudaStream_t s) {
     auto kern = warp_rows_kernel<OP, BWD, R, VEC>;
-    int grid;
-    int rc = resident_grid((const void*)kern, kWarpCtaThreads, 0, (P.geo.rows + kWarpsPerCta - 1) / kWarpsPerCta, &grid);
-    if (rc) return rc;
+    int grid = (int)warp_rows_grid(P.geo.rows);
+    if constexpr (!kRowPerWarp<OP>) {
+        int rc = resident_grid((const void*)kern, kWarpCtaThreads, 0, (P.geo.rows + kWarpsPerCta - 1) / kWarpsPerCta, &grid);
+        if (rc) return rc;
+    }
     if constexpr (OP == OP_UNIFORM && BWD == (int)BWD_MINMAX) {
         // r_b accumulation, chosen by A/B (tools/headline_ab.py, 64 Mi floats): the fused forward+backward is faster
         // with one float64 add per element, the backward alone with the grouped lane sum.  So the variant follows the

@@ -9,9 +9,9 @@
 // (r*4+j)*32 + L, still fully coalesced.  Row reductions are shuffle
 // butterflies of NaN-propagating min / max (warp_min / warp_max, qd_common.cuh).
 //
-// The grid is persistent: min(ceil(rows / warps_per_cta), SMs * resident CTAs)
-// CTAs, each warp walking rows with a grid stride, so consecutive warps stream
-// consecutive rows.
+// Consecutive warps stream consecutive rows: the uniform op launches one warp per
+// row, the other ops a persistent grid that walks the rows with a grid stride
+// (kRowPerWarp).
 #pragma once
 #include "qd_rowops.cuh"
 
@@ -381,11 +381,18 @@ __device__ __forceinline__ void warp_process_row(const Params& P, const Centroid
     warp_compute_row<OP, AUX, R, VEC, FULL, ACC_A>(P, cen, rt, row, lane, v, gv);
 }
 
-// Forward-only ops move 8-9 B/elt and, once the divisions were gone, were limited by the
-// number of loads in flight (2 x LDG.128 per lane); they keep the NEXT row's loads in flight
-// while the current row is reduced, quantized and stored (register double buffering).
-template <int OP, int AUX>
-constexpr bool kPrefetchNextRow = (OP != OP_UNIFORM) || (AUX == (int)BWD_OFF);
+// Row order.  The uniform op (forward, every backward mode) gives every row its own warp: one CTA per 8 rows
+// (warp_rows_grid) instead of a persistent grid of SMs x resident CTAs walking the rows with a grid stride.  The
+// hardware then issues CTAs in row order as earlier ones retire, so the rows in flight stay one compact band.  On a
+// plain copy of the headline's traffic (tools/stream_ceiling.py: 64 Mi floats in rows of 256, x and g read, q and gout
+// written) that order moves 3011 GB/s against 2886 GB/s for the persistent grid at 3 CTAs per SM; 2 / 4 CTAs per SM,
+// contiguous per-CTA spans, two rows per warp and L2 evict_first hints all stay at or below 2886 (H100 80GB HBM3,
+// 700 W; DESIGN.md section 3).  The other ops keep the persistent grid and hold the NEXT row's loads in flight while
+// the current row is reduced, quantized and stored (register double buffering): the centroid op at 384 .. 768 floats
+// loses 30-80 % with one row per warp (tools/block_bench.py --small), and stats / scale / stochastic rounding were not
+// measured with it.
+template <int OP>
+constexpr bool kRowPerWarp = (OP == OP_UNIFORM);
 
 // minimum resident CTAs per SM the register allocator must allow: 256-element rows (every
 // experiment of the reference) are tuned for 4 x 8 warps per SM (<= 64 registers) in the forward-only
@@ -411,12 +418,13 @@ __global__ void __launch_bounds__(kWarpCtaThreads, kMinCtas<OP, AUX, R>) warp_ro
         __syncthreads();
         if constexpr (AUX <= 32) rt.load(cen, lane);
     }
+    // with one warp per row (kRowPerWarp) the stride only matters past the 2^31 - 1 CTAs a grid can hold
     const int64_t stride = (int64_t)gridDim.x * kWarpsPerCta;
     int64_t row = (int64_t)blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5);
     // rows [0, full_rows) are complete, 16-byte aligned rows of exactly R*128 elements
     const int64_t full_rows = (VEC && P.geo.row_len == R * 128) ? (P.geo.n / P.geo.row_len) : 0;
     if constexpr (VEC) {
-        if constexpr (kPrefetchNextRow<OP, AUX> && R <= 4) {
+        if constexpr (!kRowPerWarp<OP> && R <= 4) {
             if (row < full_rows) {
                 float v[4 * R], gv[4 * R];
                 warp_load_row<OP, AUX, R, true, true>(P, row, lane, v, gv);
@@ -437,6 +445,12 @@ __global__ void __launch_bounds__(kWarpCtaThreads, kMinCtas<OP, AUX, R>) warp_ro
         }
     }
     for (; row < P.geo.rows; row += stride) warp_process_row<OP, AUX, R, VEC, false, ACC_A>(P, cen, rt, row, lane);
+}
+
+// grid of the one-warp-per-row ops: one CTA per 8 rows
+inline int64_t warp_rows_grid(int64_t rows) {
+    const int64_t ctas = (rows + kWarpsPerCta - 1) / kWarpsPerCta;
+    return ctas < 0x7fffffff ? ctas : 0x7fffffff;
 }
 
 }  // namespace qd
