@@ -165,6 +165,37 @@ int qd_unpack_dequant_uniform(const uint8_t* packed, int bits, const float* alph
 int qd_unpack_dequant_nonuniform(const uint8_t* packed, int bits, const float* points, int num_points,
                                  const float* alpha, const float* beta, float* q, int64_t n, int64_t bucket,
                                  qd_stream_t stream);
+/* Quantize straight to packed codes: packed (ceil(n*bits/8) bytes), alpha and beta are byte-identical to
+ * qd_uniform_fwd / qd_nonuniform_fwd (uint8 levels) followed by qd_pack_indices, and no level array is written.
+ * bits in {1, 2, 4, 8} and 2^bits >= levels (num_points).  Rows of at most 1024 floats with a 16-byte aligned x, a
+ * 4-byte aligned packed and a packed row start on a whole byte (one row, or bucket*bits a multiple of 8) are packed in
+ * registers by the fake-quantization kernel itself; other layouts write uint8 levels into the workspace and pack them.
+ * workspace: qd_packed_workspace_bytes(n, bucket) bytes (required in either case). */
+size_t qd_packed_workspace_bytes(int64_t n, int64_t bucket);
+int qd_uniform_fwd_packed(const float* x, uint8_t* packed, int bits, float* alpha, float* beta, int64_t n,
+                          int64_t bucket, int levels, void* workspace, size_t workspace_bytes, qd_stream_t stream);
+int qd_nonuniform_fwd_packed(const float* x, const float* points, int num_points, int rule, uint8_t* packed, int bits,
+                             float* alpha, float* beta, int64_t n, int64_t bucket,
+                             void* workspace, size_t workspace_bytes, qd_stream_t stream);
+/* Whole model in one launch: every quantized tensor of a model at its own code width, with the model-wide levels and
+ * bucket; q of each tensor is bit-identical to qd_unpack_dequant_* on it.  The host array is validated, then copied
+ * into `workspace` (device, 16-byte aligned, >= qd_unpack_model_workspace_bytes(count) bytes, private to the stream
+ * until the launch has run) with a stream-ordered copy; the call neither allocates nor synchronises, and the host
+ * array may be reused as soon as it returns. */
+typedef struct {                 /* one quantized tensor of a model; every pointer is DEVICE memory */
+    const uint8_t* packed;       /* ceil(n*bits/8) bytes */
+    const float* alpha;          /* float32[rows] */
+    const float* beta;
+    const float* points;         /* non-uniform: this tensor's points; NULL for uniform */
+    float* q;                    /* n floats, contiguous; 4-byte alignment is enough */
+    int64_t n;                   /* >= 1 */
+    int32_t bits;                /* 1, 2, 4 or 8 */
+    int32_t num_points;          /* non-uniform: 1..2^bits; uniform: 0 */
+} qd_packed_tensor;
+size_t qd_unpack_model_workspace_bytes(int count);
+int qd_unpack_dequant_model(const qd_packed_tensor* tensors /* HOST array */, int count, int64_t bucket,
+                            int levels /* uniform: s in [2, 2^bits]; 0: non-uniform */,
+                            void* workspace, size_t workspace_bytes, qd_stream_t stream);
 
 /* ---- next row f2: Huffman-coded storage (the model helpers/functions.py:226-262 only sizes) ----------
  * Canonical code over uint8 symbols, codes of 1..QD_HUFFMAN_MAX_LENGTH bits (built on the host: codec.py).

@@ -44,6 +44,11 @@ SIGNATURES = {
     "qd_pack_indices": (C.c_int, [_p, _p, _i64, _i32, _p]),
     "qd_unpack_dequant_uniform": (C.c_int, [_p, _i32, _p, _p, _p, _i64, _i64, _i32, _p]),
     "qd_unpack_dequant_nonuniform": (C.c_int, [_p, _i32, _p, _i32, _p, _p, _p, _i64, _i64, _p]),
+    "qd_packed_workspace_bytes": (_sz, [_i64, _i64]),
+    "qd_uniform_fwd_packed": (C.c_int, [_p, _p, _i32, _p, _p, _i64, _i64, _i32, _p, _sz, _p]),
+    "qd_nonuniform_fwd_packed": (C.c_int, [_p, _p, _i32, _i32, _p, _i32, _p, _p, _i64, _i64, _p, _sz, _p]),
+    "qd_unpack_model_workspace_bytes": (_sz, [_i32]),
+    "qd_unpack_dequant_model": (C.c_int, [_p, _i32, _i64, _i32, _p, _sz, _p]),
     "qd_huffman_encode": (C.c_int, [_p, _i64, _p, _p, _i64, _p, _p, _p]),
     "qd_huffman_decode_dequant_uniform": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _i64, _i64, _i32, _p]),
     "qd_huffman_decode_dequant_nonuniform": (C.c_int, [_p, _i64, _p, _p, _p, _i32, _p, _p, _p, _i64, _i64, _p]),

@@ -549,12 +549,18 @@ def save_compressed(cm: CompressedModel, path) -> int:
     """Writes the container: magic, version, JSON header, 16-byte-aligned little-endian sections.  Returns the
     file size in bytes."""
     header, sections, data_bytes = _layout(cm)
+    return _write_container(path, FILE_MAGIC, FILE_VERSION if cm.buffers is None else FILE_VERSION_BUFFERS, header, sections,
+                            data_bytes)
+
+
+def _write_container(path, magic, version, header, sections, data_bytes) -> int:
+    """prefix (magic, version, 0, header length), the JSON header, then every (tensor, nbytes, offset) section
+    little-endian at its offset from the first 16-byte boundary after the header.  Returns the file size."""
     start = _align(_PREFIX.size + len(header))
     buf = bytearray(start + data_bytes)
-    version = FILE_VERSION if cm.buffers is None else FILE_VERSION_BUFFERS
-    buf[:_PREFIX.size] = _PREFIX.pack(FILE_MAGIC, version, 0, len(header))
+    buf[:_PREFIX.size] = _PREFIX.pack(magic, version, 0, len(header))
     buf[_PREFIX.size:_PREFIX.size + len(header)] = header
-    little = {torch.int32: "<i4", torch.float32: "<f4", torch.int64: "<i8"}
+    little = {torch.int32: "<i4", torch.float32: "<f4", torch.int64: "<i8", torch.uint8: "u1"}
     for tensor, nb, off in sections:
         buf[start + off:start + off + nb] = tensor.detach().contiguous().cpu().numpy().astype(little[tensor.dtype], copy=False).tobytes()
     with open(path, "wb") as f:
@@ -662,29 +668,7 @@ def load_compressed(path, device=None) -> CompressedModel:
                                      points=pts, code_bits=int(e.get("code_bits", 0))))
     buffers = None
     if version == FILE_VERSION_BUFFERS:
-        if not isinstance(h["buffers"], list):
-            _bad("buffers is not a list")
-        buffers, names = [], set()
-        for e in h["buffers"]:
-            try:
-                name, shape, dtype = str(e["name"]), tuple(int(d) for d in e["shape"]), e["dtype"]
-                off, nb = (int(v) for v in e["section"])
-            except (KeyError, TypeError, ValueError):
-                _bad("buffer entry without name / shape / dtype / section")
-            if dtype not in _BUFFER_DTYPES:
-                _bad(f"buffer {name}: unknown dtype {dtype!r}")
-            if any(d < 0 for d in shape):
-                _bad(f"buffer {name}: bad shape")
-            if name in names:
-                _bad(f"buffer {name} appears twice")
-            names.add(name)
-            tdtype = _BUFFER_DTYPES[dtype]
-            size = int(math.prod(shape)) * tdtype.itemsize
-            if nb != size:
-                _bad(f"buffer {name}: {nb} bytes, its shape and dtype need {size}")
-            if off < 0 or off % _ALIGN or off + nb > data_bytes:
-                _bad(f"buffer {name}: section out of range")
-            buffers.append((name, view(off, nb, tdtype, shape)))
+        buffers = _read_buffers(h["buffers"], view, data_bytes, _bad)
     cm = CompressedModel(kind, levels, bucket, code, tensors, buffers=buffers)
     cm._data = region
     if device is not None:                       # everything is validated before anything reaches the GPU
@@ -701,6 +685,424 @@ def load_compressed(path, device=None) -> CompressedModel:
             cm.buffers = [(name, move(b)) for name, b in buffers]
         cm._data = move(region)
     return cm
+
+
+def _read_buffers(entries, view, data_bytes, bad, spans=None):
+    """[(name, tensor view)] of a header's buffer entries, each checked against the data region; ``bad(msg)`` raises.
+    ``spans``: a list that receives every buffer's (offset, bytes)."""
+    if not isinstance(entries, list):
+        bad("buffers is not a list")
+    buffers, names = [], set()
+    for e in entries:
+        try:
+            name, shape, dtype = str(e["name"]), tuple(int(d) for d in e["shape"]), e["dtype"]
+            off, nb = (int(v) for v in e["section"])
+        except (KeyError, TypeError, ValueError):
+            bad("buffer entry without name / shape / dtype / section")
+        if dtype not in _BUFFER_DTYPES:
+            bad(f"buffer {name}: unknown dtype {dtype!r}")
+        if any(d < 0 for d in shape):
+            bad(f"buffer {name}: bad shape")
+        if name in names:
+            bad(f"buffer {name} appears twice")
+        names.add(name)
+        tdtype = _BUFFER_DTYPES[dtype]
+        size = int(math.prod(shape)) * tdtype.itemsize
+        if nb != size:
+            bad(f"buffer {name}: {nb} bytes, its shape and dtype need {size}")
+        if off < 0 or off % _ALIGN or off + nb > data_bytes:
+            bad(f"buffer {name}: section out of range")
+        if spans is not None:
+            spans.append((off, nb))
+        buffers.append((name, view(off, nb, tdtype, shape)))
+    return buffers
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Fixed-width model container.  Every quantized tensor is stored as its packed codes (qd_pack_indices layout, its own
+# width bits_for(levels or points)) + (alpha, beta) per bucket: the size get_size_reduction accounts for.  It decodes
+# at HBM rate in one launch (qd_unpack_dequant_model) and can be read at any bucket without a chunk index.
+PACKED_MAGIC = b"QDPACK\x00\x00"
+PACKED_VERSION = 1
+# qd_packed_tensor (include/qd_b200.h): one entry of the whole-model unpack
+_PACKED_TENSOR = np.dtype([("packed", "<u8"), ("alpha", "<u8"), ("beta", "<u8"), ("points", "<u8"), ("q", "<u8"), ("n", "<i8"),
+                           ("bits", "<i4"), ("num_points", "<i4")])
+assert _PACKED_TENSOR.itemsize == 56
+
+
+@dataclass
+class PackedEntry:
+    """One parameter of a PackedModel: packed codes + (alpha, beta) per bucket, or float32 as is."""
+    name: str
+    shape: tuple
+    bits: int = 0                       # code width of a quantized tensor: 1, 2, 4 or 8
+    packed: torch.Tensor = None         # uint8[ceil(n * bits / 8)]
+    alpha: torch.Tensor = None          # float32[rows]
+    beta: torch.Tensor = None
+    points: torch.Tensor = None         # non-uniform: this tensor's centroids
+    raw: torch.Tensor = None            # unquantized tensor (float32)
+
+    @property
+    def numel(self) -> int:
+        return int(math.prod(self.shape))
+
+    @property
+    def quantized(self) -> bool:
+        return self.raw is None
+
+
+@dataclass
+class PackedModel:
+    """A model whose quantized parameters are stored fixed-width (pack_model, load_packed)."""
+    kind: str                       # "uniform" | "nonuniform"
+    levels: object                  # uniform: s; non-uniform: None
+    bucket_size: object
+    tensors: list
+    # persistent buffers as [(name, tensor)] in state_dict() order; None: not stored
+    buffers: list = None
+    # a loaded file's data region: every section is a view into it, so it reaches a device in one copy
+    _data: torch.Tensor = field(default=None, init=False, repr=False, compare=False)
+
+    def size_breakdown(self) -> dict:
+        """Bytes of the saved file by what they hold.  code_bytes + scale_bytes is what get_size_reduction accounts
+        for, up to the round-up of each tensor's codes to whole bytes; the rest is the format and the stored buffers."""
+        header, sections, data_bytes = _packed_layout(self)
+        q = [t for t in self.tensors if t.quantized]
+        section_bytes = sum(nb for _, nb, _ in sections)
+        return {
+            "code_bytes": sum(t.packed.numel() for t in q),
+            "scale_bytes": sum((t.alpha.numel() + t.beta.numel()) * 4 for t in q),
+            "unquantized_bytes": sum(t.raw.numel() * 4 for t in self.tensors if not t.quantized),
+            "buffer_bytes": sum(b.numel() * b.element_size() for _, b in self.buffers or []),
+            "header_bytes": _PREFIX.size + len(header),
+            "alignment_bytes": _align(_PREFIX.size + len(header)) - _PREFIX.size - len(header) + data_bytes - section_bytes,
+            "file_bytes": _align(_PREFIX.size + len(header)) + data_bytes,
+        }
+
+
+def _packed_sections(t: PackedEntry):
+    return [("raw", t.raw)] if not t.quantized else [("packed", t.packed), ("alpha", t.alpha), ("beta", t.beta)]
+
+
+def _packed_layout(pm: PackedModel):
+    """(JSON header bytes, [(tensor, nbytes, offset)], data bytes); offsets are relative to the first 16-byte
+    boundary after the header, every section starts on a 16-byte boundary.  The header lists buffers only when the
+    model stores them."""
+    sections, entries, off = [], [], 0
+    for t in pm.tensors:
+        e = {"name": t.name, "shape": list(t.shape), "dtype": "float32", "quantized": t.quantized, "sections": {}}
+        if t.quantized:
+            e["bits"] = int(t.bits)
+            if t.points is not None:
+                e["points"] = [float(v) for v in t.points.detach().cpu().numpy().astype(np.float32)]
+        for name, tensor in _packed_sections(t):
+            nb = tensor.numel() * tensor.element_size()
+            e["sections"][name] = [off, nb]
+            sections.append((tensor, nb, off))
+            off = _align(off + nb)
+        entries.append(e)
+    buffers = []
+    for name, b in pm.buffers or []:
+        nb = b.numel() * b.element_size()
+        buffers.append({"name": name, "shape": list(b.shape), "dtype": _dtype_name(b), "section": [off, nb]})
+        sections.append((b, nb, off))
+        off = _align(off + nb)
+    header = {"kind": pm.kind, "levels": pm.levels, "bucket": pm.bucket_size, "tensors": entries, "data_bytes": off}
+    if pm.buffers is not None:
+        header["buffers"] = buffers
+    return json.dumps(header, separators=(",", ":")).encode("utf-8"), sections, off
+
+
+def pack_model(model, numBits=None, bucket_size=256, quantize_first_and_last_layer=True, *, points=None, rule="nearest",
+               include_buffers=False) -> PackedModel:
+    """Stores a model's quantized parameters fixed-width, one fused quantize-and-pack launch per tensor.  Parameters
+    are selected as in compress_model.  Uniform: ``numBits`` (s = 2**numBits levels, uniformQuantization), codes of
+    bits_for(s) bits.  Non-uniform: ``points`` -- one ascending list for every tensor, or one list per quantized tensor
+    (the differentiable-quantization output) -- with nonUniformQuantization's ``rule``; tensor t gets codes of
+    bits_for(K_t) bits.  ``include_buffers`` also stores the persistent buffers (float32 / int64) as they are."""
+    buffers = None
+    if include_buffers:
+        buffers = _persistent_buffers(model)
+        for _, b in buffers:
+            _dtype_name(b)
+    N.require_cuda()
+    if (numBits is None) == (points is None):
+        raise ValueError("give numBits (uniform) or points (non-uniform), not both")
+    named = list(model.named_parameters())
+    sel = _selected(named, quantize_first_and_last_layer)
+    order = [i for i in range(len(named)) if i in sel]
+    if not order:
+        raise ValueError("no parameter is selected for quantization")
+    uniform = points is None
+    if uniform:
+        s = 2 ** int(numBits)
+        if not 2 <= s <= 256:
+            raise ValueError("the packed codec stores at most 8 bits per weight: numBits must be in [1, 8]")
+    else:
+        per_tensor = len(points) > 0 and (torch.is_tensor(points[0]) or isinstance(points[0], (list, tuple, np.ndarray)))
+        pts_list = list(points) if per_tensor else [points] * len(order)
+        if len(pts_list) != len(order):
+            raise ValueError(f"{len(pts_list)} point lists for {len(order)} quantized tensors")
+        if rule not in ("nearest", "midpoint"):
+            raise ValueError(f"unknown rule {rule!r}")
+    dev = next((p.device for _, p in named if p.is_cuda), torch.device("cuda", torch.cuda.current_device()))
+    b = 0 if bucket_size is None else int(bucket_size)
+    tensors = []
+    with torch.cuda.device(dev):
+        sp = N.stream_ptr(dev)
+        ws_bytes = max(int(N.lib().qd_packed_workspace_bytes(named[i][1].numel(), b)) for i in order)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)     # stream-ordered: free to reuse once the launches ran
+        k = 0
+        for i, (name, p) in enumerate(named):
+            if i not in sel:
+                tensors.append(PackedEntry(name, tuple(p.shape), raw=p.detach().to(dev, torch.float32).contiguous().view(-1).clone()))
+                continue
+            x = p.detach().to(dev, torch.float32).contiguous().view(-1)
+            n = x.numel()
+            rows = _rows(n, bucket_size)
+            alpha = torch.empty(rows, device=dev)
+            beta = torch.empty(rows, device=dev)
+            if uniform:
+                bits, pts = bits_for(s), None
+                packed = torch.empty((n * bits + 7) // 8, dtype=torch.uint8, device=dev)
+                N.check(N.lib().qd_uniform_fwd_packed(N.ptr(x), N.ptr(packed), bits, N.ptr(alpha), N.ptr(beta), n, b, s, N.ptr(ws),
+                                                      ws.numel(), sp))
+            else:
+                pts = torch.as_tensor(pts_list[k], dtype=torch.float32).detach().to(dev).contiguous().view(-1)
+                if not 1 <= pts.numel() <= 256:
+                    raise ValueError(f"{name}: {pts.numel()} points, the packed codec stores 1 to 256")
+                bits = bits_for(pts.numel())
+                packed = torch.empty((n * bits + 7) // 8, dtype=torch.uint8, device=dev)
+                N.check(N.lib().qd_nonuniform_fwd_packed(N.ptr(x), N.ptr(pts), pts.numel(),
+                                                         N.RULE_MIDPOINT if rule == "midpoint" else N.RULE_NEAREST, N.ptr(packed), bits,
+                                                         N.ptr(alpha), N.ptr(beta), n, b, N.ptr(ws), ws.numel(), sp))
+            tensors.append(PackedEntry(name, tuple(p.shape), bits=bits, packed=packed, alpha=alpha, beta=beta, points=pts))
+            k += 1
+    return PackedModel("uniform" if uniform else "nonuniform", s if uniform else None, bucket_size, tensors,
+                       buffers=None if buffers is None else [(name, b_.detach().to(dev).clone()) for name, b_ in buffers])
+
+
+def _packed_decode_args(pm: PackedModel, items, dev, move):
+    """Arguments of one qd_unpack_dequant_model call that decodes every (quantized entry, out) of ``items`` on
+    ``dev`` (the current device); out: contiguous float32 on ``dev``.  Also returns the tensors the call reads, which
+    must outlive its enqueueing."""
+    desc = np.zeros(len(items), _PACKED_TENSOR)
+    keep = []
+    if pm.kind != "uniform":                     # every tensor's points in one upload
+        src = items[0][0].points.device
+        flat = move(torch.cat([t.points.reshape(-1).to(src, torch.float32) for t, _ in items]))
+        keep.append(flat)
+    at = 0
+    for i, (t, out) in enumerate(items):
+        packed, alpha, beta = (move(x) for x in (t.packed, t.alpha, t.beta))
+        keep += [packed, alpha, beta]
+        points, k = 0, 0
+        if pm.kind != "uniform":
+            k = t.points.numel()
+            points = flat[at:at + k].data_ptr()
+            at += k
+        desc[i] = (N.ptr(packed), N.ptr(alpha), N.ptr(beta), points, N.ptr(out), t.numel, t.bits, k)
+    ws = torch.empty(int(N.lib().qd_unpack_model_workspace_bytes(len(items))), dtype=torch.uint8, device=dev)
+    keep += [desc, ws]
+    args = (desc.ctypes.data, len(items), 0 if pm.bucket_size is None else int(pm.bucket_size),
+            int(pm.levels) if pm.kind == "uniform" else 0, N.ptr(ws), ws.numel(), N.stream_ptr(dev))
+    return args, keep
+
+
+def _packed_device_of(pm: PackedModel, device=None):
+    N.require_cuda()
+    if device is not None:
+        return torch.device(device)
+    for t in pm.tensors:
+        for x in (t.packed, t.raw):
+            if x is not None and x.is_cuda:
+                return x.device
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def unpack_(pm: PackedModel, model) -> None:
+    """Writes every parameter of ``model`` in place from ``pm`` (existing parameter handles stay valid), and its
+    persistent buffers when ``pm`` stores them.  Everything is checked before anything is written.  Per device, the
+    quantized tensors decode in one launch, straight into parameters that are contiguous float32 on that device."""
+    named = list(model.named_parameters())
+    if len(named) != len(pm.tensors):
+        raise ValueError(f"model has {len(named)} parameters, the packed model {len(pm.tensors)}")
+    for (name, p), t in zip(named, pm.tensors):
+        if tuple(p.shape) != tuple(t.shape):
+            raise ValueError(f"{name}: shape {tuple(p.shape)} != stored {tuple(t.shape)} ({t.name})")
+    bufs = []
+    if pm.buffers is not None:
+        bufs = _persistent_buffers(model)
+        if len(bufs) != len(pm.buffers):
+            raise ValueError(f"model has {len(bufs)} persistent buffers, the packed model {len(pm.buffers)}")
+        for (name, b), (stored, s) in zip(bufs, pm.buffers):
+            if tuple(b.shape) != tuple(s.shape) or b.dtype != s.dtype:
+                raise ValueError(f"buffer {name}: {b.dtype} {tuple(b.shape)} != stored {s.dtype} {tuple(s.shape)} ({stored})")
+    default = _packed_device_of(pm)
+    groups = {}                                  # device -> parameter indices (host parameters decode on `default`)
+    for k, (_, p) in enumerate(named):
+        groups.setdefault(p.device if p.is_cuda else default, []).append(k)
+    for _, b in bufs:
+        if b.is_cuda:
+            groups.setdefault(b.device, [])
+    with torch.no_grad():
+        for dev, ks in groups.items():
+            with torch.cuda.device(dev):
+                move = _mover(pm, dev)
+                items, temps = [], []
+                for k in ks:
+                    t, d = pm.tensors[k], named[k][1].data
+                    if not t.quantized:
+                        d.copy_((move(t.raw) if d.is_cuda else t.raw).view_as(d))
+                    elif d.device == dev and d.dtype == torch.float32 and d.is_contiguous():
+                        items.append((t, d))
+                    else:
+                        out = torch.empty(t.numel, dtype=torch.float32, device=dev)
+                        items.append((t, out))
+                        temps.append((d, out))
+                if items:
+                    args, keep = _packed_decode_args(pm, items, dev, move)
+                    N.check(N.lib().qd_unpack_dequant_model(*args))
+                for d, out in temps:
+                    d.copy_(out.view_as(d))
+                for (_, b), (_, s) in zip(bufs, pm.buffers or []):
+                    if b.is_cuda and b.device == dev:
+                        b.copy_(move(s))
+        for (_, b), (_, s) in zip(bufs, pm.buffers or []):
+            if not b.is_cuda:
+                b.copy_(s)
+
+
+def save_packed(pm: PackedModel, path) -> int:
+    """Writes the fixed-width container: magic QDPACK, version 1, JSON header, 16-byte-aligned little-endian sections
+    (packed codes as bytes).  Returns the file size in bytes."""
+    header, sections, data_bytes = _packed_layout(pm)
+    return _write_container(path, PACKED_MAGIC, PACKED_VERSION, header, sections, data_bytes)
+
+
+def _bad_packed(msg):
+    raise ValueError(f"not a valid fixed-width model file: {msg}")
+
+
+def load_packed(path, device=None) -> PackedModel:
+    """Reads and validates a file written by save_packed; everything is checked on the host before anything reaches a
+    device.  Every section is a view into one tensor holding the file's data region.  device=None keeps it in host
+    memory (unpack_ moves it to the GPU in one copy); a device gets it in one copy here."""
+    bad = _bad_packed
+    with open(path, "rb") as f:
+        buf = bytearray(f.read())
+    if len(buf) < _PREFIX.size:
+        bad("shorter than its prefix")
+    magic, version, reserved, hlen = _PREFIX.unpack_from(buf)
+    if magic != PACKED_MAGIC:
+        bad("bad magic")
+    if version != PACKED_VERSION:
+        bad(f"format version {version}, this reader knows {PACKED_VERSION}")
+    if reserved != 0:
+        bad("reserved prefix field is not 0")
+    if _PREFIX.size + hlen > len(buf):
+        bad("header runs past the end of the file")
+    try:
+        h = json.loads(buf[_PREFIX.size:_PREFIX.size + hlen].decode("utf-8"))
+        kind, levels, bucket, entries, data_bytes = h["kind"], h["levels"], h["bucket"], h["tensors"], h["data_bytes"]
+    except (ValueError, KeyError, TypeError) as e:
+        bad(f"unreadable header ({e})")
+    if not isinstance(data_bytes, int) or not isinstance(entries, list):
+        bad("data_bytes must be an integer and tensors a list")
+    start = _align(_PREFIX.size + hlen)
+    if data_bytes < 0 or start + data_bytes != len(buf):
+        bad(f"{len(buf)} bytes, the header describes {start + data_bytes}")
+    if kind not in ("uniform", "nonuniform"):
+        bad(f"unknown kind {kind!r}")
+    if kind == "uniform" and not (isinstance(levels, int) and not isinstance(levels, bool) and 2 <= levels <= 256):
+        bad("uniform levels must be in [2, 256]")
+    if kind == "nonuniform" and levels is not None:
+        bad("a non-uniform model has no levels")
+    if bucket is not None and not (isinstance(bucket, int) and not isinstance(bucket, bool) and bucket > 0):
+        bad("bucket must be a positive integer or null")
+    region = torch.from_numpy(np.frombuffer(buf, np.uint8, count=data_bytes, offset=start)) if data_bytes else \
+        torch.empty(0, dtype=torch.uint8)
+    spans = []
+
+    def view(off, nb, dtype, shape):
+        return region[off:off + nb].view(dtype).view(shape)
+
+    def section(e, name, dtype, nbytes):
+        try:
+            off, nb = (int(v) for v in e["sections"][name])
+        except (KeyError, TypeError, ValueError):
+            bad(f"{e.get('name')}: section {name} missing")
+        if nb != nbytes:
+            bad(f"{e.get('name')}: section {name} holds {nb} bytes, {nbytes} expected")
+        if off < 0 or off % _ALIGN or off + nb > data_bytes:
+            bad(f"{e.get('name')}: section {name} out of range")
+        spans.append((off, nb))
+        return view(off, nb, dtype, (nbytes // dtype.itemsize,))
+
+    tensors, names = [], set()
+    for e in entries:
+        try:
+            name, shape, quantized = str(e["name"]), tuple(int(d) for d in e["shape"]), e["quantized"]
+        except (KeyError, TypeError, ValueError):
+            bad("tensor entry without name / shape / quantized")
+        if not isinstance(quantized, bool) or e.get("dtype") != "float32" or any(d < 0 for d in shape):
+            bad(f"{name}: bad dtype, shape or quantized flag")
+        if name in names:
+            bad(f"tensor {name} appears twice")
+        names.add(name)
+        if not isinstance(e.get("sections"), dict) or set(e["sections"]) != ({"packed", "alpha", "beta"} if quantized else {"raw"}):
+            bad(f"{name}: unexpected sections")
+        n = int(math.prod(shape))
+        if not quantized:
+            tensors.append(PackedEntry(name, shape, raw=section(e, "raw", torch.float32, 4 * n)))
+            continue
+        if n == 0:
+            bad(f"{name}: empty quantized tensor")
+        bits = e.get("bits")
+        if bits not in (1, 2, 4, 8) or isinstance(bits, bool):
+            bad(f"{name}: bits must be 1, 2, 4 or 8")
+        pts = None
+        if kind == "uniform":
+            if "points" in e:
+                bad(f"{name}: a uniform tensor has no points")
+            if levels > 1 << bits:
+                bad(f"{name}: {levels} levels do not fit in {bits}-bit codes")
+        else:
+            try:
+                pts = torch.tensor([float(v) for v in e["points"]], dtype=torch.float32)
+            except (KeyError, TypeError, ValueError):
+                bad(f"{name}: non-uniform tensor without points")
+            if not 1 <= pts.numel() <= 1 << bits:
+                bad(f"{name}: {pts.numel()} points do not fit in {bits}-bit codes")
+        rows = _rows(n, bucket)
+        tensors.append(PackedEntry(name, shape, bits=bits, packed=section(e, "packed", torch.uint8, (n * bits + 7) // 8),
+                                   alpha=section(e, "alpha", torch.float32, 4 * rows),
+                                   beta=section(e, "beta", torch.float32, 4 * rows), points=pts))
+    if not any(t.quantized for t in tensors):
+        bad("no quantized tensor")
+    buffers = None
+    if "buffers" in h:
+        buffers = _read_buffers(h["buffers"], view, data_bytes, bad, spans)
+    spans.sort()
+    for (o1, n1), (o2, _) in zip(spans, spans[1:]):
+        if o1 + n1 > o2:
+            bad(f"sections at {o1} and {o2} overlap")
+    pm = PackedModel(kind, levels, bucket, tensors, buffers=buffers)
+    pm._data = region
+    if device is not None:                       # everything is validated before anything reaches the GPU
+        move = _mover(pm, torch.device(device))
+        pts = [t.points for t in tensors if t.points is not None]
+        flat = torch.cat(pts).to(device) if pts else None          # every tensor's points in one upload too
+        at = 0
+        for t in tensors:
+            for f_ in ("packed", "alpha", "beta", "raw"):
+                setattr(t, f_, move(getattr(t, f_)))
+            if t.points is not None:
+                t.points, at = flat[at:at + t.points.numel()], at + t.points.numel()
+        if buffers is not None:
+            pm.buffers = [(name, move(b)) for name, b in buffers]
+        pm._data = move(region)
+    return pm
 
 
 def get_size_reduction(effective_number_bits, bucket_size=256, full_precision_bits=32):

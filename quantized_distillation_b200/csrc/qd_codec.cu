@@ -8,17 +8,6 @@
 
 using namespace qd;
 
-// Calls f(std::integral_constant<int, BITS>{}) for a code width `bits` already checked to be 1, 2, 4 or 8.
-template <class F>
-static void with_bits(int bits, F&& f) {
-    if (bits == 8) f(std::integral_constant<int, 8>{});
-    else if (bits == 4) f(std::integral_constant<int, 4>{});
-    else if (bits == 2) f(std::integral_constant<int, 2>{});
-    else f(std::integral_constant<int, 1>{});
-}
-
-static bool bits_ok(int bits) { return bits == 1 || bits == 2 || bits == 4 || bits == 8; }
-
 // ------------------------------------------------------------------ f2: histogram of indices
 __global__ void __launch_bounds__(256) index_histogram_kernel(const uint8_t* __restrict__ idx, int64_t n, int bins,
                                                              unsigned long long* __restrict__ counts) {
@@ -162,17 +151,21 @@ __device__ __forceinline__ uint32_t load_codes4_fast(const uint8_t* __restrict__
     else return (uint32_t)__ldcs(packed + (g >> 1)) >> (unsigned)((g & 1) * 4);
 }
 
-template <bool UNIFORM, int BITS>
-__global__ void __launch_bounds__(256, 4) unpack_dequant_kernel(const uint8_t* __restrict__ packed,
-                                                            const float* __restrict__ points, int K,
-                                                            const float* __restrict__ alpha, const float* __restrict__ beta,
-                                                            float* __restrict__ q, Geometry geo, float S) {
-    __shared__ float s_unit[256];
+template <bool UNIFORM>
+__device__ __forceinline__ void load_unit_table(float* s_unit, const float* __restrict__ points, int K, float S) {
     for (int i = threadIdx.x; i < 256; i += blockDim.x) {
         if (UNIFORM) s_unit[i] = ((float)i <= S) ? level_to_unit((float)i, S) : 0.f;
         else s_unit[i] = (i < K) ? points[i] : 0.f;
     }
-    __syncthreads();
+}
+
+// The element loop of one tensor's unpack, as CTA `block` of the `nblocks` CTAs that serve the tensor: the per-tensor
+// kernel calls it with its own grid, the whole-model kernel with the tensor's share of its grid, so both write the
+// same bits by construction.
+template <int BITS>
+__device__ __forceinline__ void unpack_dequant_body(const float* s_unit, const uint8_t* __restrict__ packed,
+                                                    const float* __restrict__ alpha, const float* __restrict__ beta,
+                                                    float* __restrict__ q, const Geometry& geo, unsigned block, unsigned nblocks) {
     const int64_t L = geo.row_len;
     const int64_t groups = (geo.n + 3) / 4;
     constexpr unsigned mask = (1u << BITS) - 1u;
@@ -183,14 +176,14 @@ __global__ void __launch_bounds__(256, 4) unpack_dequant_kernel(const uint8_t* _
     const bool fast_ok = ((reinterpret_cast<uintptr_t>(q) & 15) == 0) && ((reinterpret_cast<uintptr_t>(packed) & 3) == 0) &&
                          (single || (L % 4 == 0 && L < (1ll << 30) && geo.rows < (1ll << 31)));
     const int64_t full_tiles = fast_ok ? geo.n / (kTileGroups * 4) : 0;
-    if (full_tiles > (int64_t)blockIdx.x) {
+    if (full_tiles > (int64_t)block) {
         const uint32_t L32 = single ? 1u : (uint32_t)L;
-        const int64_t e_first = ((int64_t)blockIdx.x * kTileGroups + threadIdx.x) * 4;
+        const int64_t e_first = ((int64_t)block * kTileGroups + threadIdx.x) * 4;
         int row = single ? 0 : (int)(e_first / L);
         uint32_t rem = single ? 0u : (uint32_t)(e_first % L);
         const int du_rows = single ? 0 : (int)((256 * 4) / L);
         const uint32_t du_rem = single ? 0u : (uint32_t)((256 * 4) % L);
-        const int64_t dt = (int64_t)gridDim.x * kTileGroups * 4;
+        const int64_t dt = (int64_t)nblocks * kTileGroups * 4;
         const int dt_rows = single ? 0 : (int)(dt / L);
         const uint32_t dt_rem = single ? 0u : (uint32_t)(dt % L);
         // Everything a tile READS (codes, alpha, beta of its kTileU groups) is fetched one tile ahead: the stores of a
@@ -211,13 +204,13 @@ __global__ void __launch_bounds__(256, 4) unpack_dequant_kernel(const uint8_t* _
             }
         };
         Fetched cur;
-        fetch(blockIdx.x, row, rem, cur);
-        for (int64_t tile = blockIdx.x; tile < full_tiles; tile += gridDim.x) {
+        fetch(block, row, rem, cur);
+        for (int64_t tile = block; tile < full_tiles; tile += nblocks) {
             Fetched nxt = cur;
             row += dt_rows;
             rem += dt_rem;
             if (rem >= L32) { rem -= L32; ++row; }
-            if (tile + gridDim.x < full_tiles) fetch(tile + gridDim.x, row, rem, nxt);
+            if (tile + nblocks < full_tiles) fetch(tile + nblocks, row, rem, nxt);
             float* dst = q + (tile * kTileGroups + threadIdx.x) * 4;
 #pragma unroll
             for (int u = 0; u < kTileU; ++u) {
@@ -232,8 +225,8 @@ __global__ void __launch_bounds__(256, 4) unpack_dequant_kernel(const uint8_t* _
     // general loop: the last partial tile, unaligned pointers, ragged buckets
     const int64_t in_bytes = (geo.n * BITS + 7) / 8;
     const bool ivec = (reinterpret_cast<uintptr_t>(packed) & 3) == 0;
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t g = full_tiles * kTileGroups + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += stride) {
+    const int64_t stride = (int64_t)nblocks * blockDim.x;
+    for (int64_t g = full_tiles * kTileGroups + (int64_t)block * blockDim.x + threadIdx.x; g < groups; g += stride) {
         const int64_t e0 = g * 4;
         const uint32_t w = load_codes4<BITS>(packed, e0, in_bytes, ivec);
         for (int j = 0; j < 4; ++j) {
@@ -242,6 +235,17 @@ __global__ void __launch_bounds__(256, 4) unpack_dequant_kernel(const uint8_t* _
             q[e0 + j] = from_unit(s_unit[(w >> (j * BITS)) & mask], alpha[r], beta[r]);
         }
     }
+}
+
+template <bool UNIFORM, int BITS>
+__global__ void __launch_bounds__(256, 4) unpack_dequant_kernel(const uint8_t* __restrict__ packed,
+                                                            const float* __restrict__ points, int K,
+                                                            const float* __restrict__ alpha, const float* __restrict__ beta,
+                                                            float* __restrict__ q, Geometry geo, float S) {
+    __shared__ float s_unit[256];
+    load_unit_table<UNIFORM>(s_unit, points, K, S);
+    __syncthreads();
+    unpack_dequant_body<BITS>(s_unit, packed, alpha, beta, q, geo, blockIdx.x, gridDim.x);
 }
 
 // Checks the arguments both unpacks share and launches unpack_dequant_kernel<UNIFORM, bits>.
@@ -273,6 +277,89 @@ extern "C" int qd_unpack_dequant_nonuniform(const uint8_t* packed, int bits, con
                                             qd_stream_t stream) {
     if (points == nullptr || num_points < 1 || num_points > (1 << bits)) return fail(QD_ERR_INVALID_ARG, "num_points must be in [1, 2^bits]");
     return unpack_dequant<false>(packed, bits, points, num_points, alpha, beta, q, n, bucket, 0.f, stream);
+}
+
+// A whole model in one launch.  Tensor t owns CTAs [cta_start[t], cta_start[t + 1]), one per tile of kTileGroups groups
+// of four elements, found by binary search; every CTA loads its tensor's unit table once and runs the per-tensor body
+// as CTA (blockIdx.x - cta_start[t]) of the tensor's share of the grid, at the tensor's own code width.
+template <bool UNIFORM>
+__global__ void __launch_bounds__(256, 4) unpack_dequant_model_kernel(const qd_packed_tensor* __restrict__ tensors,
+                                                                  const int32_t* __restrict__ cta_start, int count,
+                                                                  int64_t bucket, float S) {
+    __shared__ float s_unit[256];
+    const int b = (int)blockIdx.x;
+    int lo = 0, hi = count;                       // cta_start[lo] <= b < cta_start[hi]
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(cta_start + mid) <= b) lo = mid;
+        else hi = mid;
+    }
+    const qd_packed_tensor& t = tensors[lo];
+    load_unit_table<UNIFORM>(s_unit, t.points, t.num_points, S);
+    __syncthreads();
+    Geometry geo;                                 // geometry_of
+    geo.n = t.n;
+    geo.row_len = (bucket == 0 || t.n < bucket) ? t.n : bucket;
+    geo.rows = (t.n + geo.row_len - 1) / geo.row_len;
+    const int first = __ldg(cta_start + lo);
+    const unsigned block = (unsigned)(b - first), nblocks = (unsigned)(__ldg(cta_start + lo + 1) - first);
+    switch (t.bits) {
+        case 8: unpack_dequant_body<8>(s_unit, t.packed, t.alpha, t.beta, t.q, geo, block, nblocks); break;
+        case 4: unpack_dequant_body<4>(s_unit, t.packed, t.alpha, t.beta, t.q, geo, block, nblocks); break;
+        case 2: unpack_dequant_body<2>(s_unit, t.packed, t.alpha, t.beta, t.q, geo, block, nblocks); break;
+        default: unpack_dequant_body<1>(s_unit, t.packed, t.alpha, t.beta, t.q, geo, block, nblocks); break;
+    }
+}
+
+// workspace of the model unpack: the tensor array, then cta_start[count + 1] (int32)
+static_assert(sizeof(qd_packed_tensor) == 56 && sizeof(qd_packed_tensor) % alignof(int32_t) == 0,
+              "qd_packed_tensor layout is shared with codec.py");
+
+extern "C" size_t qd_unpack_model_workspace_bytes(int count) {
+    return count < 1 ? 0 : (size_t)count * sizeof(qd_packed_tensor) + ((size_t)count + 1) * sizeof(int32_t);
+}
+
+extern "C" int qd_unpack_dequant_model(const qd_packed_tensor* tensors, int count, int64_t bucket, int levels, void* workspace,
+                                       size_t workspace_bytes, qd_stream_t stream) {
+    if (tensors == nullptr || count < 1) return fail(QD_ERR_INVALID_ARG, "NULL tensors or count < 1");
+    if (bucket < 0) return fail(QD_ERR_INVALID_ARG, "bucket must be >= 0");
+    if (levels != 0 && (levels < 2 || levels > 256)) return fail(QD_ERR_INVALID_ARG, "levels must be in [2, 256] (uniform) or 0 (non-uniform)");
+    const size_t need = qd_unpack_model_workspace_bytes(count);
+    if (workspace == nullptr || (reinterpret_cast<uintptr_t>(workspace) & 15) || workspace_bytes < need)
+        return fail(QD_ERR_WORKSPACE, "workspace must be 16-byte aligned and hold %zu bytes (got %zu)", need, workspace_bytes);
+    const bool uniform = levels != 0;
+    // host image of the workspace, consumed by the pageable copy before it returns (kept per thread: no allocation once grown)
+    thread_local std::vector<unsigned char> image;
+    image.resize(need);
+    int32_t* cta_start = reinterpret_cast<int32_t*>(image.data() + (size_t)count * sizeof(qd_packed_tensor));
+    int64_t ctas = 0;
+    for (int i = 0; i < count; ++i) {
+        const qd_packed_tensor& t = tensors[i];
+        if (t.packed == nullptr || t.alpha == nullptr || t.beta == nullptr || t.q == nullptr)
+            return fail(QD_ERR_INVALID_ARG, "tensor %d: NULL argument", i);
+        if (t.n < 1) return fail(QD_ERR_INVALID_ARG, "tensor %d: n must be >= 1", i);
+        if (!bits_ok(t.bits)) return fail(QD_ERR_INVALID_ARG, "tensor %d: bits must be 1, 2, 4 or 8", i);
+        if (uniform && (t.points != nullptr || t.num_points != 0))
+            return fail(QD_ERR_INVALID_ARG, "tensor %d: a uniform model has no points (points NULL, num_points 0)", i);
+        if (uniform && levels > (1 << t.bits)) return fail(QD_ERR_INVALID_ARG, "tensor %d: %d levels do not fit in %d-bit codes", i, levels, t.bits);
+        if (!uniform && (t.points == nullptr || t.num_points < 1 || t.num_points > (1 << t.bits)))
+            return fail(QD_ERR_INVALID_ARG, "tensor %d: num_points must be in [1, 2^bits]", i);
+        cta_start[i] = (int32_t)ctas;
+        ctas += ((t.n + 3) / 4 + kTileGroups - 1) / kTileGroups;
+        if (ctas > INT32_MAX) return fail(QD_ERR_INVALID_ARG, "the model has more than 2^31 - 1 tiles of %d elements", kTileGroups * 4);
+    }
+    cta_start[count] = (int32_t)ctas;
+    memcpy(image.data(), tensors, (size_t)count * sizeof(qd_packed_tensor));
+    cudaStream_t st = as_stream(stream);
+    QD_CUDA(cudaMemcpyAsync(workspace, image.data(), need, cudaMemcpyHostToDevice, st));
+    const qd_packed_tensor* dev_tensors = static_cast<const qd_packed_tensor*>(workspace);
+    const int32_t* dev_start = reinterpret_cast<const int32_t*>(static_cast<const unsigned char*>(workspace) + (size_t)count * sizeof(qd_packed_tensor));
+    if (uniform)
+        unpack_dequant_model_kernel<true><<<(unsigned)ctas, 256, 0, st>>>(dev_tensors, dev_start, count, bucket, (float)(levels - 1));
+    else
+        unpack_dequant_model_kernel<false><<<(unsigned)ctas, 256, 0, st>>>(dev_tensors, dev_start, count, bucket, 0.f);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
 }
 
 // ------------------------------------------------------------------ f2: Huffman-coded storage (qd_huffman.cuh)

@@ -55,4 +55,18 @@ int with_row_regs(int64_t row_len, F&& f) {
     return f(std::integral_constant<int, 4>{});
 }
 
+// code widths of the fixed-width packed codec
+inline bool bits_ok(int bits) { return bits == 1 || bits == 2 || bits == 4 || bits == 8; }
+// smallest code width that holds `symbols` distinct codes (symbols in [1, 256])
+inline int bits_for(int symbols) { return symbols <= 2 ? 1 : symbols <= 4 ? 2 : symbols <= 16 ? 4 : 8; }
+
+// Calls f(std::integral_constant<int, BITS>{}) for a code width `bits` already checked to be 1, 2, 4 or 8.
+template <class F>
+decltype(auto) with_bits(int bits, F&& f) {
+    if (bits == 8) return f(std::integral_constant<int, 8>{});
+    if (bits == 4) return f(std::integral_constant<int, 4>{});
+    if (bits == 2) return f(std::integral_constant<int, 2>{});
+    return f(std::integral_constant<int, 1>{});
+}
+
 }  // namespace qd

@@ -43,9 +43,9 @@ extern "C" size_t qd_workspace_bytes(int64_t n, int64_t bucket) {
 }
 
 // ------------------------------------------------------------------ launchers
-template <int OP, int BWD, int R, bool VEC>
+template <int OP, int BWD, int R, bool VEC, int PACK = 0>
 static int launch_warp_inst(const Params& P, cudaStream_t s) {
-    auto kern = warp_rows_kernel<OP, BWD, R, VEC>;
+    auto kern = warp_rows_kernel<OP, BWD, R, VEC, false, PACK>;
     int grid = (int)warp_rows_grid(P.geo.rows);
     if constexpr (!kRowPerWarp<OP>) {
         int rc = resident_grid((const void*)kern, kWarpCtaThreads, 0, (P.geo.rows + kWarpsPerCta - 1) / kWarpsPerCta, &grid);
@@ -665,4 +665,103 @@ extern "C" int qd_centroid_index(const float* xhat, const float* points, int num
     centroid_index_kernel<<<grid, 256, 0, as_stream(stream)>>>(xhat, points, num_points, rule, idx_u8, idx_i64, unit_out, n);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
+}
+
+// ------------------------------------------------------------------ f2: quantize straight to packed codes
+// The register warp path writes the packed stream itself (store_levels, qd_warp_path.cuh): 16-byte aligned rows of at
+// most 1024 floats whose packed start is a whole byte, and a 4-byte aligned stream.  Every other layout runs the level
+// kernel into the caller's workspace, then qd_pack_indices; the bytes are the same either way.
+extern "C" size_t qd_packed_workspace_bytes(int64_t n, int64_t bucket) {
+    const size_t ws = qd_workspace_bytes(n, bucket);
+    return ws == 0 ? 0 : ((size_t)n + 255) / 256 * 256 + ws;
+}
+
+static bool packed_in_registers(const Params& P, int bits) {
+    return P.geo.row_len <= 1024 && rows_vectorizable(P) && (reinterpret_cast<uintptr_t>(P.idx8) & 3) == 0 &&
+           (P.geo.rows == 1 || (P.geo.row_len * bits) % 8 == 0);
+}
+
+// checks shared by both packed encoders; on success the fallback's uint8 levels and level-kernel scratch are split
+// out of the workspace
+static int packed_common(const float* x, uint8_t* packed, int bits, int symbols, const char* what, const float* alpha,
+                         const float* beta, int64_t n, int64_t bucket, void* workspace, size_t workspace_bytes,
+                         uint8_t** idx, void** ws_rest, size_t* ws_rest_bytes) {
+    if (x == nullptr || packed == nullptr || alpha == nullptr || beta == nullptr) return fail(QD_ERR_INVALID_ARG, "x, packed, alpha and beta are required");
+    if (!bits_ok(bits)) return fail(QD_ERR_INVALID_ARG, "bits must be 1, 2, 4 or 8");
+    if (symbols < 1 || symbols > 256 || bits < bits_for(symbols))
+        return fail(QD_ERR_INVALID_ARG, "%s = %d does not fit in %d-bit codes", what, symbols, bits);
+    const size_t need = qd_packed_workspace_bytes(n, bucket);
+    if (need == 0) return fail(QD_ERR_INVALID_ARG, "bad geometry n=%lld bucket=%lld", (long long)n, (long long)bucket);
+    if (workspace == nullptr || workspace_bytes < need) return fail(QD_ERR_WORKSPACE, "workspace of %zu bytes needed, %zu given", need, workspace_bytes);
+    const size_t idx_bytes = ((size_t)n + 255) / 256 * 256;
+    *idx = static_cast<uint8_t*>(workspace);
+    *ws_rest = static_cast<unsigned char*>(workspace) + idx_bytes;
+    *ws_rest_bytes = workspace_bytes - idx_bytes;
+    return QD_OK;
+}
+
+extern "C" int qd_uniform_fwd_packed(const float* x, uint8_t* packed, int bits, float* alpha, float* beta, int64_t n,
+                                     int64_t bucket, int levels, void* workspace, size_t workspace_bytes, qd_stream_t stream) {
+    uint8_t* idx;
+    void* rest;
+    size_t rest_bytes;
+    if (levels < 2) return fail(QD_ERR_INVALID_ARG, "levels (s) must be >= 2, got %d", levels);
+    int rc = packed_common(x, packed, bits, levels, "levels", alpha, beta, n, bucket, workspace, workspace_bytes, &idx, &rest, &rest_bytes);
+    if (rc) return rc;
+    Params P = blank_params();
+    rc = uniform_common(P, n, bucket, levels);
+    if (rc) return rc;
+    P.x = x; P.idx8 = packed; P.alpha = alpha; P.beta = beta;
+    cudaStream_t s = as_stream(stream);
+    if (packed_in_registers(P, bits))
+        return with_row_regs(P.geo.row_len, [&](auto r) {
+            return with_bits(bits, [&](auto b) { return launch_warp_inst<OP_UNIFORM, BWD_OFF, decltype(r)::value, true, decltype(b)::value>(P, s); });
+        });
+    rc = qd_uniform_fwd(x, nullptr, idx, alpha, beta, nullptr, nullptr, n, bucket, levels, nullptr, 0.f, 0, 0, 0, rest, rest_bytes, stream);
+    if (rc) return rc;
+    return qd_pack_indices(idx, packed, n, bits, stream);
+}
+
+// smallest code width a centroid-table size class KP can need: KP = 4 holds K = 1 .. 4, every larger class K > KP / 2
+template <int KP>
+constexpr int kMinPackBits = KP <= 4 ? 1 : KP <= 16 ? 4 : 8;
+
+extern "C" int qd_nonuniform_fwd_packed(const float* x, const float* points, int num_points, int rule, uint8_t* packed,
+                                        int bits, float* alpha, float* beta, int64_t n, int64_t bucket, void* workspace,
+                                        size_t workspace_bytes, qd_stream_t stream) {
+    uint8_t* idx;
+    void* rest;
+    size_t rest_bytes;
+    if (points == nullptr) return fail(QD_ERR_INVALID_ARG, "points is required");
+    if (rule != QD_RULE_NEAREST && rule != QD_RULE_MIDPOINT) return fail(QD_ERR_INVALID_ARG, "unknown rule %d", rule);
+    int rc = packed_common(x, packed, bits, num_points, "num_points", alpha, beta, n, bucket, workspace, workspace_bytes, &idx, &rest,
+                           &rest_bytes);
+    if (rc) return rc;
+    Params P = blank_params();
+    if (geometry_of(n, bucket, &P.geo)) return fail(QD_ERR_INVALID_ARG, "bad geometry n=%lld bucket=%lld", (long long)n, (long long)bucket);
+    P.x = x; P.idx8 = packed; P.alpha = alpha; P.beta = beta;
+    P.points = points; P.num_points = num_points; P.rule = rule;
+    cudaStream_t s = as_stream(stream);
+    if (packed_in_registers(P, bits)) {
+        // same centroid-table classes as qd_nonuniform_fwd; widths below a class's smallest need are refused above
+        auto go = [&](auto kp) {
+            constexpr int KP = decltype(kp)::value;
+            return with_row_regs(P.geo.row_len, [&](auto r) {
+                return with_bits(bits, [&](auto b) {
+                    constexpr int B = decltype(b)::value;
+                    if constexpr (B >= kMinPackBits<KP>) return launch_warp_inst<OP_NONUNIFORM, KP, decltype(r)::value, true, B>(P, s);
+                    else return fail(QD_ERR_INVALID_ARG, "%d points do not fit in %d-bit codes", num_points, B);
+                });
+            });
+        };
+        if (num_points <= 4) return go(std::integral_constant<int, 4>{});
+        if (num_points <= 8) return go(std::integral_constant<int, 8>{});
+        if (num_points <= 16) return go(std::integral_constant<int, 16>{});
+        if (num_points <= 32) return go(std::integral_constant<int, 32>{});
+        if (num_points <= 64) return go(std::integral_constant<int, 64>{});
+        return go(std::integral_constant<int, 256>{});
+    }
+    rc = qd_nonuniform_fwd(x, points, num_points, rule, nullptr, idx, nullptr, alpha, beta, n, bucket, nullptr, 0.f, rest, rest_bytes, stream);
+    if (rc) return rc;
+    return qd_pack_indices(idx, packed, n, bits, stream);
 }

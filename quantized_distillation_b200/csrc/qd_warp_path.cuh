@@ -110,6 +110,53 @@ __device__ __forceinline__ void store_row_u8(uint8_t* __restrict__ p, int len, i
     }
 }
 
+// Fixed-width packed store of a row's levels (the layout of qd_pack_indices): element e of the tensor has its BITS-bit
+// code in byte e*BITS/8 at bit (e*BITS)%8.  `p` is the row's first byte, so the row must start on a byte boundary,
+// and in the 128-bit lane layout (VEC) lane L's four codes r*128+4L .. +3 are one aligned 4*BITS-bit field: one byte
+// store at 2 bits, a 16-bit store at 4, a 32-bit store at 8 (the caller aligns `p` to 4 bytes).  At 1 bit the even
+// lane merges its odd neighbour's nibble (one shuffle) and stores the byte.  Codes past `len` are zero and the bytes
+// that hold none of the row's codes are not written, so the last byte of the tensor is exactly qd_pack_indices'.
+template <int BITS, int R, bool FULL, typename T>
+__device__ __forceinline__ void store_row_packed(uint8_t* __restrict__ p, int len, int lane, const T (&lv)[4 * R]) {
+    static_assert(BITS == 1 || BITS == 2 || BITS == 4 || BITS == 8, "code width");
+    constexpr int kPerByte = 8 / BITS;                 // codes per byte: byte b of a lane holds codes e0 + b*kPerByte ..
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+        const int e0 = r * 128 + lane * 4;
+        uint32_t w = 0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (FULL || e0 + j < len) w |= (uint32_t)(int)lv[4 * r + j] << (j * BITS);
+        if constexpr (BITS == 1) {
+            const uint32_t odd = __shfl_down_sync(kFullMask, w, 1);
+            if ((lane & 1) == 0 && (FULL || e0 < len)) __stcs(p + r * 16 + (lane >> 1), (uint8_t)(w | (odd << 4)));
+        } else {
+            uint8_t* dst = p + r * 16 * BITS + lane * (BITS / 2);
+            if (FULL || e0 + 4 <= len) {
+                if constexpr (BITS == 8) __stcs(reinterpret_cast<uint32_t*>(dst), w);
+                else if constexpr (BITS == 4) __stcs(reinterpret_cast<uint16_t*>(dst), (uint16_t)w);
+                else __stcs(dst, (uint8_t)w);
+            } else {
+#pragma unroll
+                for (int b = 0; b < BITS / 2; ++b)
+                    if (e0 + b * kPerByte < len) dst[b] = (uint8_t)(w >> (8 * b));
+            }
+        }
+    }
+}
+
+// The level output of the row kernels: uint8 levels at P.idx8 + base (PACK = 0), or PACK-bit packed codes of the
+// row starting at byte base*PACK/8 of P.idx8 (only in the 128-bit lane layout).
+template <int PACK, int R, bool VEC, bool FULL, typename T>
+__device__ __forceinline__ void store_levels(uint8_t* __restrict__ idx8, int64_t base, int len, int lane, const T (&lv)[4 * R]) {
+    if constexpr (PACK == 0) {
+        store_row_u8<R, VEC, FULL>(idx8 + base, len, lane, lv);
+    } else {
+        static_assert(VEC, "the packed store needs the 128-bit lane layout");
+        store_row_packed<PACK, R, FULL>(idx8 + base * PACK / 8, len, lane, lv);
+    }
+}
+
 // AUX is the backward mode for OP_UNIFORM and the centroid-table size class KP for
 // OP_NONUNIFORM (power of two >= K; <= 32: table in the lanes of the warp, else shared memory).
 template <int OP, int AUX>
@@ -126,7 +173,7 @@ __device__ __forceinline__ void warp_load_row(const Params& P, int64_t row, int 
 
 // ACC_A: A/B switch of the r_b accumulation of the min/max backward (benchmarks only, qd_debug_set_tuning key 3):
 // false = minmax_lane_sum (division mode hoisted, float32 groups), true = one float64 add per element
-template <int OP, int AUX, int R, bool VEC, bool FULL, bool ACC_A = false>
+template <int OP, int AUX, int R, bool VEC, bool FULL, bool ACC_A = false, int PACK = 0>
 __device__ __forceinline__ void warp_compute_row(const Params& P, const Centroids& cen, const LaneTable<OP, AUX>& rt, int64_t row,
                                                  int lane, float (&v)[4 * R], float (&gv)[4 * R]) {
     constexpr int BWD = (OP == OP_UNIFORM) ? AUX : (int)BWD_OFF;
@@ -317,7 +364,7 @@ __device__ __forceinline__ void warp_compute_row(const Params& P, const Centroid
             }
             store_row<R, VEC, FULL>(P.q + base, len, lane, qv);
         }
-        if (P.idx8 != nullptr) store_row_u8<R, VEC, FULL>(P.idx8 + base, len, lane, lv);
+        if (P.idx8 != nullptr) store_levels<PACK, R, VEC, FULL>(P.idx8, base, len, lane, lv);
         if constexpr (BWD != BWD_OFF) store_row<R, VEC, FULL>(P.gout + base, len, lane, gv);
         return;
     }
@@ -359,7 +406,7 @@ __device__ __forceinline__ void warp_compute_row(const Params& P, const Centroid
             }
         }
         if (P.q != nullptr) store_row<R, VEC, FULL>(P.q + base, len, lane, qv);
-        if (P.idx8 != nullptr) store_row_u8<R, VEC, FULL>(P.idx8 + base, len, lane, li);
+        if (P.idx8 != nullptr) store_levels<PACK, R, VEC, FULL>(P.idx8, base, len, lane, li);
         if (P.idx64 != nullptr) {
 #pragma unroll
             for (int r = 0; r < R; ++r)
@@ -373,12 +420,12 @@ __device__ __forceinline__ void warp_compute_row(const Params& P, const Centroid
     }
 }
 
-template <int OP, int AUX, int R, bool VEC, bool FULL, bool ACC_A = false>
+template <int OP, int AUX, int R, bool VEC, bool FULL, bool ACC_A = false, int PACK = 0>
 __device__ __forceinline__ void warp_process_row(const Params& P, const Centroids& cen, const LaneTable<OP, AUX>& rt, int64_t row,
                                                  int lane) {
     float v[4 * R], gv[4 * R];
     warp_load_row<OP, AUX, R, VEC, FULL>(P, row, lane, v, gv);
-    warp_compute_row<OP, AUX, R, VEC, FULL, ACC_A>(P, cen, rt, row, lane, v, gv);
+    warp_compute_row<OP, AUX, R, VEC, FULL, ACC_A, PACK>(P, cen, rt, row, lane, v, gv);
 }
 
 // Row order.  The uniform op (forward, every backward mode) gives every row its own warp: one CTA per 8 rows
@@ -406,7 +453,9 @@ constexpr int kMinCtas = (OP == OP_UNIFORM && R == 2 && AUX == (int)BWD_OFF) ? 4
                          : (OP == OP_UNIFORM && R == 8 && AUX != (int)BWD_OFF) ? 2   // 1024-element rows with a gradient: cap at 128 regs
                                                                                : 0;
 
-template <int OP, int AUX, int R, bool VEC, bool ACC_A = false>
+// PACK: 0 = uint8 levels at P.idx8; 1 / 2 / 4 / 8 = P.idx8 receives the levels as packed codes of that width
+// (store_levels; VEC only, every row starting on a byte of the packed stream)
+template <int OP, int AUX, int R, bool VEC, bool ACC_A = false, int PACK = 0>
 __global__ void __launch_bounds__(kWarpCtaThreads, kMinCtas<OP, AUX, R>) warp_rows_kernel(const __grid_constant__ Params P) {
     __shared__ float s_k[OP == OP_NONUNIFORM ? 256 : 1];
     __shared__ float s_t[OP == OP_NONUNIFORM ? 256 : 1];
@@ -433,7 +482,7 @@ __global__ void __launch_bounds__(kWarpCtaThreads, kMinCtas<OP, AUX, R>) warp_ro
                     const bool has_next = next < full_rows;
                     float vn[4 * R], gn[4 * R];
                     if (has_next) warp_load_row<OP, AUX, R, true, true>(P, next, lane, vn, gn);
-                    warp_compute_row<OP, AUX, R, true, true>(P, cen, rt, row, lane, v, gv);
+                    warp_compute_row<OP, AUX, R, true, true, false, PACK>(P, cen, rt, row, lane, v, gv);
                     row = next;
                     if (!has_next) break;
 #pragma unroll
@@ -441,10 +490,10 @@ __global__ void __launch_bounds__(kWarpCtaThreads, kMinCtas<OP, AUX, R>) warp_ro
                 }
             }
         } else {
-            for (; row < full_rows; row += stride) warp_process_row<OP, AUX, R, true, true, ACC_A>(P, cen, rt, row, lane);
+            for (; row < full_rows; row += stride) warp_process_row<OP, AUX, R, true, true, ACC_A, PACK>(P, cen, rt, row, lane);
         }
     }
-    for (; row < P.geo.rows; row += stride) warp_process_row<OP, AUX, R, VEC, false, ACC_A>(P, cen, rt, row, lane);
+    for (; row < P.geo.rows; row += stride) warp_process_row<OP, AUX, R, VEC, false, ACC_A, PACK>(P, cen, rt, row, lane);
 }
 
 // grid of the one-warp-per-row ops: one CTA per 8 rows
