@@ -196,6 +196,18 @@ size_t qd_unpack_model_workspace_bytes(int count);
 int qd_unpack_dequant_model(const qd_packed_tensor* tensors /* HOST array */, int count, int64_t bucket,
                             int levels /* uniform: s in [2, 2^bits]; 0: non-uniform */,
                             void* workspace, size_t workspace_bytes, qd_stream_t stream);
+/* Fully-connected layer straight from packed weights: y[i, o] = sum_k x[i, k] * q[o*K + k] (+ bias[o]) for
+ * x float32[m, K] and y float32[m, O] (K = in_features, O = out_features, both C order), where q is the tensor of
+ * O*K elements that qd_unpack_dequant_* writes from (packed, alpha, beta) at this bucket: the weights are the stored
+ * ones, bit for bit.  levels: uniform s in [2, 2^bits] (points NULL, num_points 0); 0: non-uniform, points[num_points]
+ * with num_points in [1, 2^bits].  bias may be NULL.  Accumulation is float32 fmaf in an order fixed by K and bits
+ * alone (no atomics, no dependence on m, the grid or timing): repeated calls and replicas give identical bits.
+ * 1 <= m <= QD_PACKED_LINEAR_MAX_ROWS, larger m is QD_ERR_UNSUPPORTED (decode, then a dense GEMM).  y must not
+ * overlap x.  Needs no workspace; only enqueues work on `stream`. */
+#define QD_PACKED_LINEAR_MAX_ROWS 64
+int qd_packed_linear(const float* x, int64_t m, int64_t in_features, int64_t out_features, const uint8_t* packed, int bits,
+                     const float* alpha, const float* beta, const float* points, int num_points, int levels, int64_t bucket,
+                     const float* bias, float* y, qd_stream_t stream);
 
 /* ---- next row f2: Huffman-coded storage (the model helpers/functions.py:226-262 only sizes) ----------
  * Canonical code over uint8 symbols, codes of 1..QD_HUFFMAN_MAX_LENGTH bits (built on the host: codec.py).

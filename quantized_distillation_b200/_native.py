@@ -19,6 +19,7 @@ BWD_STE, BWD_TRUNCATED, BWD_MINMAX = 0, 1, 2
 RULE_NEAREST, RULE_MIDPOINT = 0, 1
 SCALE_ABSMAX, SCALE_ABSNORM = 1, 2
 MAX_STAGED_BUCKET = 49152
+PACKED_LINEAR_MAX_ROWS = 64     # QD_PACKED_LINEAR_MAX_ROWS
 
 _p, _i64, _i32, _u64, _f32, _sz = C.c_void_p, C.c_int64, C.c_int, C.c_uint64, C.c_float, C.c_size_t
 
@@ -49,6 +50,7 @@ SIGNATURES = {
     "qd_nonuniform_fwd_packed": (C.c_int, [_p, _p, _i32, _i32, _p, _i32, _p, _p, _i64, _i64, _p, _sz, _p]),
     "qd_unpack_model_workspace_bytes": (_sz, [_i32]),
     "qd_unpack_dequant_model": (C.c_int, [_p, _i32, _i64, _i32, _p, _sz, _p]),
+    "qd_packed_linear": (C.c_int, [_p, _i64, _i64, _i64, _p, _i32, _p, _p, _p, _i32, _i32, _i64, _p, _p, _p]),
     "qd_huffman_encode": (C.c_int, [_p, _i64, _p, _p, _i64, _p, _p, _p]),
     "qd_huffman_decode_dequant_uniform": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _i64, _i64, _i32, _p]),
     "qd_huffman_decode_dequant_nonuniform": (C.c_int, [_p, _i64, _p, _p, _p, _i32, _p, _p, _p, _i64, _i64, _p]),

@@ -924,6 +924,12 @@ def unpack_(pm: PackedModel, model) -> None:
     """Writes every parameter of ``model`` in place from ``pm`` (existing parameter handles stay valid), and its
     persistent buffers when ``pm`` stores them.  Everything is checked before anything is written.  Per device, the
     quantized tensors decode in one launch, straight into parameters that are contiguous float32 on that device."""
+    named, bufs = _check_unpack(pm, model)
+    _unpack_into(pm, named, bufs, skip=())
+
+
+def _check_unpack(pm: PackedModel, model):
+    """(named parameters, persistent buffers) of ``model`` once they are known to match ``pm``; ValueError otherwise."""
     named = list(model.named_parameters())
     if len(named) != len(pm.tensors):
         raise ValueError(f"model has {len(named)} parameters, the packed model {len(pm.tensors)}")
@@ -938,10 +944,16 @@ def unpack_(pm: PackedModel, model) -> None:
         for (name, b), (stored, s) in zip(bufs, pm.buffers):
             if tuple(b.shape) != tuple(s.shape) or b.dtype != s.dtype:
                 raise ValueError(f"buffer {name}: {b.dtype} {tuple(b.shape)} != stored {s.dtype} {tuple(s.shape)} ({stored})")
+    return named, bufs
+
+
+def _unpack_into(pm: PackedModel, named, bufs, skip) -> None:
+    """The writing half of unpack_: every parameter but those whose indices are in ``skip``, then the buffers."""
     default = _packed_device_of(pm)
     groups = {}                                  # device -> parameter indices (host parameters decode on `default`)
     for k, (_, p) in enumerate(named):
-        groups.setdefault(p.device if p.is_cuda else default, []).append(k)
+        if k not in skip:
+            groups.setdefault(p.device if p.is_cuda else default, []).append(k)
     for _, b in bufs:
         if b.is_cuda:
             groups.setdefault(b.device, [])
@@ -971,6 +983,129 @@ def unpack_(pm: PackedModel, model) -> None:
         for (_, b), (_, s) in zip(bufs, pm.buffers or []):
             if not b.is_cuda:
                 b.copy_(s)
+
+
+class PackedLinear(torch.nn.Module):
+    """Inference replacement of an ``nn.Linear`` whose weight stays in its fixed-width stored form (one PackedEntry of
+    a PackedModel: codes, alpha and beta per bucket, points) on the device.  For batches of at most CROSSOVER_ROWS
+    rows, forward runs qd_packed_linear, which reads the codes and never materialises the float32 weight; its weights
+    are the decoded ones bit for bit, the sum is float32 in a fixed order.  Larger batches decode the weight into a
+    scratch tensor (qd_unpack_dequant_*) and call F.linear: exactly what an unpack_-loaded model computes.  Forward
+    only: an input that needs a gradient in grad mode is refused.  No host synchronisation, so it can be captured in
+    a CUDA graph."""
+    # largest batch (rows of x after flattening) that runs on the packed kernel.  Measured (DESIGN.md section 3.7.2):
+    # up to 4 rows the kernel beats decode + F.linear on the AlexNet heads (37.7 M and 16.8 M weights) at every width,
+    # from 16 rows on it loses there; on layers of under a million weights it loses at every batch size.
+    CROSSOVER_ROWS = 4
+
+    def __init__(self, entry: PackedEntry, kind: str, levels, bucket_size, bias: torch.Tensor = None):
+        super().__init__()
+        if not entry.quantized or len(entry.shape) != 2:
+            raise ValueError(f"{entry.name}: a PackedLinear needs a quantized two-dimensional weight")
+        if kind not in ("uniform", "nonuniform"):
+            raise ValueError(f"unknown kind {kind!r}")
+        self.out_features, self.in_features = (int(d) for d in entry.shape)
+        self.kind, self.bits, self.bucket_size = kind, int(entry.bits), bucket_size
+        self.levels = int(levels) if kind == "uniform" else 0
+        dev = entry.packed.device
+        if not dev.type == "cuda":
+            raise ValueError(f"{entry.name}: the packed sections must be on a CUDA device")
+
+        def own(t):                              # a view into a loaded file's region is copied out of it
+            t = t.to(dev).contiguous()
+            return t.clone() if t.untyped_storage().nbytes() > t.numel() * t.element_size() else t
+        self.register_buffer("packed", own(entry.packed), persistent=False)
+        self.register_buffer("alpha", own(entry.alpha.to(torch.float32)), persistent=False)
+        self.register_buffer("beta", own(entry.beta.to(torch.float32)), persistent=False)
+        self.register_buffer("points", None if kind == "uniform" else own(entry.points.reshape(-1).to(torch.float32)), persistent=False)
+        if bias is not None:
+            if tuple(bias.shape) != (self.out_features,):
+                raise ValueError(f"{entry.name}: bias of shape {tuple(bias.shape)}, expected ({self.out_features},)")
+            bias = bias.detach().to(dev, torch.float32).contiguous()
+        self.register_buffer("bias", bias, persistent=False)
+
+    def extra_repr(self) -> str:
+        return (f"in_features={self.in_features}, out_features={self.out_features}, bias={self.bias is not None}, "
+                f"{self.kind}, bits={self.bits}, bucket_size={self.bucket_size}")
+
+    def decoded_weight(self) -> torch.Tensor:
+        """The decoded float32 weight [out_features, in_features], bit for bit what unpack_ writes."""
+        w = torch.empty(self.out_features, self.in_features, dtype=torch.float32, device=self.packed.device)
+        n, b = w.numel(), 0 if self.bucket_size is None else int(self.bucket_size)
+        sp = N.stream_ptr(w.device)
+        if self.kind == "uniform":
+            N.check(N.lib().qd_unpack_dequant_uniform(N.ptr(self.packed), self.bits, N.ptr(self.alpha), N.ptr(self.beta), N.ptr(w), n, b,
+                                                      self.levels, sp))
+        else:
+            N.check(N.lib().qd_unpack_dequant_nonuniform(N.ptr(self.packed), self.bits, N.ptr(self.points), self.points.numel(),
+                                                         N.ptr(self.alpha), N.ptr(self.beta), N.ptr(w), n, b, sp))
+        return w
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        if not torch.is_tensor(x) or not x.is_cuda or x.dtype != torch.float32:
+            raise ValueError("PackedLinear takes a float32 CUDA tensor")
+        if x.device != self.packed.device:
+            raise ValueError(f"input on {x.device}, the packed weight on {self.packed.device}")
+        if x.dim() < 1 or x.shape[-1] != self.in_features:
+            raise ValueError(f"input of shape {tuple(x.shape)}, expected (..., {self.in_features})")
+        if self.packed.dtype != torch.uint8 or any(t is not None and t.dtype != torch.float32 for t in (self.alpha, self.beta, self.points, self.bias)):
+            raise RuntimeError("PackedLinear's sections must stay uint8 codes and float32 scales, points and bias "
+                               "(the module was cast, e.g. by .half() or .double())")
+        if torch.is_grad_enabled() and x.requires_grad:
+            raise RuntimeError("PackedLinear is forward only: it cannot propagate a gradient to its input "
+                               "(run it under torch.no_grad() or torch.inference_mode())")
+        lead = x.shape[:-1]
+        x2 = x.reshape(-1, self.in_features).contiguous()
+        m = x2.shape[0]
+        with torch.cuda.device(x.device):
+            if m > self.CROSSOVER_ROWS:
+                return torch.nn.functional.linear(x2, self.decoded_weight(), self.bias).view(*lead, self.out_features)
+            y = torch.empty(m, self.out_features, dtype=torch.float32, device=x.device)
+            if m:
+                b = 0 if self.bucket_size is None else int(self.bucket_size)
+                N.check(N.lib().qd_packed_linear(N.ptr(x2), m, self.in_features, self.out_features, N.ptr(self.packed), self.bits,
+                                                 N.ptr(self.alpha), N.ptr(self.beta), N.ptr(self.points),
+                                                 0 if self.points is None else self.points.numel(), self.levels, b, N.ptr(self.bias),
+                                                 N.ptr(y), N.stream_ptr(x.device)))
+        return y.view(*lead, self.out_features)
+
+
+def attach_packed_linear_(pm: PackedModel, model) -> list:
+    """unpack_, except that every ``nn.Linear`` whose weight ``pm`` stores quantized is replaced in its parent module
+    by a PackedLinear holding that weight's packed sections (and the Linear's bias, decoded as unpack_ decodes it);
+    the float32 weight is released.  Everything else -- the other parameters, Linear layers kept float32, the stored
+    buffers -- is written exactly as unpack_ writes it, quantized tensors in one launch per device.  Everything is
+    checked before anything is written.  A Linear whose weight is also held elsewhere -- tied to another module (a
+    generator sharing the embedding's matrix) or the Linear itself registered under two parents -- stays an nn.Linear
+    and its weight is decoded as unpack_ decodes it: replacing it in one place would leave the other holder with a
+    weight that was never written.  Returns the names of the replaced modules."""
+    named, bufs = _check_unpack(pm, model)
+    index = {id(p): k for k, (_, p) in enumerate(named)}
+    holders = {}                                 # parameter -> registrations in the module tree, every path counted
+    for _, mod in model.named_modules(remove_duplicate=False):
+        for p in mod._parameters.values():
+            if p is not None:
+                holders[id(p)] = holders.get(id(p), 0) + 1
+    targets = []                                 # (module name, parent, attribute, Linear, weight index)
+    for mname, mod in model.named_modules():
+        if isinstance(mod, torch.nn.Linear) and id(mod.weight) in index and pm.tensors[index[id(mod.weight)]].quantized \
+                and holders[id(mod.weight)] == 1:
+            if not mod.weight.is_cuda:
+                raise ValueError(f"{mname}: a PackedLinear runs on a CUDA device, the Linear is on {mod.weight.device}")
+            parent_name, _, attr = mname.rpartition(".")
+            targets.append((mname, model.get_submodule(parent_name) if parent_name else model, attr, mod, index[id(mod.weight)]))
+    _unpack_into(pm, named, bufs, skip={k for *_, k in targets})
+    movers = {}
+    for mname, parent, attr, lin, k in targets:
+        dev = lin.weight.device
+        t = pm.tensors[k]
+        with torch.cuda.device(dev):
+            move = movers.setdefault(dev, _mover(pm, dev))
+            entry = PackedEntry(t.name, t.shape, bits=t.bits, packed=move(t.packed), alpha=move(t.alpha), beta=move(t.beta),
+                                points=None if t.points is None else t.points.to(dev))
+            layer = PackedLinear(entry, pm.kind, pm.levels, pm.bucket_size, None if lin.bias is None else lin.bias.data)
+        setattr(parent, attr, layer)
+    return [mname for mname, *_ in targets]
 
 
 def save_packed(pm: PackedModel, path) -> int:

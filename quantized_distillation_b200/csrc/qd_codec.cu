@@ -1,5 +1,6 @@
 // qd_codec.cu -- stored-model codecs: histogram of level indices, fixed-width 1/2/4/8-bit packing and its fused
 // unpack + dequantization, and the Huffman-coded stream (qd_huffman.cuh) per tensor and per model.
+#include <algorithm>
 #include <cstring>
 #include <vector>
 
@@ -360,6 +361,279 @@ extern "C" int qd_unpack_dequant_model(const qd_packed_tensor* tensors, int coun
         unpack_dequant_model_kernel<false><<<(unsigned)ctas, 256, 0, st>>>(dev_tensors, dev_start, count, bucket, 0.f);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
+}
+
+// ------------------------------------------------------------------ f2: fully-connected layer on packed weights
+// y[i, o] = sum_k x[i, k] * q[o*K + k] (+ bias[o]) where q is the tensor qd_unpack_dequant_* writes: every weight is
+// from_unit(unit[code], alpha[bucket], beta[bucket]) with the unit table of load_unit_table.
+//
+// A warp owns four consecutive output features and walks their rows together, so that one shared-memory read of x
+// feeds four weight rows.  A row is cut into quads of 4*E codes (E = 32/BITS per 32-bit word; quad d holds columns
+// 4*E*d .. 4*E*d+4*E-1, one 128-bit load when rows start on 16-byte boundaries); lane L takes quads L, L+32, ... in
+// increasing order and sums its elements in column order, one fmaf per element and x row, then the warp folds its
+// 32 partial sums with a fixed xor butterfly.  The order is therefore fixed by K and BITS alone: neither the grid,
+// the chunking of x nor the batch size m changes a single bit of y[i, o].
+//
+// x rows m0 .. m0+MT-1 (MT = 1, 2, 4, 8 accumulators per lane and row, blockIdx.y = row tile) are staged in shared
+// memory, in chunks of kc columns when MT*K floats exceed kPlSmemBytes.  With one chunk the tile is staged once and
+// the CTA walks its slabs of output features; with several, each slab restages them.  The float4 groups of the tile
+// are XOR-swizzled within blocks of eight so that the 32 lanes' reads (stride 4*E floats) hit distinct banks.
+constexpr int kPlWarps = 8;
+constexpr int kPlThreads = kPlWarps * 32;
+constexpr int kPlRowsPerWarp = 4;
+constexpr int kPlSlab = kPlWarps * kPlRowsPerWarp;   // output features per CTA iteration
+constexpr size_t kPlSmemBytes = 96 * 1024;           // x tile, unless one warp-wide step of MT rows needs more
+
+struct PackedLinearArgs {
+    const float* x;
+    const uint8_t* packed;
+    const float* alpha;
+    const float* beta;
+    const float* points;
+    const float* bias;
+    float* y;
+    int64_t m, K, O;
+    int64_t in_bytes;           // ceil(O*K*bits/8)
+    int64_t L, rows;            // bucket row length and bucket count (geometry_of)
+    int64_t step_q, step_r;     // (128*E) / L and (128*E) % L: a lane's bucket cursor from one of its quads to the next
+    int64_t kc;                 // columns per chunk of the x tile, a multiple of 128*E
+    int num_points;
+    float S;
+    bool quad_aligned;          // packed 16-byte aligned and K*bits a multiple of 128: every quad is one aligned load
+    bool x_vec;                 // x 16-byte aligned and K a multiple of 4
+};
+
+// position of float4 group g of a tile row: bits 0-2 XOR-ed with the quad index (E float4 groups per quad)
+template <int BITS>
+__device__ __forceinline__ int pl_slot(int g) {
+    constexpr int shift = BITS == 8 ? 2 : BITS == 4 ? 3 : BITS == 2 ? 4 : 5;   // log2(E)
+    return g ^ ((g >> shift) & 7);
+}
+
+// the 32 code bits of elements e0 .. e0+E-1 (e0*BITS need not be a multiple of 32); bytes past the tensor read as 0
+template <int BITS>
+__device__ __forceinline__ uint32_t pl_word(const PackedLinearArgs& a, int64_t e0) {
+    const int64_t bit = e0 * BITS;
+    const int64_t b0 = bit >> 3;
+    unsigned long long v = 0;
+    for (int i = 0; i < 5; ++i)
+        if (b0 + i < a.in_bytes) v |= (unsigned long long)a.packed[b0 + i] << (8 * i);
+    return (uint32_t)(v >> (unsigned)(bit & 7));
+}
+
+template <int BITS>
+__device__ __forceinline__ uint4 pl_quad(const PackedLinearArgs& a, int64_t e0) {
+    if (a.quad_aligned) return __ldcs(reinterpret_cast<const uint4*>(a.packed + ((e0 * BITS) >> 3)));
+    constexpr int E = 32 / BITS;
+    return make_uint4(pl_word<BITS>(a, e0), pl_word<BITS>(a, e0 + E), pl_word<BITS>(a, e0 + 2 * E), pl_word<BITS>(a, e0 + 3 * E));
+}
+
+template <bool UNIFORM, int BITS, int MT>
+__global__ void __launch_bounds__(kPlThreads, 1) packed_linear_kernel(PackedLinearArgs a) {
+    constexpr int E = 32 / BITS, E4 = E / 4;
+    constexpr unsigned mask = (1u << BITS) - 1u;
+    extern __shared__ float4 s_x[];
+    __shared__ float s_unit[256];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t m0 = (int64_t)blockIdx.y * MT;
+    const int kc4 = (int)(a.kc / 4);
+    const int64_t kq = a.kc / (4 * E);                    // quads per chunk (a multiple of 32)
+    const int64_t qpr = (a.K + 4 * E - 1) / (4 * E);      // quads per weight row
+    const int64_t chunks = (a.K + a.kc - 1) / a.kc;
+    const int64_t slabs = (a.O + kPlSlab - 1) / kPlSlab;
+    auto stage = [&](int64_t c) {
+        const int64_t c0 = c * a.kc;
+        for (int t = threadIdx.x; t < MT * kc4; t += kPlThreads) {
+            const int i = t / kc4, g = t - i * kc4;
+            const int64_t k = c0 + 4 * (int64_t)g;
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (m0 + i < a.m && k < a.K) {
+                const float* xr = a.x + (m0 + i) * a.K;
+                if (a.x_vec) {
+                    v = __ldg(reinterpret_cast<const float4*>(xr + k));
+                } else {
+                    v.x = xr[k];
+                    if (k + 1 < a.K) v.y = xr[k + 1];
+                    if (k + 2 < a.K) v.z = xr[k + 2];
+                    if (k + 3 < a.K) v.w = xr[k + 3];
+                }
+            }
+            s_x[i * kc4 + pl_slot<BITS>(g)] = v;
+        }
+    };
+    load_unit_table<UNIFORM>(s_unit, a.points, a.num_points, a.S);
+    if (chunks == 1) stage(0);
+    __syncthreads();
+    for (int64_t slab = blockIdx.x; slab < slabs; slab += gridDim.x) {
+        // rows past O repeat row O-1: computed, never written
+        int64_t orow[kPlRowsPerWarp];
+#pragma unroll
+        for (int r = 0; r < kPlRowsPerWarp; ++r) {
+            const int64_t o = slab * kPlSlab + warp * kPlRowsPerWarp + r;
+            orow[r] = o < a.O ? o : a.O - 1;
+        }
+        float acc[kPlRowsPerWarp][MT];
+#pragma unroll
+        for (int r = 0; r < kPlRowsPerWarp; ++r)
+#pragma unroll
+            for (int i = 0; i < MT; ++i) acc[r][i] = 0.f;
+        for (int64_t c = 0; c < chunks; ++c) {
+            if (chunks > 1) {
+                __syncthreads();
+                stage(c);
+                __syncthreads();
+            }
+            const int64_t d_first = c * kq + lane, d_end = min(qpr, (c + 1) * kq);
+            if (d_first >= d_end) continue;
+            int64_t bk[kPlRowsPerWarp], rk[kPlRowsPerWarp];   // bucket of the quad's first element, offset in it
+#pragma unroll
+            for (int r = 0; r < kPlRowsPerWarp; ++r) {
+                const int64_t e0 = orow[r] * a.K + d_first * 4 * E;
+                bk[r] = e0 / a.L;
+                rk[r] = e0 - bk[r] * a.L;
+            }
+            for (int64_t d = d_first; d < d_end; d += 32) {
+                uint4 cq[kPlRowsPerWarp];
+#pragma unroll
+                for (int r = 0; r < kPlRowsPerWarp; ++r) cq[r] = pl_quad<BITS>(a, orow[r] * a.K + d * 4 * E);
+                // per row, a cursor (bucket bc, offset rc) that walks the quad's elements in order: alpha / beta are
+                // fetched once per bucket, and a bucket ending inside the quad costs one compare per element
+                float al[kPlRowsPerWarp], be[kPlRowsPerWarp];
+                int64_t bc[kPlRowsPerWarp], rc[kPlRowsPerWarp];
+#pragma unroll
+                for (int r = 0; r < kPlRowsPerWarp; ++r) {
+                    bc[r] = bk[r];
+                    rc[r] = rk[r];
+                    al[r] = __ldg(a.alpha + bc[r]);
+                    be[r] = __ldg(a.beta + bc[r]);
+                }
+                // columns of the quad inside the row: < 4*E only in its last quad
+                const int valid = (int)min((int64_t)(4 * E), a.K - d * 4 * E);
+                const int gbase = (int)(d - c * kq) * E;
+                // loops over the quad's words and float4 groups stay rolled: the kernel body must fit the instruction
+                // cache, since a lane runs it only a few times per launch
+#pragma unroll 1
+                for (int u = 0; u < 4; ++u) {
+#pragma unroll 1
+                    for (int t = 0; t < E4; ++t) {
+                        float q[kPlRowsPerWarp][4];
+#pragma unroll
+                        for (int r = 0; r < kPlRowsPerWarp; ++r) {
+                            const uint32_t cw = u == 0 ? cq[r].x : u == 1 ? cq[r].y : u == 2 ? cq[r].z : cq[r].w;
+#pragma unroll
+                            for (int jj = 0; jj < 4; ++jj) {
+                                const int jw = 4 * t + jj, j = u * E + jw;
+                                q[r][jj] = j < valid ? from_unit(s_unit[(cw >> (jw * BITS)) & mask], al[r], be[r]) : 0.f;
+                                if (++rc[r] == a.L) {                  // next element starts bucket bc + 1
+                                    rc[r] = 0;
+                                    const int64_t b = min(++bc[r], a.rows - 1);
+                                    al[r] = __ldg(a.alpha + b);
+                                    be[r] = __ldg(a.beta + b);
+                                }
+                            }
+                        }
+#pragma unroll
+                        for (int i = 0; i < MT; ++i) {
+                            const float4 xv = s_x[i * kc4 + pl_slot<BITS>(gbase + u * E4 + t)];
+#pragma unroll
+                            for (int r = 0; r < kPlRowsPerWarp; ++r) {
+                                acc[r][i] = __fmaf_rn(xv.x, q[r][0], acc[r][i]);
+                                acc[r][i] = __fmaf_rn(xv.y, q[r][1], acc[r][i]);
+                                acc[r][i] = __fmaf_rn(xv.z, q[r][2], acc[r][i]);
+                                acc[r][i] = __fmaf_rn(xv.w, q[r][3], acc[r][i]);
+                            }
+                        }
+                    }
+                }
+#pragma unroll
+                for (int r = 0; r < kPlRowsPerWarp; ++r) {
+                    bk[r] += a.step_q;
+                    rk[r] += a.step_r;
+                    if (rk[r] >= a.L) { rk[r] -= a.L; ++bk[r]; }
+                }
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < kPlRowsPerWarp; ++r) {
+            const int64_t o = slab * kPlSlab + warp * kPlRowsPerWarp + r;
+            const float b = (a.bias != nullptr && o < a.O) ? __ldg(a.bias + o) : 0.f;
+#pragma unroll
+            for (int i = 0; i < MT; ++i) {
+                float s = warp_sum(acc[r][i]);
+                if (a.bias != nullptr) s = __fadd_rn(s, b);
+                if (lane == 0 && o < a.O && m0 + i < a.m) a.y[(m0 + i) * a.O + o] = s;
+            }
+        }
+    }
+}
+
+template <int MT, bool UNIFORM, int BITS>
+static int launch_packed_linear(PackedLinearArgs a, cudaStream_t st) {
+    constexpr int64_t step_cols = 32 * 4 * (32 / BITS);   // columns of one warp-wide step
+    const int64_t room = std::max<int64_t>(1, (int64_t)(kPlSmemBytes / (MT * sizeof(float))) / step_cols) * step_cols;
+    a.kc = std::min(room, (a.K + step_cols - 1) / step_cols * step_cols);
+    a.step_q = step_cols / a.L;
+    a.step_r = step_cols % a.L;
+    const size_t smem = (size_t)MT * a.kc * sizeof(float);
+    auto kern = packed_linear_kernel<UNIFORM, BITS, MT>;
+    static size_t opted[64] = {};
+    int rc = opt_in_smem((const void*)kern, smem, opted);
+    if (rc) return rc;
+    const int64_t row_tiles = (a.m + MT - 1) / MT;
+    int grid;
+    const int64_t slabs = (a.O + kPlSlab - 1) / kPlSlab;
+    rc = resident_grid((const void*)kern, kPlThreads, smem, slabs * row_tiles, &grid);
+    if (rc) return rc;
+    grid = std::max(1, grid / (int)row_tiles);           // at most one resident wave over all row tiles
+    kern<<<dim3((unsigned)grid, (unsigned)row_tiles), kPlThreads, smem, st>>>(a);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+extern "C" int qd_packed_linear(const float* x, int64_t m, int64_t in_features, int64_t out_features, const uint8_t* packed,
+                                int bits, const float* alpha, const float* beta, const float* points, int num_points, int levels,
+                                int64_t bucket, const float* bias, float* y, qd_stream_t stream) {
+    if (x == nullptr || packed == nullptr || alpha == nullptr || beta == nullptr || y == nullptr)
+        return fail(QD_ERR_INVALID_ARG, "NULL argument");
+    if (m < 1) return fail(QD_ERR_INVALID_ARG, "m must be >= 1 (got %lld)", (long long)m);
+    if (m > QD_PACKED_LINEAR_MAX_ROWS)
+        return fail(QD_ERR_UNSUPPORTED, "m = %lld rows: the packed linear kernel serves at most %d", (long long)m, QD_PACKED_LINEAR_MAX_ROWS);
+    if (in_features < 1 || out_features < 1) return fail(QD_ERR_INVALID_ARG, "in_features and out_features must be >= 1");
+    if (in_features > INT64_MAX / 8 / out_features) return fail(QD_ERR_INVALID_ARG, "in_features * out_features is too large");
+    if (!bits_ok(bits)) return fail(QD_ERR_INVALID_ARG, "bits must be 1, 2, 4 or 8");
+    const bool uniform = levels != 0;
+    if (uniform) {
+        if (points != nullptr || num_points != 0) return fail(QD_ERR_INVALID_ARG, "uniform weights have no points (points NULL, num_points 0)");
+        if (levels < 2 || levels > (1 << bits)) return fail(QD_ERR_INVALID_ARG, "levels must be in [2, 2^bits]");
+    } else if (points == nullptr || num_points < 1 || num_points > (1 << bits)) {
+        return fail(QD_ERR_INVALID_ARG, "num_points must be in [1, 2^bits]");
+    }
+    Geometry geo;
+    const int64_t n = in_features * out_features;
+    if (geometry_of(n, bucket, &geo)) return fail(QD_ERR_INVALID_ARG, "bucket must be >= 0");
+    const uintptr_t xb = reinterpret_cast<uintptr_t>(x), xe = xb + (uintptr_t)(m * in_features) * sizeof(float);
+    const uintptr_t yb = reinterpret_cast<uintptr_t>(y), ye = yb + (uintptr_t)(m * out_features) * sizeof(float);
+    if (xb < ye && yb < xe) return fail(QD_ERR_INVALID_ARG, "y must not overlap x");
+    PackedLinearArgs a{};
+    a.x = x, a.packed = packed, a.alpha = alpha, a.beta = beta, a.points = points, a.bias = bias, a.y = y;
+    a.m = m, a.K = in_features, a.O = out_features;
+    a.in_bytes = (n * bits + 7) / 8;
+    a.L = geo.row_len;
+    a.rows = geo.rows;
+    a.num_points = num_points;
+    a.S = uniform ? (float)(levels - 1) : 0.f;
+    a.quad_aligned = aligned16(packed) && (in_features * bits) % 128 == 0;
+    a.x_vec = aligned16(x) && in_features % 4 == 0;
+    cudaStream_t st = as_stream(stream);
+    auto go = [&](auto mt) {
+        return with_bits(bits, [&](auto b) {
+            return uniform ? launch_packed_linear<mt, true, b>(a, st) : launch_packed_linear<mt, false, b>(a, st);
+        });
+    };
+    if (m == 1) return go(std::integral_constant<int, 1>{});
+    if (m == 2) return go(std::integral_constant<int, 2>{});
+    if (m <= 4) return go(std::integral_constant<int, 4>{});
+    return go(std::integral_constant<int, 8>{});
 }
 
 // ------------------------------------------------------------------ f2: Huffman-coded storage (qd_huffman.cuh)
