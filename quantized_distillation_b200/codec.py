@@ -45,71 +45,83 @@ def _rows(n, bucket_size):
     return N.geometry(n, 0 if bucket_size is None else int(bucket_size))[0]
 
 
+def _bucket(bucket_size) -> int:
+    """The C ABI's bucket argument: 0 for one bucket per tensor."""
+    return 0 if bucket_size is None else int(bucket_size)
+
+
+def _levels(x, s, pts, bucket_size, rule, sp):
+    """(uint8 level indices, alpha, beta) of x (contiguous float32 on the current device) from the fused forward op:
+    uniformQuantization's s levels when ``pts`` is None, else nonUniformQuantization's over ``pts`` with ``rule``."""
+    n, b = x.numel(), _bucket(bucket_size)
+    rows = _rows(n, bucket_size)
+    alpha = torch.empty(rows, device=x.device)
+    beta = torch.empty(rows, device=x.device)
+    idx = torch.empty(n, dtype=torch.uint8, device=x.device)
+    ws = N.workspace(n, b, x.device)
+    if pts is None:
+        N.check(N.lib().qd_uniform_fwd(N.ptr(x), None, N.ptr(idx), N.ptr(alpha), N.ptr(beta), None, None, n, b, int(s), None, 0.0,
+                                       0, 0, 0, N.ptr(ws), ws.numel(), sp))
+    else:
+        N.check(N.lib().qd_nonuniform_fwd(N.ptr(x), N.ptr(pts), pts.numel(), N.RULE_MIDPOINT if rule == "midpoint" else N.RULE_NEAREST,
+                                          None, N.ptr(idx), None, N.ptr(alpha), N.ptr(beta), n, b, None, 0.0, N.ptr(ws), ws.numel(), sp))
+    return idx, alpha, beta
+
+
+def _encode(tensor, s, bucket_size, points=None, rule="nearest") -> PackedTensor:
+    """Level indices of ``tensor`` (uniform with s levels, or non-uniform on ``points``) packed at the width they need."""
+    x = tensor.detach().cuda().contiguous().float()
+    pts = None if points is None else torch.as_tensor(points, dtype=torch.float32).detach().to(x.device).contiguous()
+    sp = N.stream_ptr(x.device)
+    idx, alpha, beta = _levels(x, s, pts, bucket_size, rule, sp)
+    levels = int(s) if pts is None else pts.numel()
+    bits = bits_for(levels)
+    packed = torch.empty((x.numel() * bits + 7) // 8, dtype=torch.uint8, device=x.device)
+    N.check(N.lib().qd_pack_indices(N.ptr(idx), N.ptr(packed), x.numel(), bits, sp))
+    return PackedTensor(packed, alpha, beta, tensor.shape, bits, levels, bucket_size, points=pts)
+
+
 def encode_uniform(tensor: torch.Tensor, s: int, bucket_size=None) -> PackedTensor:
     """uniformQuantization (quant_functions.py:155-194) straight to packed codes: the float
     fake-quantized tensor is never written."""
     N.require_cuda()
     if s > 256:
         raise ValueError("the packed codec stores at most 8 bits per weight")
-    x = tensor.detach().cuda().contiguous().float()
-    n = x.numel()
-    b = 0 if bucket_size is None else int(bucket_size)
-    rows = _rows(n, bucket_size)
-    alpha = torch.empty(rows, device=x.device)
-    beta = torch.empty(rows, device=x.device)
-    idx = torch.empty(n, dtype=torch.uint8, device=x.device)
-    ws = N.workspace(n, b, x.device)
-    sp = N.stream_ptr(x.device)
-    N.check(N.lib().qd_uniform_fwd(N.ptr(x), None, N.ptr(idx), N.ptr(alpha), N.ptr(beta), None, None, n, b, int(s), None, 0.0,
-                                   0, 0, 0, N.ptr(ws), ws.numel(), sp))
-    bits = bits_for(s)
-    packed = torch.empty((n * bits + 7) // 8, dtype=torch.uint8, device=x.device)
-    N.check(N.lib().qd_pack_indices(N.ptr(idx), N.ptr(packed), n, bits, sp))
-    return PackedTensor(packed, alpha, beta, tensor.shape, bits, int(s), bucket_size)
+    return _encode(tensor, s, bucket_size)
 
 
 def encode_nonuniform(tensor: torch.Tensor, points, bucket_size=None, rule="nearest") -> PackedTensor:
     N.require_cuda()
-    x = tensor.detach().cuda().contiguous().float()
-    pts = torch.as_tensor(points, dtype=torch.float32).detach().to(x.device).contiguous()
-    n = x.numel()
-    b = 0 if bucket_size is None else int(bucket_size)
-    rows = _rows(n, bucket_size)
-    alpha = torch.empty(rows, device=x.device)
-    beta = torch.empty(rows, device=x.device)
-    idx = torch.empty(n, dtype=torch.uint8, device=x.device)
-    ws = N.workspace(n, b, x.device)
-    sp = N.stream_ptr(x.device)
-    N.check(N.lib().qd_nonuniform_fwd(N.ptr(x), N.ptr(pts), pts.numel(), N.RULE_MIDPOINT if rule == "midpoint" else N.RULE_NEAREST,
-                                      None, N.ptr(idx), None, N.ptr(alpha), N.ptr(beta), n, b, None, 0.0, N.ptr(ws), ws.numel(), sp))
-    bits = bits_for(pts.numel())
-    packed = torch.empty((n * bits + 7) // 8, dtype=torch.uint8, device=x.device)
-    N.check(N.lib().qd_pack_indices(N.ptr(idx), N.ptr(packed), n, bits, sp))
-    return PackedTensor(packed, alpha, beta, tensor.shape, bits, pts.numel(), bucket_size, points=pts)
+    return _encode(tensor, None, bucket_size, points, rule)
+
+
+def _unpack(packed, bits, alpha, beta, points, levels, bucket_size, out: torch.Tensor) -> torch.Tensor:
+    """Decodes one tensor's packed codes into ``out`` (contiguous float32, on their device): qd_unpack_dequant_uniform
+    with ``levels``, or qd_unpack_dequant_nonuniform on ``points`` when they are given."""
+    n, b, sp = out.numel(), _bucket(bucket_size), N.stream_ptr(out.device)
+    if points is None:
+        N.check(N.lib().qd_unpack_dequant_uniform(N.ptr(packed), bits, N.ptr(alpha), N.ptr(beta), N.ptr(out), n, b, levels, sp))
+    else:
+        N.check(N.lib().qd_unpack_dequant_nonuniform(N.ptr(packed), bits, N.ptr(points), points.numel(), N.ptr(alpha), N.ptr(beta),
+                                                     N.ptr(out), n, b, sp))
+    return out
 
 
 def decode(pt: PackedTensor) -> torch.Tensor:
     """Packed codes -> the fake-quantized float32 tensor (bit-identical to the fused op)."""
     N.require_cuda()
-    n = 1
-    for d in pt.shape:
-        n *= int(d)
-    out = torch.empty(n, dtype=torch.float32, device=pt.packed.device)
-    b = 0 if pt.bucket_size is None else int(pt.bucket_size)
-    sp = N.stream_ptr(out.device)
-    if pt.points is None:
-        N.check(N.lib().qd_unpack_dequant_uniform(N.ptr(pt.packed), pt.bits, N.ptr(pt.alpha), N.ptr(pt.beta), N.ptr(out), n, b,
-                                                  pt.levels, sp))
-    else:
-        N.check(N.lib().qd_unpack_dequant_nonuniform(N.ptr(pt.packed), pt.bits, N.ptr(pt.points), pt.points.numel(),
-                                                     N.ptr(pt.alpha), N.ptr(pt.beta), N.ptr(out), n, b, sp))
-    return out.view(pt.shape)
+    out = torch.empty(int(math.prod(pt.shape)), dtype=torch.float32, device=pt.packed.device)
+    return _unpack(pt.packed, pt.bits, pt.alpha, pt.beta, pt.points, pt.levels, pt.bucket_size, out).view(pt.shape)
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# Huffman-coded model container.  The code is the one the size accounting uses (huffman_code_of_histogram over
-# the level histogram of every quantized tensor), made canonical; the stream and table layout are declared in
-# include/qd_b200.h and produced / consumed by csrc/qd_huffman.cuh.
+# Stored models.  Two containers share one file layout -- magic, version, reserved 0, JSON header length, the JSON
+# header, then 16-byte-aligned little-endian sections -- one reader with one set of checks, and one whole-model decode
+# protocol (a descriptor per quantized tensor, every tensor's points in one upload, one launch per device).
+#
+# Huffman-coded: the code is the one the size accounting uses (huffman_code_of_histogram over the level histogram of
+# every quantized tensor), made canonical; the stream and table layout are declared in include/qd_b200.h and produced /
+# consumed by csrc/qd_huffman.cuh.
 HUFFMAN_CHUNK = 1024            # symbols per independently decodable chunk (QD_HUFFMAN_CHUNK)
 HUFFMAN_MAX_LENGTH = 57         # QD_HUFFMAN_MAX_LENGTH
 HUFFMAN_LUT_BITS = 11           # QD_HUFFMAN_LUT_BITS
@@ -117,6 +129,12 @@ HUFFMAN_TABLE_BYTES = 13328     # sizeof(qd_huffman_table)
 FILE_MAGIC = b"QDHUFF\x00\x00"
 FILE_VERSION = 1                # parameters only
 FILE_VERSION_BUFFERS = 2        # parameters + persistent buffers: a version-1 reader refuses it rather than drop them
+# Fixed-width: every quantized tensor is stored as its packed codes (qd_pack_indices layout, its own width
+# bits_for(levels or points)) + (alpha, beta) per bucket: the size get_size_reduction accounts for.  It decodes at HBM
+# rate in one launch (qd_unpack_dequant_model) and can be read at any bucket without a chunk index.  Buffers are stored
+# as in Huffman version 2.
+PACKED_MAGIC = b"QDPACK\x00\x00"
+PACKED_VERSION = 1
 _PREFIX = struct.Struct("<8sIIQ")   # magic, version, reserved (0), JSON header length
 _ALIGN = 16
 # dtypes a stored buffer may have, by their name in the header
@@ -125,6 +143,10 @@ _BUFFER_DTYPES = {"float32": torch.float32, "int64": torch.int64}
 _MODEL_TENSOR = np.dtype([("words", "<u8"), ("chunk_offsets", "<u8"), ("alpha", "<u8"), ("beta", "<u8"), ("points", "<u8"),
                           ("q", "<u8"), ("num_words", "<i8"), ("n", "<i8"), ("num_points", "<i4"), ("reserved", "<i4")])
 assert _MODEL_TENSOR.itemsize == 72
+# qd_packed_tensor (include/qd_b200.h): one entry of the whole-model unpack
+_PACKED_TENSOR = np.dtype([("packed", "<u8"), ("alpha", "<u8"), ("beta", "<u8"), ("points", "<u8"), ("q", "<u8"), ("n", "<i8"),
+                           ("bits", "<i4"), ("num_points", "<i4")])
+assert _PACKED_TENSOR.itemsize == 56
 
 
 def huffman_code_lengths(counts) -> dict:
@@ -215,7 +237,53 @@ class HuffmanTensor:
 
 
 @dataclass
-class CompressedModel:
+class PackedEntry:
+    """One parameter of a PackedModel: packed codes + (alpha, beta) per bucket, or float32 as is."""
+    name: str
+    shape: tuple
+    bits: int = 0                       # code width of a quantized tensor: 1, 2, 4 or 8
+    packed: torch.Tensor = None         # uint8[ceil(n * bits / 8)]
+    alpha: torch.Tensor = None          # float32[rows]
+    beta: torch.Tensor = None
+    points: torch.Tensor = None         # non-uniform: this tensor's centroids
+    raw: torch.Tensor = None            # unquantized tensor (float32)
+
+    @property
+    def numel(self) -> int:
+        return int(math.prod(self.shape))
+
+    @property
+    def quantized(self) -> bool:
+        return self.raw is None
+
+
+class _Container:
+    """What CompressedModel and PackedModel share: the file layout, its size accounting, the reader and the
+    whole-model decode are written once (module functions below).  Each format names its sections, magic, versions,
+    descriptor and native decode, and supplies its extra header and entry fields, the reading of one quantized entry
+    and the descriptor of one tensor."""
+
+    def size_breakdown(self) -> dict:
+        """Bytes of the saved file by what they hold: the format's code bytes, then scales, unquantized parameters,
+        stored buffers, header and alignment.  Huffman: code_bits / 8 + scale_bytes + unquantized_bytes is what
+        get_size_quantized_model accounts for.  Fixed-width: code_bytes + scale_bytes is what get_size_reduction
+        accounts for, up to the round-up of each tensor's codes to whole bytes.  The rest is the price of the format."""
+        header, sections, data_bytes = _layout(self)
+        q = [t for t in self.tensors if t.quantized]
+        start = _align(_PREFIX.size + len(header))
+        return {
+            **self._code_sizes(q),
+            "scale_bytes": sum((t.alpha.numel() + t.beta.numel()) * 4 for t in q),
+            "unquantized_bytes": sum(t.raw.numel() * 4 for t in self.tensors if not t.quantized),
+            "buffer_bytes": sum(b.numel() * b.element_size() for _, b in self.buffers or []),
+            "header_bytes": _PREFIX.size + len(header),
+            "alignment_bytes": start - _PREFIX.size - len(header) + data_bytes - sum(nb for _, nb, _ in sections),
+            "file_bytes": start + data_bytes,
+        }
+
+
+@dataclass
+class CompressedModel(_Container):
     """A model whose quantized parameters are Huffman-coded (compress_model, load_compressed)."""
     kind: str                       # "uniform" | "nonuniform"
     levels: object                  # uniform: s; non-uniform: None
@@ -229,40 +297,140 @@ class CompressedModel:
     # a loaded file's data region: every section is a view into it, so it reaches a device in one copy
     _data: torch.Tensor = field(default=None, init=False, repr=False, compare=False)
 
+    _SECTIONS = ("words", "chunk_offsets", "alpha", "beta")
+    _MAGIC, _VERSIONS, _FILE, _WHAT = FILE_MAGIC, (FILE_VERSION, FILE_VERSION_BUFFERS), "Huffman-coded model file", "compressed model"
+    _ENTRY, _DESCRIPTOR = HuffmanTensor, _MODEL_TENSOR
+    _WORKSPACE, _DECODE = "qd_huffman_model_workspace_bytes", "qd_huffman_decode_dequant_model"
+
     def table(self, device) -> torch.Tensor:
         key = str(device)
         if key not in self._tables:
             self._tables[key] = torch.from_numpy(huffman_table(self.code_lengths)).to(device)
         return self._tables[key]
 
-    def size_breakdown(self) -> dict:
-        """Bytes of the saved file by what they hold.  code_bits / 8 + scale_bytes + unquantized_bytes is what
-        get_size_quantized_model accounts for; the rest is the price of the format (and the stored buffers)."""
-        header, sections, data_bytes = _layout(self)
-        q = [t for t in self.tensors if t.quantized]
+    def _code_sizes(self, q) -> dict:
         code_bits = sum(t.code_bits for t in q)
-        section_bytes = sum(nb for _, nb, _ in sections)
-        return {
-            "code_bits": code_bits,
-            "padding_bits": sum(t.words.numel() for t in q) * 32 - code_bits,
-            "chunk_index_bytes": sum(t.chunk_offsets.numel() * 4 for t in q),
-            "scale_bytes": sum((t.alpha.numel() + t.beta.numel()) * 4 for t in q),
-            "unquantized_bytes": sum(t.raw.numel() * 4 for t in self.tensors if not t.quantized),
-            "buffer_bytes": sum(b.numel() * b.element_size() for _, b in self.buffers or []),
-            "header_bytes": _PREFIX.size + len(header),
-            "alignment_bytes": _align(_PREFIX.size + len(header)) - _PREFIX.size - len(header) + data_bytes - section_bytes,
-            "file_bytes": _align(_PREFIX.size + len(header)) + data_bytes,
-        }
+        return {"code_bits": code_bits, "padding_bits": sum(t.words.numel() for t in q) * 32 - code_bits,
+                "chunk_index_bytes": sum(t.chunk_offsets.numel() * 4 for t in q)}
+
+    def _version(self) -> int:
+        # the buffers' key exists only in a version-2 header, so a file without buffers is exactly what version 1 was
+        return FILE_VERSION if self.buffers is None else FILE_VERSION_BUFFERS
+
+    def _header(self, common: dict) -> dict:
+        return {"chunk": self.chunk, **common, "code": [[int(s), int(l)] for s, l in sorted(self.code_lengths.items())]}
+
+    @staticmethod
+    def _entry_fields(t) -> dict:
+        return {"code_bits": int(t.code_bits)}
+
+    @staticmethod
+    def _read_header(h, version, levels, bad) -> dict:
+        if ("buffers" in h) != (version == FILE_VERSION_BUFFERS):
+            bad(f"a version-{version} file {'must not list' if version == FILE_VERSION else 'must list its'} buffers")
+        try:
+            chunk, code = h["chunk"], {int(s): int(l) for s, l in h["code"]}
+        except (ValueError, KeyError, TypeError) as e:
+            bad(f"unreadable header ({e})")
+        if chunk != HUFFMAN_CHUNK:
+            bad(f"chunk of {chunk} symbols, this reader decodes {HUFFMAN_CHUNK}")
+        if len(code) != len(h["code"]):
+            bad("a symbol appears twice in the code")
+        try:
+            check_code_lengths(code)
+        except ValueError as e:
+            bad(str(e))
+        if levels is not None and max(code) >= levels:
+            bad("a code symbol is not a level")
+        return {"code_lengths": code}
+
+    @staticmethod
+    def _read_entry(e, name, n, levels, pts, section, bad) -> dict:
+        # the code is model-wide: a tensor with fewer points than another never emits the higher symbols
+        if pts is not None and not 1 <= pts.numel() <= 256:
+            bad(f"{name}: {pts.numel()} points, expected 1 to 256")
+        span = e["sections"]["words"]
+        words_nb = span[1] if isinstance(span, list) and len(span) == 2 else None
+        if not isinstance(words_nb, int) or words_nb < 0 or words_nb % 4:
+            bad(f"{name}: section words out of range")
+        words = section(e, "words", torch.int32, words_nb)
+        offs = section(e, "chunk_offsets", torch.int32, 4 * -(-n // HUFFMAN_CHUNK))
+        o = offs.numpy().view(np.uint32).astype(np.int64)
+        if o[0] != 0 or np.any(np.diff(o) < 0) or o[-1] > words.numel():
+            bad(f"{name}: chunk offsets out of range")
+        return {"words": words, "chunk_offsets": offs, "code_bits": int(e.get("code_bits", 0))}
+
+    def _descriptor(self, t, sections, points, num_points, out) -> tuple:
+        words, offs, alpha, beta = sections
+        return (N.ptr(words) if words.numel() else 0, N.ptr(offs), N.ptr(alpha), N.ptr(beta), points, N.ptr(out), words.numel(),
+                t.numel, num_points, 0)
+
+    def _decode_tables(self, dev) -> tuple:
+        return (N.ptr(self.table(dev)),)
+
+
+@dataclass
+class PackedModel(_Container):
+    """A model whose quantized parameters are stored fixed-width (pack_model, load_packed)."""
+    kind: str                       # "uniform" | "nonuniform"
+    levels: object                  # uniform: s; non-uniform: None
+    bucket_size: object
+    tensors: list
+    # persistent buffers as [(name, tensor)] in state_dict() order; None: not stored
+    buffers: list = None
+    # a loaded file's data region: every section is a view into it, so it reaches a device in one copy
+    _data: torch.Tensor = field(default=None, init=False, repr=False, compare=False)
+
+    _SECTIONS = ("packed", "alpha", "beta")
+    _MAGIC, _VERSIONS, _FILE, _WHAT = PACKED_MAGIC, (PACKED_VERSION,), "fixed-width model file", "packed model"
+    _ENTRY, _DESCRIPTOR = PackedEntry, _PACKED_TENSOR
+    _WORKSPACE, _DECODE = "qd_unpack_model_workspace_bytes", "qd_unpack_dequant_model"
+
+    @staticmethod
+    def _code_sizes(q) -> dict:
+        return {"code_bytes": sum(t.packed.numel() for t in q)}
+
+    @staticmethod
+    def _version() -> int:
+        return PACKED_VERSION
+
+    @staticmethod
+    def _header(common: dict) -> dict:
+        return common
+
+    @staticmethod
+    def _entry_fields(t) -> dict:
+        return {"bits": int(t.bits)}
+
+    @staticmethod
+    def _read_header(h, version, levels, bad) -> dict:
+        if not any(isinstance(e, dict) and e.get("quantized") is True for e in h["tensors"]):
+            bad("no quantized tensor")
+        return {}
+
+    @staticmethod
+    def _read_entry(e, name, n, levels, pts, section, bad) -> dict:
+        bits = e.get("bits")
+        if bits not in (1, 2, 4, 8) or isinstance(bits, bool):
+            bad(f"{name}: bits must be 1, 2, 4 or 8")
+        if pts is None and levels > 1 << bits:
+            bad(f"{name}: {levels} levels do not fit in {bits}-bit codes")
+        if pts is not None and not 1 <= pts.numel() <= 1 << bits:
+            bad(f"{name}: {pts.numel()} points do not fit in {bits}-bit codes")
+        return {"bits": bits, "packed": section(e, "packed", torch.uint8, (n * bits + 7) // 8)}
+
+    @staticmethod
+    def _descriptor(t, sections, points, num_points, out) -> tuple:
+        packed, alpha, beta = sections
+        return (N.ptr(packed), N.ptr(alpha), N.ptr(beta), points, N.ptr(out), t.numel, t.bits, num_points)
+
+    @staticmethod
+    def _decode_tables(dev) -> tuple:
+        return ()
 
 
 def _align(x: int) -> int:
     return (x + _ALIGN - 1) // _ALIGN * _ALIGN
-
-
-def _sections_of(t: HuffmanTensor):
-    if not t.quantized:
-        return [("raw", t.raw)]
-    return [("words", t.words), ("chunk_offsets", t.chunk_offsets), ("alpha", t.alpha), ("beta", t.beta)]
 
 
 def _dtype_name(tensor) -> str:
@@ -272,34 +440,49 @@ def _dtype_name(tensor) -> str:
     return name
 
 
-def _layout(cm: CompressedModel):
-    """(JSON header bytes, [(tensor, nbytes, offset)], data bytes); offsets are relative to the first 16-byte
-    boundary after the header.  The buffers' sections follow the parameters' and their key exists only in a
-    version-2 header, so a file without buffers is laid out exactly as version 1 always was."""
+def _layout(m):
+    """(JSON header bytes, [(tensor, nbytes, offset)], data bytes) of a CompressedModel or PackedModel; offsets are
+    relative to the first 16-byte boundary after the header, every section starts on a 16-byte boundary.  The
+    buffers' sections follow the parameters', and the header lists buffers only when the model stores them."""
     sections, entries, off = [], [], 0
-    for t in cm.tensors:
+
+    def place(tensor):
+        nonlocal off
+        nb = tensor.numel() * tensor.element_size()
+        sections.append((tensor, nb, off))
+        span, off = [off, nb], _align(off + nb)
+        return span
+
+    for t in m.tensors:
         e = {"name": t.name, "shape": list(t.shape), "dtype": "float32", "quantized": t.quantized, "sections": {}}
         if t.quantized:
-            e["code_bits"] = int(t.code_bits)
+            e.update(m._entry_fields(t))
             if t.points is not None:
                 e["points"] = [float(v) for v in t.points.detach().cpu().numpy().astype(np.float32)]
-        for name, tensor in _sections_of(t):
-            nb = tensor.numel() * 4
-            e["sections"][name] = [off, nb]
-            sections.append((tensor, nb, off))
-            off = _align(off + nb)
+        for name in m._SECTIONS if t.quantized else ("raw",):
+            e["sections"][name] = place(getattr(t, name))
         entries.append(e)
-    buffers = []
-    for name, b in cm.buffers or []:
-        nb = b.numel() * b.element_size()
-        buffers.append({"name": name, "shape": list(b.shape), "dtype": _dtype_name(b), "section": [off, nb]})
-        sections.append((b, nb, off))
-        off = _align(off + nb)
-    header = {"chunk": cm.chunk, "kind": cm.kind, "levels": cm.levels, "bucket": cm.bucket_size,
-              "code": [[int(s), int(l)] for s, l in sorted(cm.code_lengths.items())], "tensors": entries, "data_bytes": off}
-    if cm.buffers is not None:
+    buffers = [{"name": name, "shape": list(b.shape), "dtype": _dtype_name(b), "section": place(b)} for name, b in m.buffers or []]
+    header = {**m._header({"kind": m.kind, "levels": m.levels, "bucket": m.bucket_size}), "tensors": entries, "data_bytes": off}
+    if m.buffers is not None:
         header["buffers"] = buffers
     return json.dumps(header, separators=(",", ":")).encode("utf-8"), sections, off
+
+
+def _write_container(m, path) -> int:
+    """prefix (magic, version, 0, header length), the JSON header, then every section little-endian at its offset from
+    the first 16-byte boundary after the header.  Returns the file size."""
+    header, sections, data_bytes = _layout(m)
+    start = _align(_PREFIX.size + len(header))
+    buf = bytearray(start + data_bytes)
+    buf[:_PREFIX.size] = _PREFIX.pack(m._MAGIC, m._version(), 0, len(header))
+    buf[_PREFIX.size:_PREFIX.size + len(header)] = header
+    little = {torch.int32: "<i4", torch.float32: "<f4", torch.int64: "<i8", torch.uint8: "u1"}
+    for tensor, nb, off in sections:
+        buf[start + off:start + off + nb] = tensor.detach().contiguous().cpu().numpy().astype(little[tensor.dtype], copy=False).tobytes()
+    with open(path, "wb") as f:
+        f.write(buf)
+    return len(buf)
 
 
 def _persistent_buffers(model):
@@ -308,10 +491,306 @@ def _persistent_buffers(model):
     return [(k, v) for k, v in model.state_dict(keep_vars=True).items() if torch.is_tensor(v) and id(v) not in params]
 
 
-def _selected(named, quantize_first_and_last_layer):
-    """Indices of the quantized parameters: all, or all but the first and the last, exactly as
-    get_size_quantized_model selects them."""
-    return set(range(len(named))) if quantize_first_and_last_layer is True else set(range(1, len(named) - 1))
+def _flat(p, dev):
+    return p.detach().to(dev, torch.float32).contiguous().view(-1)
+
+
+def _points(points, dev):
+    return torch.as_tensor(points, dtype=torch.float32).detach().to(dev).contiguous().view(-1)
+
+
+def _quantization_plan(model, numBits, quantize_first_and_last_layer, points, rule, include_buffers):
+    """The arguments of compress_model and pack_model, checked before any device work: (named parameters,
+    {index of a quantized parameter: its points, None when uniform}, s (uniform) or None, the persistent buffers copied
+    to the device or None, the device).  The quantized parameters are all of them, or all but the first and the last,
+    exactly as get_size_quantized_model selects them."""
+    buffers = None
+    if include_buffers:
+        buffers = _persistent_buffers(model)
+        for _, b in buffers:
+            _dtype_name(b)
+    if (numBits is None) == (points is None):
+        raise ValueError("give numBits (uniform) or points (non-uniform), not both")
+    named = list(model.named_parameters())
+    order = list(range(len(named))) if quantize_first_and_last_layer is True else list(range(1, len(named) - 1))
+    if not order:
+        raise ValueError("no parameter is selected for quantization")
+    s = None
+    if points is None:
+        s = 2 ** int(numBits)
+        if not 2 <= s <= 256:
+            raise ValueError("stored codes have at most 8 bits: numBits must be in [1, 8]")
+        pts_list = [None] * len(order)
+    else:
+        per_tensor = len(points) > 0 and (torch.is_tensor(points[0]) or isinstance(points[0], (list, tuple, np.ndarray)))
+        pts_list = list(points) if per_tensor else [points] * len(order)
+        if len(pts_list) != len(order):
+            raise ValueError(f"{len(pts_list)} point lists for {len(order)} quantized tensors")
+        if rule not in ("nearest", "midpoint"):
+            raise ValueError(f"unknown rule {rule!r}")
+    N.require_cuda()
+    dev = next((p.device for _, p in named if p.is_cuda), torch.device("cuda", torch.cuda.current_device()))
+    if buffers is not None:
+        buffers = [(name, b.detach().to(dev).clone()) for name, b in buffers]
+    return named, dict(zip(order, pts_list)), s, buffers, dev
+
+
+def _device_of(m, device=None):
+    N.require_cuda()
+    if device is not None:
+        return torch.device(device)
+    for t in m.tensors:
+        for x in (getattr(t, m._SECTIONS[0]), t.raw):
+            if x is not None and x.is_cuda:
+                return x.device
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def _mover(m, dev):
+    """tensor -> the same tensor on ``dev``.  Sections of a file loaded to the host are views into its data region,
+    which goes to ``dev`` in one copy (on first use); any other tensor moves by itself (no copy when it is there)."""
+    host = m._data if m._data is not None and not m._data.is_cuda else None
+    region = []
+
+    def move(x):
+        if x is None:
+            return None
+        if host is not None and not x.is_cuda and x.untyped_storage().data_ptr() == host.untyped_storage().data_ptr():
+            if not region:
+                region.append(host.to(dev))
+            off = x.data_ptr() - host.data_ptr()
+            return region[0][off:off + x.numel() * x.element_size()].view(x.dtype).view(x.shape)
+        return x.to(dev)
+    return move
+
+
+def _decode_args(m, items, dev, move):
+    """Arguments of the format's whole-model decode (qd_huffman_decode_dequant_model / qd_unpack_dequant_model) of every
+    (quantized tensor, out) of ``items`` on ``dev`` (the current device); out: contiguous float32 on ``dev``.  Also
+    returns the tensors the call reads, which must outlive its enqueueing."""
+    desc = np.zeros(len(items), m._DESCRIPTOR)
+    keep = []
+    if m.kind != "uniform":                      # every tensor's points in one upload
+        src = items[0][0].points.device
+        flat = move(torch.cat([t.points.reshape(-1).to(src, torch.float32) for t, _ in items]))
+        keep.append(flat)
+    at = 0
+    for i, (t, out) in enumerate(items):
+        sections = [move(getattr(t, name)) for name in m._SECTIONS]
+        keep += sections
+        points, k = 0, 0
+        if m.kind != "uniform":
+            k = t.points.numel()
+            points = flat[at:at + k].data_ptr()
+            at += k
+        desc[i] = m._descriptor(t, sections, points, k, out)
+    ws = torch.empty(int(getattr(N.lib(), m._WORKSPACE)(len(items))), dtype=torch.uint8, device=dev)
+    keep += [desc, ws]
+    args = (desc.ctypes.data, len(items), *m._decode_tables(dev), _bucket(m.bucket_size), int(m.levels) if m.kind == "uniform" else 0,
+            N.ptr(ws), ws.numel(), N.stream_ptr(dev))
+    return args, keep
+
+
+def _check_target(m, model):
+    """(named parameters, persistent buffers) of ``model`` once they are known to match ``m``; ValueError otherwise."""
+    named = list(model.named_parameters())
+    if len(named) != len(m.tensors):
+        raise ValueError(f"model has {len(named)} parameters, the {m._WHAT} {len(m.tensors)}")
+    for (name, p), t in zip(named, m.tensors):
+        if tuple(p.shape) != tuple(t.shape):
+            raise ValueError(f"{name}: shape {tuple(p.shape)} != stored {tuple(t.shape)} ({t.name})")
+    bufs = []
+    if m.buffers is not None:
+        bufs = _persistent_buffers(model)
+        if len(bufs) != len(m.buffers):
+            raise ValueError(f"model has {len(bufs)} persistent buffers, the {m._WHAT} {len(m.buffers)}")
+        for (name, b), (stored, s) in zip(bufs, m.buffers):
+            if tuple(b.shape) != tuple(s.shape) or b.dtype != s.dtype:
+                raise ValueError(f"buffer {name}: {b.dtype} {tuple(b.shape)} != stored {s.dtype} {tuple(s.shape)} ({stored})")
+    return named, bufs
+
+
+def _write_into(m, named, bufs, skip=()) -> None:
+    """The writing half of decompress_ / unpack_: every parameter but those whose indices are in ``skip``, then the
+    buffers.  Per device, the quantized tensors decode in one launch, straight into parameters that are contiguous
+    float32 on that device; the others go through a temporary."""
+    default = _device_of(m)
+    groups = {}                                  # device -> parameter indices (host parameters decode on `default`)
+    for k, (_, p) in enumerate(named):
+        if k not in skip:
+            groups.setdefault(p.device if p.is_cuda else default, []).append(k)
+    for _, b in bufs:
+        if b.is_cuda:
+            groups.setdefault(b.device, [])
+    with torch.no_grad():
+        for dev, ks in groups.items():
+            with torch.cuda.device(dev):
+                move = _mover(m, dev)
+                items, temps = [], []
+                for k in ks:
+                    t, d = m.tensors[k], named[k][1].data
+                    if not t.quantized:
+                        d.copy_((move(t.raw) if d.is_cuda else t.raw).view_as(d))
+                    elif d.device == dev and d.dtype == torch.float32 and d.is_contiguous():
+                        items.append((t, d))
+                    else:
+                        out = torch.empty(t.numel, dtype=torch.float32, device=dev)
+                        items.append((t, out))
+                        temps.append((d, out))
+                if items:
+                    args, keep = _decode_args(m, items, dev, move)
+                    N.check(getattr(N.lib(), m._DECODE)(*args))
+                for d, out in temps:
+                    d.copy_(out.view_as(d))
+                for (_, b), (_, s) in zip(bufs, m.buffers or []):
+                    if b.is_cuda and b.device == dev:
+                        b.copy_(move(s))
+        for (_, b), (_, s) in zip(bufs, m.buffers or []):
+            if not b.is_cuda:
+                b.copy_(s)
+
+
+def _read_container(cls, path, device):
+    """A CompressedModel or PackedModel (``cls``) read from ``path`` and validated on the host before anything reaches a
+    device: prefix, header, every tensor entry (unique names, exactly its format's sections, each in bounds, aligned and
+    of the size its shape needs), buffers, and no two sections overlapping.  Every section is a view into one tensor
+    holding the file's data region; a ``device`` gets that region in one copy."""
+    def bad(msg):
+        raise ValueError(f"not a valid {cls._FILE}: {msg}")
+
+    with open(path, "rb") as f:
+        buf = bytearray(f.read())
+    if len(buf) < _PREFIX.size:
+        bad("shorter than its prefix")
+    magic, version, reserved, hlen = _PREFIX.unpack_from(buf)
+    if magic != cls._MAGIC:
+        bad("bad magic")
+    if version not in cls._VERSIONS:
+        bad(f"format version {version}, this reader knows {' and '.join(str(v) for v in cls._VERSIONS)}")
+    if reserved != 0:
+        bad("reserved prefix field is not 0")
+    if _PREFIX.size + hlen > len(buf):
+        bad("header runs past the end of the file")
+    try:
+        h = json.loads(buf[_PREFIX.size:_PREFIX.size + hlen].decode("utf-8"))
+        kind, levels, bucket, entries, data_bytes = h["kind"], h["levels"], h["bucket"], h["tensors"], h["data_bytes"]
+    except (ValueError, KeyError, TypeError) as e:
+        bad(f"unreadable header ({e})")
+    if not isinstance(data_bytes, int) or not isinstance(entries, list):
+        bad("data_bytes must be an integer and tensors a list")
+    start = _align(_PREFIX.size + hlen)
+    if data_bytes < 0 or start + data_bytes != len(buf):
+        bad(f"{len(buf)} bytes, the header describes {start + data_bytes}")
+    if kind not in ("uniform", "nonuniform"):
+        bad(f"unknown kind {kind!r}")
+    if kind == "uniform" and not (isinstance(levels, int) and not isinstance(levels, bool) and 2 <= levels <= 256):
+        bad("uniform levels must be in [2, 256]")
+    if kind == "nonuniform" and levels is not None:
+        bad("a non-uniform model has no levels")
+    if bucket is not None and not (isinstance(bucket, int) and not isinstance(bucket, bool) and bucket > 0):
+        bad("bucket must be a positive integer or null")
+    extra = cls._read_header(h, version, levels, bad)
+    region = torch.from_numpy(np.frombuffer(buf, np.uint8, count=data_bytes, offset=start)) if data_bytes else \
+        torch.empty(0, dtype=torch.uint8)
+    spans = []
+
+    def view(off, nb, dtype, shape):
+        return region[off:off + nb].view(dtype).view(shape)
+
+    def section(e, name, dtype, nbytes):
+        try:
+            off, nb = (int(v) for v in e["sections"][name])
+        except (KeyError, TypeError, ValueError):
+            bad(f"{e.get('name')}: section {name} missing")
+        if nb != nbytes:
+            bad(f"{e.get('name')}: section {name} holds {nb} bytes, {nbytes} expected")
+        if off < 0 or off % _ALIGN or off + nb > data_bytes:
+            bad(f"{e.get('name')}: section {name} out of range")
+        spans.append((off, nb))
+        return view(off, nb, dtype, (nbytes // dtype.itemsize,))
+
+    tensors, names = [], set()
+    for e in entries:
+        try:
+            name, shape, quantized = str(e["name"]), tuple(int(d) for d in e["shape"]), e["quantized"]
+        except (KeyError, TypeError, ValueError):
+            bad("tensor entry without name / shape / quantized")
+        if not isinstance(quantized, bool) or e.get("dtype") != "float32" or any(d < 0 for d in shape):
+            bad(f"{name}: bad dtype, shape or quantized flag")
+        if name in names:
+            bad(f"tensor {name} appears twice")
+        names.add(name)
+        if not isinstance(e.get("sections"), dict) or set(e["sections"]) != (set(cls._SECTIONS) if quantized else {"raw"}):
+            bad(f"{name}: unexpected sections")
+        n = int(math.prod(shape))
+        if not quantized:
+            tensors.append(cls._ENTRY(name, shape, raw=section(e, "raw", torch.float32, 4 * n)))
+            continue
+        if n == 0:
+            bad(f"{name}: empty quantized tensor")
+        pts = None
+        if kind == "uniform" and "points" in e:
+            bad(f"{name}: a uniform tensor has no points")
+        if kind == "nonuniform":
+            try:
+                pts = torch.tensor([float(v) for v in e["points"]], dtype=torch.float32)
+            except (KeyError, TypeError, ValueError):
+                bad(f"{name}: non-uniform tensor without points")
+        fields = cls._read_entry(e, name, n, levels, pts, section, bad)
+        rows = _rows(n, bucket)
+        tensors.append(cls._ENTRY(name, shape, alpha=section(e, "alpha", torch.float32, 4 * rows),
+                                  beta=section(e, "beta", torch.float32, 4 * rows), points=pts, **fields))
+    buffers = _read_buffers(h["buffers"], view, data_bytes, bad, spans) if "buffers" in h else None
+    spans.sort()
+    for (o1, n1), (o2, _) in zip(spans, spans[1:]):
+        if o1 + n1 > o2:
+            bad(f"sections at {o1} and {o2} overlap")
+    m = cls(kind=kind, levels=levels, bucket_size=bucket, tensors=tensors, buffers=buffers, **extra)
+    m._data = region
+    if device is not None:                       # everything is validated before anything reaches the GPU
+        move = _mover(m, torch.device(device))
+        pts = [t.points for t in tensors if t.points is not None]
+        flat = torch.cat(pts).to(device) if pts else None          # every tensor's points in one upload too
+        at = 0
+        for t in tensors:
+            for f_ in cls._SECTIONS + ("raw",):
+                setattr(t, f_, move(getattr(t, f_)))
+            if t.points is not None:
+                t.points, at = flat[at:at + t.points.numel()], at + t.points.numel()
+        if buffers is not None:
+            m.buffers = [(name, move(b)) for name, b in buffers]
+        m._data = move(region)
+    return m
+
+
+def _read_buffers(entries, view, data_bytes, bad, spans):
+    """[(name, tensor view)] of a header's buffer entries, each checked against the data region; ``bad(msg)`` raises.
+    Every buffer's (offset, bytes) is appended to ``spans``."""
+    if not isinstance(entries, list):
+        bad("buffers is not a list")
+    buffers, names = [], set()
+    for e in entries:
+        try:
+            name, shape, dtype = str(e["name"]), tuple(int(d) for d in e["shape"]), e["dtype"]
+            off, nb = (int(v) for v in e["section"])
+        except (KeyError, TypeError, ValueError):
+            bad("buffer entry without name / shape / dtype / section")
+        if dtype not in _BUFFER_DTYPES:
+            bad(f"buffer {name}: unknown dtype {dtype!r}")
+        if any(d < 0 for d in shape):
+            bad(f"buffer {name}: bad shape")
+        if name in names:
+            bad(f"buffer {name} appears twice")
+        names.add(name)
+        tdtype = _BUFFER_DTYPES[dtype]
+        size = int(math.prod(shape)) * tdtype.itemsize
+        if nb != size:
+            bad(f"buffer {name}: {nb} bytes, its shape and dtype need {size}")
+        if off < 0 or off % _ALIGN or off + nb > data_bytes:
+            bad(f"buffer {name}: section out of range")
+        spans.append((off, nb))
+        buffers.append((name, view(off, nb, tdtype, shape)))
+    return buffers
 
 
 def compress_model(model, numBits=None, bucket_size=256, quantize_first_and_last_layer=True, *, points=None,
@@ -323,63 +802,22 @@ def compress_model(model, numBits=None, bucket_size=256, quantize_first_and_last
     get_huffman_encoding_mean_bit_length x the number of quantized weights.  ``include_buffers``: also store the
     persistent buffers (state_dict() order, float32 or int64, e.g. BatchNorm running statistics) as they are, so
     that decompress_ into a freshly built network gives back the whole eval-mode model."""
-    buffers = None
-    if include_buffers:
-        buffers = _persistent_buffers(model)
-        for _, b in buffers:
-            _dtype_name(b)
-    N.require_cuda()
-    if (numBits is None) == (points is None):
-        raise ValueError("give numBits (uniform) or points (non-uniform), not both")
-    named = list(model.named_parameters())
-    sel = _selected(named, quantize_first_and_last_layer)
-    order = [i for i in range(len(named)) if i in sel]
-    uniform = points is None
-    if uniform:
-        s = 2 ** int(numBits)
-        if not 2 <= s <= 256:
-            raise ValueError("the Huffman codec stores uint8 levels: numBits must be in [1, 8]")
-        bins = s
-    else:
-        per_tensor = len(points) > 0 and (torch.is_tensor(points[0]) or isinstance(points[0], (list, tuple, np.ndarray)))
-        pts_list = list(points) if per_tensor else [points] * len(order)
-        if len(pts_list) != len(order):
-            raise ValueError(f"{len(pts_list)} point lists for {len(order)} quantized tensors")
-        bins = 256
-    dev = next((p.device for _, p in named if p.is_cuda), torch.device("cuda", torch.cuda.current_device()))
-    b = 0 if bucket_size is None else int(bucket_size)
+    named, quantized, s, buffers, dev = _quantization_plan(model, numBits, quantize_first_and_last_layer, points, rule, include_buffers)
     sp = N.stream_ptr(dev)
-    counts = torch.zeros(len(order), 256, dtype=torch.int64, device=dev)
+    counts = torch.zeros(len(quantized), 256, dtype=torch.int64, device=dev)
     tensors, idxs = [], []
     with torch.cuda.device(dev):
         for i, (name, p) in enumerate(named):
-            if i not in sel:
-                tensors.append(HuffmanTensor(name, tuple(p.shape), raw=p.detach().to(dev, torch.float32).contiguous().view(-1).clone()))
+            if i not in quantized:
+                tensors.append(HuffmanTensor(name, tuple(p.shape), raw=_flat(p, dev).clone()))
                 continue
-            k = len(idxs)
-            x = p.detach().to(dev, torch.float32).contiguous().view(-1)
-            n = x.numel()
-            rows = _rows(n, bucket_size)
-            alpha = torch.empty(rows, device=dev)
-            beta = torch.empty(rows, device=dev)
-            idx = torch.empty(n, dtype=torch.uint8, device=dev)
-            ws = N.workspace(n, b, dev)
-            pts = None
-            if uniform:
-                N.check(N.lib().qd_uniform_fwd(N.ptr(x), None, N.ptr(idx), N.ptr(alpha), N.ptr(beta), None, None, n, b, s, None, 0.0,
-                                               0, 0, 0, N.ptr(ws), ws.numel(), sp))
-            else:
-                pts = torch.as_tensor(pts_list[k], dtype=torch.float32).detach().to(dev).contiguous().view(-1)
-                N.check(N.lib().qd_nonuniform_fwd(N.ptr(x), N.ptr(pts), pts.numel(), N.RULE_MIDPOINT if rule == "midpoint" else N.RULE_NEAREST,
-                                                  None, N.ptr(idx), None, N.ptr(alpha), N.ptr(beta), n, b, None, 0.0, N.ptr(ws), ws.numel(), sp))
-            N.check(N.lib().qd_index_histogram(N.ptr(idx), n, bins, N.ptr(counts[k]), sp))
+            pts = None if s is not None else _points(quantized[i], dev)
+            idx, alpha, beta = _levels(_flat(p, dev), s, pts, bucket_size, rule, sp)
+            N.check(N.lib().qd_index_histogram(N.ptr(idx), idx.numel(), 256 if s is None else s, N.ptr(counts[len(idxs)]), sp))
             idxs.append(idx)
             tensors.append(HuffmanTensor(name, tuple(p.shape), alpha=alpha, beta=beta, points=pts))
-        if not idxs:
-            raise ValueError("no parameter is selected for quantization")
         lengths = huffman_code_lengths(counts.sum(0).cpu().numpy())
-        cm = CompressedModel("uniform" if uniform else "nonuniform", s if uniform else None, bucket_size, lengths, tensors,
-                             buffers=None if buffers is None else [(name, b.detach().to(dev).clone()) for name, b in buffers])
+        cm = CompressedModel("uniform" if s is not None else "nonuniform", s, bucket_size, lengths, tensors, buffers=buffers)
         table = cm.table(dev)
         len_vec = torch.zeros(256, dtype=torch.int64)
         for sym, l in lengths.items():
@@ -406,17 +844,6 @@ def compress_model(model, numBits=None, bucket_size=256, quantize_first_and_last
     return cm
 
 
-def _device_of(cm: CompressedModel, device=None):
-    N.require_cuda()
-    if device is not None:
-        return torch.device(device)
-    for t in cm.tensors:
-        for x in (t.words, t.raw):
-            if x is not None and x.is_cuda:
-                return x.device
-    return torch.device("cuda", torch.cuda.current_device())
-
-
 def decompress_tensor(cm: CompressedModel, which, out: torch.Tensor = None, device=None) -> torch.Tensor:
     """Decodes one tensor (index or name) of a CompressedModel to float32 on the GPU: the fake-quantized tensor
     bit for bit, or the stored tensor when it was kept unquantized.  ``out``: contiguous float32 CUDA tensor of
@@ -433,7 +860,7 @@ def decompress_tensor(cm: CompressedModel, which, out: torch.Tensor = None, devi
             return out
         words, offs = t.words.to(dev), t.chunk_offsets.to(dev)
         alpha, beta = t.alpha.to(dev), t.beta.to(dev)
-        b = 0 if cm.bucket_size is None else int(cm.bucket_size)
+        b = _bucket(cm.bucket_size)
         sp = N.stream_ptr(dev)
         args = (N.ptr(words) if words.numel() else None, words.numel(), N.ptr(offs), N.ptr(cm.table(dev)))
         if cm.kind == "uniform":
@@ -445,372 +872,24 @@ def decompress_tensor(cm: CompressedModel, which, out: torch.Tensor = None, devi
     return out
 
 
-def _mover(cm: CompressedModel, dev):
-    """tensor -> the same tensor on ``dev``.  Sections of a file loaded to the host are views into its data region,
-    which goes to ``dev`` in one copy (on first use); any other tensor moves by itself (no copy when it is there)."""
-    host = cm._data if cm._data is not None and not cm._data.is_cuda else None
-    region = []
-
-    def move(x):
-        if x is None:
-            return None
-        if host is not None and not x.is_cuda and x.untyped_storage().data_ptr() == host.untyped_storage().data_ptr():
-            if not region:
-                region.append(host.to(dev))
-            off = x.data_ptr() - host.data_ptr()
-            return region[0][off:off + x.numel() * x.element_size()].view(x.dtype).view(x.shape)
-        return x.to(dev)
-    return move
-
-
-def _model_decode_args(cm: CompressedModel, items, dev, move):
-    """Arguments of one qd_huffman_decode_dequant_model call that decodes every (quantized tensor, out) of
-    ``items`` on ``dev`` (the current device); out: contiguous float32 on ``dev``.  Also returns the device tensors
-    the call reads, which must outlive its enqueueing."""
-    desc = np.zeros(len(items), _MODEL_TENSOR)
-    keep = []
-    if cm.kind != "uniform":                     # every tensor's points in one upload
-        src = items[0][0].points.device
-        flat = move(torch.cat([t.points.reshape(-1).to(src, torch.float32) for t, _ in items]))
-        keep.append(flat)
-    at = 0
-    for i, (t, out) in enumerate(items):
-        words, offs, alpha, beta = (move(x) for x in (t.words, t.chunk_offsets, t.alpha, t.beta))
-        keep += [words, offs, alpha, beta]
-        points, k = 0, 0
-        if cm.kind != "uniform":
-            k = t.points.numel()
-            points = flat[at:at + k].data_ptr()
-            at += k
-        desc[i] = (N.ptr(words) if words.numel() else 0, N.ptr(offs), N.ptr(alpha), N.ptr(beta), points, N.ptr(out), words.numel(),
-                   t.numel, k, 0)
-    ws = torch.empty(int(N.lib().qd_huffman_model_workspace_bytes(len(items))), dtype=torch.uint8, device=dev)
-    keep += [desc, ws]
-    table = cm.table(dev)
-    args = (desc.ctypes.data, len(items), N.ptr(table), 0 if cm.bucket_size is None else int(cm.bucket_size),
-            int(cm.levels) if cm.kind == "uniform" else 0, N.ptr(ws), ws.numel(), N.stream_ptr(dev))
-    return args, keep
-
-
 def decompress_(cm: CompressedModel, model) -> None:
     """Writes every parameter of ``model`` in place from ``cm`` (existing parameter handles stay valid), and its
     persistent buffers when ``cm`` stores them.  Everything is checked before anything is written.  Per device, the
     quantized tensors decode in one launch, straight into parameters that are contiguous float32 on that device."""
-    named = list(model.named_parameters())
-    if len(named) != len(cm.tensors):
-        raise ValueError(f"model has {len(named)} parameters, the compressed model {len(cm.tensors)}")
-    for (name, p), t in zip(named, cm.tensors):
-        if tuple(p.shape) != tuple(t.shape):
-            raise ValueError(f"{name}: shape {tuple(p.shape)} != stored {tuple(t.shape)} ({t.name})")
-    bufs = []
-    if cm.buffers is not None:
-        bufs = _persistent_buffers(model)
-        if len(bufs) != len(cm.buffers):
-            raise ValueError(f"model has {len(bufs)} persistent buffers, the compressed model {len(cm.buffers)}")
-        for (name, b), (stored, s) in zip(bufs, cm.buffers):
-            if tuple(b.shape) != tuple(s.shape) or b.dtype != s.dtype:
-                raise ValueError(f"buffer {name}: {b.dtype} {tuple(b.shape)} != stored {s.dtype} {tuple(s.shape)} ({stored})")
-    default = _device_of(cm)
-    groups = {}                                  # device -> parameter indices (host parameters decode on `default`)
-    for k, (_, p) in enumerate(named):
-        groups.setdefault(p.device if p.is_cuda else default, []).append(k)
-    for _, b in bufs:
-        if b.is_cuda:
-            groups.setdefault(b.device, [])
-    with torch.no_grad():
-        for dev, ks in groups.items():
-            with torch.cuda.device(dev):
-                move = _mover(cm, dev)
-                items, temps = [], []
-                for k in ks:
-                    t, d = cm.tensors[k], named[k][1].data
-                    if not t.quantized:
-                        d.copy_((move(t.raw) if d.is_cuda else t.raw).view_as(d))
-                    elif d.device == dev and d.dtype == torch.float32 and d.is_contiguous():
-                        items.append((t, d))
-                    else:
-                        out = torch.empty(t.numel, dtype=torch.float32, device=dev)
-                        items.append((t, out))
-                        temps.append((d, out))
-                if items:
-                    args, keep = _model_decode_args(cm, items, dev, move)
-                    N.check(N.lib().qd_huffman_decode_dequant_model(*args))
-                for d, out in temps:
-                    d.copy_(out.view_as(d))
-                for (_, b), (_, s) in zip(bufs, cm.buffers or []):
-                    if b.is_cuda and b.device == dev:
-                        b.copy_(move(s))
-        for (_, b), (_, s) in zip(bufs, cm.buffers or []):
-            if not b.is_cuda:
-                b.copy_(s)
+    _write_into(cm, *_check_target(cm, model))
 
 
 def save_compressed(cm: CompressedModel, path) -> int:
-    """Writes the container: magic, version, JSON header, 16-byte-aligned little-endian sections.  Returns the
-    file size in bytes."""
-    header, sections, data_bytes = _layout(cm)
-    return _write_container(path, FILE_MAGIC, FILE_VERSION if cm.buffers is None else FILE_VERSION_BUFFERS, header, sections,
-                            data_bytes)
-
-
-def _write_container(path, magic, version, header, sections, data_bytes) -> int:
-    """prefix (magic, version, 0, header length), the JSON header, then every (tensor, nbytes, offset) section
-    little-endian at its offset from the first 16-byte boundary after the header.  Returns the file size."""
-    start = _align(_PREFIX.size + len(header))
-    buf = bytearray(start + data_bytes)
-    buf[:_PREFIX.size] = _PREFIX.pack(magic, version, 0, len(header))
-    buf[_PREFIX.size:_PREFIX.size + len(header)] = header
-    little = {torch.int32: "<i4", torch.float32: "<f4", torch.int64: "<i8", torch.uint8: "u1"}
-    for tensor, nb, off in sections:
-        buf[start + off:start + off + nb] = tensor.detach().contiguous().cpu().numpy().astype(little[tensor.dtype], copy=False).tobytes()
-    with open(path, "wb") as f:
-        f.write(buf)
-    return len(buf)
-
-
-def _bad(msg):
-    raise ValueError(f"not a valid Huffman-coded model file: {msg}")
+    """Writes the Huffman-coded container: magic QDHUFF, version 1 (2 when buffers are stored), JSON header,
+    16-byte-aligned little-endian sections.  Returns the file size in bytes."""
+    return _write_container(cm, path)
 
 
 def load_compressed(path, device=None) -> CompressedModel:
     """Reads and validates a file written by save_compressed (version 1, or 2 with buffers).  Every section is a
     view into one tensor holding the file's data region.  device=None keeps it in host memory (reading and
     validating needs no GPU; decompress_ moves it to the GPU in one copy); a device gets it in one copy here."""
-    with open(path, "rb") as f:
-        buf = bytearray(f.read())
-    if len(buf) < _PREFIX.size:
-        _bad("shorter than its prefix")
-    magic, version, _, hlen = _PREFIX.unpack_from(buf)
-    if magic != FILE_MAGIC:
-        _bad("bad magic")
-    if version not in (FILE_VERSION, FILE_VERSION_BUFFERS):
-        _bad(f"format version {version}, this reader knows {FILE_VERSION} and {FILE_VERSION_BUFFERS}")
-    if _PREFIX.size + hlen > len(buf):
-        _bad("header runs past the end of the file")
-    try:
-        h = json.loads(buf[_PREFIX.size:_PREFIX.size + hlen].decode("utf-8"))
-        kind, levels, bucket, chunk = h["kind"], h["levels"], h["bucket"], h["chunk"]
-        code = {int(s): int(l) for s, l in h["code"]}
-        entries, data_bytes = h["tensors"], int(h["data_bytes"])
-    except (ValueError, KeyError, TypeError) as e:
-        _bad(f"unreadable header ({e})")
-    start = _align(_PREFIX.size + hlen)
-    if data_bytes < 0 or start + data_bytes != len(buf):
-        _bad(f"{len(buf)} bytes, the header describes {start + data_bytes}")
-    if ("buffers" in h) != (version == FILE_VERSION_BUFFERS):
-        _bad(f"a version-{version} file {'must not list' if version == FILE_VERSION else 'must list its'} buffers")
-    region = torch.from_numpy(np.frombuffer(buf, np.uint8, count=data_bytes, offset=start)) if data_bytes else \
-        torch.empty(0, dtype=torch.uint8)
-    if chunk != HUFFMAN_CHUNK:
-        _bad(f"chunk of {chunk} symbols, this reader decodes {HUFFMAN_CHUNK}")
-    if kind not in ("uniform", "nonuniform"):
-        _bad(f"unknown kind {kind!r}")
-    if kind == "uniform" and not (isinstance(levels, int) and 2 <= levels <= 256):
-        _bad("uniform levels must be in [2, 256]")
-    if bucket is not None and not (isinstance(bucket, int) and bucket > 0):
-        _bad("bucket must be a positive integer or null")
-    if len(code) != len(h["code"]):
-        _bad("a symbol appears twice in the code")
-    try:
-        check_code_lengths(code)
-    except ValueError as e:
-        _bad(str(e))
-    if kind == "uniform" and max(code) >= levels:
-        _bad("a code symbol is not a level")
-
-    def view(off, nb, dtype, shape):
-        return region[off:off + nb].view(dtype).view(shape)
-
-    def section(e, name, dtype, count):
-        try:
-            off, nb = (int(v) for v in e["sections"][name])
-        except (KeyError, TypeError, ValueError):
-            _bad(f"{e.get('name')}: section {name} missing")
-        if off < 0 or off % _ALIGN or nb != count * 4 or off + nb > data_bytes:
-            _bad(f"{e.get('name')}: section {name} out of range")
-        return view(off, nb, dtype, (count,))
-
-    tensors = []
-    for e in entries:
-        try:
-            name, shape, quantized = str(e["name"]), tuple(int(d) for d in e["shape"]), bool(e["quantized"])
-        except (KeyError, TypeError, ValueError):
-            _bad("tensor entry without name / shape / quantized")
-        if e.get("dtype") != "float32" or any(d < 0 for d in shape):
-            _bad(f"{name}: bad dtype or shape")
-        n = int(math.prod(shape))
-        if not quantized:
-            tensors.append(HuffmanTensor(name, shape, raw=section(e, "raw", torch.float32, n)))
-            continue
-        if n == 0:
-            _bad(f"{name}: empty quantized tensor")
-        chunks = -(-n // HUFFMAN_CHUNK)
-        rows = _rows(n, bucket)
-        words_nb = e.get("sections", {}).get("words", [0, -1])[1]
-        if not isinstance(words_nb, int) or words_nb < 0 or words_nb % 4:
-            _bad(f"{name}: section words out of range")
-        words = section(e, "words", torch.int32, words_nb // 4)
-        offs = section(e, "chunk_offsets", torch.int32, chunks)
-        o = offs.numpy().view(np.uint32).astype(np.int64)
-        if o[0] != 0 or np.any(np.diff(o) < 0) or o[-1] > words.numel():
-            _bad(f"{name}: chunk offsets out of range")
-        pts = None
-        if kind == "nonuniform":
-            try:
-                pts = torch.tensor([float(v) for v in e["points"]], dtype=torch.float32)
-            except (KeyError, TypeError, ValueError):
-                _bad(f"{name}: non-uniform tensor without points")
-            # the code is model-wide: a tensor with fewer points than another never emits the higher symbols
-            if not 1 <= pts.numel() <= 256:
-                _bad(f"{name}: {pts.numel()} points, expected 1 to 256")
-        tensors.append(HuffmanTensor(name, shape, words=words, chunk_offsets=offs,
-                                     alpha=section(e, "alpha", torch.float32, rows), beta=section(e, "beta", torch.float32, rows),
-                                     points=pts, code_bits=int(e.get("code_bits", 0))))
-    buffers = None
-    if version == FILE_VERSION_BUFFERS:
-        buffers = _read_buffers(h["buffers"], view, data_bytes, _bad)
-    cm = CompressedModel(kind, levels, bucket, code, tensors, buffers=buffers)
-    cm._data = region
-    if device is not None:                       # everything is validated before anything reaches the GPU
-        move = _mover(cm, torch.device(device))
-        pts = [t.points for t in tensors if t.points is not None]
-        flat = torch.cat(pts).to(device) if pts else None          # every tensor's points in one upload too
-        at = 0
-        for t in tensors:
-            for f_ in ("words", "chunk_offsets", "alpha", "beta", "raw"):
-                setattr(t, f_, move(getattr(t, f_)))
-            if t.points is not None:
-                t.points, at = flat[at:at + t.points.numel()], at + t.points.numel()
-        if buffers is not None:
-            cm.buffers = [(name, move(b)) for name, b in buffers]
-        cm._data = move(region)
-    return cm
-
-
-def _read_buffers(entries, view, data_bytes, bad, spans=None):
-    """[(name, tensor view)] of a header's buffer entries, each checked against the data region; ``bad(msg)`` raises.
-    ``spans``: a list that receives every buffer's (offset, bytes)."""
-    if not isinstance(entries, list):
-        bad("buffers is not a list")
-    buffers, names = [], set()
-    for e in entries:
-        try:
-            name, shape, dtype = str(e["name"]), tuple(int(d) for d in e["shape"]), e["dtype"]
-            off, nb = (int(v) for v in e["section"])
-        except (KeyError, TypeError, ValueError):
-            bad("buffer entry without name / shape / dtype / section")
-        if dtype not in _BUFFER_DTYPES:
-            bad(f"buffer {name}: unknown dtype {dtype!r}")
-        if any(d < 0 for d in shape):
-            bad(f"buffer {name}: bad shape")
-        if name in names:
-            bad(f"buffer {name} appears twice")
-        names.add(name)
-        tdtype = _BUFFER_DTYPES[dtype]
-        size = int(math.prod(shape)) * tdtype.itemsize
-        if nb != size:
-            bad(f"buffer {name}: {nb} bytes, its shape and dtype need {size}")
-        if off < 0 or off % _ALIGN or off + nb > data_bytes:
-            bad(f"buffer {name}: section out of range")
-        if spans is not None:
-            spans.append((off, nb))
-        buffers.append((name, view(off, nb, tdtype, shape)))
-    return buffers
-
-
-# ---------------------------------------------------------------------------------------------------------------
-# Fixed-width model container.  Every quantized tensor is stored as its packed codes (qd_pack_indices layout, its own
-# width bits_for(levels or points)) + (alpha, beta) per bucket: the size get_size_reduction accounts for.  It decodes
-# at HBM rate in one launch (qd_unpack_dequant_model) and can be read at any bucket without a chunk index.
-PACKED_MAGIC = b"QDPACK\x00\x00"
-PACKED_VERSION = 1
-# qd_packed_tensor (include/qd_b200.h): one entry of the whole-model unpack
-_PACKED_TENSOR = np.dtype([("packed", "<u8"), ("alpha", "<u8"), ("beta", "<u8"), ("points", "<u8"), ("q", "<u8"), ("n", "<i8"),
-                           ("bits", "<i4"), ("num_points", "<i4")])
-assert _PACKED_TENSOR.itemsize == 56
-
-
-@dataclass
-class PackedEntry:
-    """One parameter of a PackedModel: packed codes + (alpha, beta) per bucket, or float32 as is."""
-    name: str
-    shape: tuple
-    bits: int = 0                       # code width of a quantized tensor: 1, 2, 4 or 8
-    packed: torch.Tensor = None         # uint8[ceil(n * bits / 8)]
-    alpha: torch.Tensor = None          # float32[rows]
-    beta: torch.Tensor = None
-    points: torch.Tensor = None         # non-uniform: this tensor's centroids
-    raw: torch.Tensor = None            # unquantized tensor (float32)
-
-    @property
-    def numel(self) -> int:
-        return int(math.prod(self.shape))
-
-    @property
-    def quantized(self) -> bool:
-        return self.raw is None
-
-
-@dataclass
-class PackedModel:
-    """A model whose quantized parameters are stored fixed-width (pack_model, load_packed)."""
-    kind: str                       # "uniform" | "nonuniform"
-    levels: object                  # uniform: s; non-uniform: None
-    bucket_size: object
-    tensors: list
-    # persistent buffers as [(name, tensor)] in state_dict() order; None: not stored
-    buffers: list = None
-    # a loaded file's data region: every section is a view into it, so it reaches a device in one copy
-    _data: torch.Tensor = field(default=None, init=False, repr=False, compare=False)
-
-    def size_breakdown(self) -> dict:
-        """Bytes of the saved file by what they hold.  code_bytes + scale_bytes is what get_size_reduction accounts
-        for, up to the round-up of each tensor's codes to whole bytes; the rest is the format and the stored buffers."""
-        header, sections, data_bytes = _packed_layout(self)
-        q = [t for t in self.tensors if t.quantized]
-        section_bytes = sum(nb for _, nb, _ in sections)
-        return {
-            "code_bytes": sum(t.packed.numel() for t in q),
-            "scale_bytes": sum((t.alpha.numel() + t.beta.numel()) * 4 for t in q),
-            "unquantized_bytes": sum(t.raw.numel() * 4 for t in self.tensors if not t.quantized),
-            "buffer_bytes": sum(b.numel() * b.element_size() for _, b in self.buffers or []),
-            "header_bytes": _PREFIX.size + len(header),
-            "alignment_bytes": _align(_PREFIX.size + len(header)) - _PREFIX.size - len(header) + data_bytes - section_bytes,
-            "file_bytes": _align(_PREFIX.size + len(header)) + data_bytes,
-        }
-
-
-def _packed_sections(t: PackedEntry):
-    return [("raw", t.raw)] if not t.quantized else [("packed", t.packed), ("alpha", t.alpha), ("beta", t.beta)]
-
-
-def _packed_layout(pm: PackedModel):
-    """(JSON header bytes, [(tensor, nbytes, offset)], data bytes); offsets are relative to the first 16-byte
-    boundary after the header, every section starts on a 16-byte boundary.  The header lists buffers only when the
-    model stores them."""
-    sections, entries, off = [], [], 0
-    for t in pm.tensors:
-        e = {"name": t.name, "shape": list(t.shape), "dtype": "float32", "quantized": t.quantized, "sections": {}}
-        if t.quantized:
-            e["bits"] = int(t.bits)
-            if t.points is not None:
-                e["points"] = [float(v) for v in t.points.detach().cpu().numpy().astype(np.float32)]
-        for name, tensor in _packed_sections(t):
-            nb = tensor.numel() * tensor.element_size()
-            e["sections"][name] = [off, nb]
-            sections.append((tensor, nb, off))
-            off = _align(off + nb)
-        entries.append(e)
-    buffers = []
-    for name, b in pm.buffers or []:
-        nb = b.numel() * b.element_size()
-        buffers.append({"name": name, "shape": list(b.shape), "dtype": _dtype_name(b), "section": [off, nb]})
-        sections.append((b, nb, off))
-        off = _align(off + nb)
-    header = {"kind": pm.kind, "levels": pm.levels, "bucket": pm.bucket_size, "tensors": entries, "data_bytes": off}
-    if pm.buffers is not None:
-        header["buffers"] = buffers
-    return json.dumps(header, separators=(",", ":")).encode("utf-8"), sections, off
+    return _read_container(CompressedModel, path, device)
 
 
 def pack_model(model, numBits=None, bucket_size=256, quantize_first_and_last_layer=True, *, points=None, rule="nearest",
@@ -820,55 +899,29 @@ def pack_model(model, numBits=None, bucket_size=256, quantize_first_and_last_lay
     bits_for(s) bits.  Non-uniform: ``points`` -- one ascending list for every tensor, or one list per quantized tensor
     (the differentiable-quantization output) -- with nonUniformQuantization's ``rule``; tensor t gets codes of
     bits_for(K_t) bits.  ``include_buffers`` also stores the persistent buffers (float32 / int64) as they are."""
-    buffers = None
-    if include_buffers:
-        buffers = _persistent_buffers(model)
-        for _, b in buffers:
-            _dtype_name(b)
-    N.require_cuda()
-    if (numBits is None) == (points is None):
-        raise ValueError("give numBits (uniform) or points (non-uniform), not both")
-    named = list(model.named_parameters())
-    sel = _selected(named, quantize_first_and_last_layer)
-    order = [i for i in range(len(named)) if i in sel]
-    if not order:
-        raise ValueError("no parameter is selected for quantization")
-    uniform = points is None
-    if uniform:
-        s = 2 ** int(numBits)
-        if not 2 <= s <= 256:
-            raise ValueError("the packed codec stores at most 8 bits per weight: numBits must be in [1, 8]")
-    else:
-        per_tensor = len(points) > 0 and (torch.is_tensor(points[0]) or isinstance(points[0], (list, tuple, np.ndarray)))
-        pts_list = list(points) if per_tensor else [points] * len(order)
-        if len(pts_list) != len(order):
-            raise ValueError(f"{len(pts_list)} point lists for {len(order)} quantized tensors")
-        if rule not in ("nearest", "midpoint"):
-            raise ValueError(f"unknown rule {rule!r}")
-    dev = next((p.device for _, p in named if p.is_cuda), torch.device("cuda", torch.cuda.current_device()))
-    b = 0 if bucket_size is None else int(bucket_size)
+    named, quantized, s, buffers, dev = _quantization_plan(model, numBits, quantize_first_and_last_layer, points, rule, include_buffers)
+    b = _bucket(bucket_size)
     tensors = []
     with torch.cuda.device(dev):
         sp = N.stream_ptr(dev)
-        ws_bytes = max(int(N.lib().qd_packed_workspace_bytes(named[i][1].numel(), b)) for i in order)
+        ws_bytes = max(int(N.lib().qd_packed_workspace_bytes(named[i][1].numel(), b)) for i in quantized)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)     # stream-ordered: free to reuse once the launches ran
-        k = 0
         for i, (name, p) in enumerate(named):
-            if i not in sel:
-                tensors.append(PackedEntry(name, tuple(p.shape), raw=p.detach().to(dev, torch.float32).contiguous().view(-1).clone()))
+            if i not in quantized:
+                tensors.append(PackedEntry(name, tuple(p.shape), raw=_flat(p, dev).clone()))
                 continue
-            x = p.detach().to(dev, torch.float32).contiguous().view(-1)
+            x = _flat(p, dev)
             n = x.numel()
             rows = _rows(n, bucket_size)
             alpha = torch.empty(rows, device=dev)
             beta = torch.empty(rows, device=dev)
-            if uniform:
+            if s is not None:
                 bits, pts = bits_for(s), None
                 packed = torch.empty((n * bits + 7) // 8, dtype=torch.uint8, device=dev)
                 N.check(N.lib().qd_uniform_fwd_packed(N.ptr(x), N.ptr(packed), bits, N.ptr(alpha), N.ptr(beta), n, b, s, N.ptr(ws),
                                                       ws.numel(), sp))
             else:
-                pts = torch.as_tensor(pts_list[k], dtype=torch.float32).detach().to(dev).contiguous().view(-1)
+                pts = _points(quantized[i], dev)
                 if not 1 <= pts.numel() <= 256:
                     raise ValueError(f"{name}: {pts.numel()} points, the packed codec stores 1 to 256")
                 bits = bits_for(pts.numel())
@@ -877,112 +930,14 @@ def pack_model(model, numBits=None, bucket_size=256, quantize_first_and_last_lay
                                                          N.RULE_MIDPOINT if rule == "midpoint" else N.RULE_NEAREST, N.ptr(packed), bits,
                                                          N.ptr(alpha), N.ptr(beta), n, b, N.ptr(ws), ws.numel(), sp))
             tensors.append(PackedEntry(name, tuple(p.shape), bits=bits, packed=packed, alpha=alpha, beta=beta, points=pts))
-            k += 1
-    return PackedModel("uniform" if uniform else "nonuniform", s if uniform else None, bucket_size, tensors,
-                       buffers=None if buffers is None else [(name, b_.detach().to(dev).clone()) for name, b_ in buffers])
-
-
-def _packed_decode_args(pm: PackedModel, items, dev, move):
-    """Arguments of one qd_unpack_dequant_model call that decodes every (quantized entry, out) of ``items`` on
-    ``dev`` (the current device); out: contiguous float32 on ``dev``.  Also returns the tensors the call reads, which
-    must outlive its enqueueing."""
-    desc = np.zeros(len(items), _PACKED_TENSOR)
-    keep = []
-    if pm.kind != "uniform":                     # every tensor's points in one upload
-        src = items[0][0].points.device
-        flat = move(torch.cat([t.points.reshape(-1).to(src, torch.float32) for t, _ in items]))
-        keep.append(flat)
-    at = 0
-    for i, (t, out) in enumerate(items):
-        packed, alpha, beta = (move(x) for x in (t.packed, t.alpha, t.beta))
-        keep += [packed, alpha, beta]
-        points, k = 0, 0
-        if pm.kind != "uniform":
-            k = t.points.numel()
-            points = flat[at:at + k].data_ptr()
-            at += k
-        desc[i] = (N.ptr(packed), N.ptr(alpha), N.ptr(beta), points, N.ptr(out), t.numel, t.bits, k)
-    ws = torch.empty(int(N.lib().qd_unpack_model_workspace_bytes(len(items))), dtype=torch.uint8, device=dev)
-    keep += [desc, ws]
-    args = (desc.ctypes.data, len(items), 0 if pm.bucket_size is None else int(pm.bucket_size),
-            int(pm.levels) if pm.kind == "uniform" else 0, N.ptr(ws), ws.numel(), N.stream_ptr(dev))
-    return args, keep
-
-
-def _packed_device_of(pm: PackedModel, device=None):
-    N.require_cuda()
-    if device is not None:
-        return torch.device(device)
-    for t in pm.tensors:
-        for x in (t.packed, t.raw):
-            if x is not None and x.is_cuda:
-                return x.device
-    return torch.device("cuda", torch.cuda.current_device())
+    return PackedModel("uniform" if s is not None else "nonuniform", s, bucket_size, tensors, buffers=buffers)
 
 
 def unpack_(pm: PackedModel, model) -> None:
     """Writes every parameter of ``model`` in place from ``pm`` (existing parameter handles stay valid), and its
     persistent buffers when ``pm`` stores them.  Everything is checked before anything is written.  Per device, the
     quantized tensors decode in one launch, straight into parameters that are contiguous float32 on that device."""
-    named, bufs = _check_unpack(pm, model)
-    _unpack_into(pm, named, bufs, skip=())
-
-
-def _check_unpack(pm: PackedModel, model):
-    """(named parameters, persistent buffers) of ``model`` once they are known to match ``pm``; ValueError otherwise."""
-    named = list(model.named_parameters())
-    if len(named) != len(pm.tensors):
-        raise ValueError(f"model has {len(named)} parameters, the packed model {len(pm.tensors)}")
-    for (name, p), t in zip(named, pm.tensors):
-        if tuple(p.shape) != tuple(t.shape):
-            raise ValueError(f"{name}: shape {tuple(p.shape)} != stored {tuple(t.shape)} ({t.name})")
-    bufs = []
-    if pm.buffers is not None:
-        bufs = _persistent_buffers(model)
-        if len(bufs) != len(pm.buffers):
-            raise ValueError(f"model has {len(bufs)} persistent buffers, the packed model {len(pm.buffers)}")
-        for (name, b), (stored, s) in zip(bufs, pm.buffers):
-            if tuple(b.shape) != tuple(s.shape) or b.dtype != s.dtype:
-                raise ValueError(f"buffer {name}: {b.dtype} {tuple(b.shape)} != stored {s.dtype} {tuple(s.shape)} ({stored})")
-    return named, bufs
-
-
-def _unpack_into(pm: PackedModel, named, bufs, skip) -> None:
-    """The writing half of unpack_: every parameter but those whose indices are in ``skip``, then the buffers."""
-    default = _packed_device_of(pm)
-    groups = {}                                  # device -> parameter indices (host parameters decode on `default`)
-    for k, (_, p) in enumerate(named):
-        if k not in skip:
-            groups.setdefault(p.device if p.is_cuda else default, []).append(k)
-    for _, b in bufs:
-        if b.is_cuda:
-            groups.setdefault(b.device, [])
-    with torch.no_grad():
-        for dev, ks in groups.items():
-            with torch.cuda.device(dev):
-                move = _mover(pm, dev)
-                items, temps = [], []
-                for k in ks:
-                    t, d = pm.tensors[k], named[k][1].data
-                    if not t.quantized:
-                        d.copy_((move(t.raw) if d.is_cuda else t.raw).view_as(d))
-                    elif d.device == dev and d.dtype == torch.float32 and d.is_contiguous():
-                        items.append((t, d))
-                    else:
-                        out = torch.empty(t.numel, dtype=torch.float32, device=dev)
-                        items.append((t, out))
-                        temps.append((d, out))
-                if items:
-                    args, keep = _packed_decode_args(pm, items, dev, move)
-                    N.check(N.lib().qd_unpack_dequant_model(*args))
-                for d, out in temps:
-                    d.copy_(out.view_as(d))
-                for (_, b), (_, s) in zip(bufs, pm.buffers or []):
-                    if b.is_cuda and b.device == dev:
-                        b.copy_(move(s))
-        for (_, b), (_, s) in zip(bufs, pm.buffers or []):
-            if not b.is_cuda:
-                b.copy_(s)
+    _write_into(pm, *_check_target(pm, model))
 
 
 class PackedLinear(torch.nn.Module):
@@ -1031,15 +986,7 @@ class PackedLinear(torch.nn.Module):
     def decoded_weight(self) -> torch.Tensor:
         """The decoded float32 weight [out_features, in_features], bit for bit what unpack_ writes."""
         w = torch.empty(self.out_features, self.in_features, dtype=torch.float32, device=self.packed.device)
-        n, b = w.numel(), 0 if self.bucket_size is None else int(self.bucket_size)
-        sp = N.stream_ptr(w.device)
-        if self.kind == "uniform":
-            N.check(N.lib().qd_unpack_dequant_uniform(N.ptr(self.packed), self.bits, N.ptr(self.alpha), N.ptr(self.beta), N.ptr(w), n, b,
-                                                      self.levels, sp))
-        else:
-            N.check(N.lib().qd_unpack_dequant_nonuniform(N.ptr(self.packed), self.bits, N.ptr(self.points), self.points.numel(),
-                                                         N.ptr(self.alpha), N.ptr(self.beta), N.ptr(w), n, b, sp))
-        return w
+        return _unpack(self.packed, self.bits, self.alpha, self.beta, self.points, self.levels, self.bucket_size, w)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if not torch.is_tensor(x) or not x.is_cuda or x.dtype != torch.float32:
@@ -1079,7 +1026,7 @@ def attach_packed_linear_(pm: PackedModel, model) -> list:
     generator sharing the embedding's matrix) or the Linear itself registered under two parents -- stays an nn.Linear
     and its weight is decoded as unpack_ decodes it: replacing it in one place would leave the other holder with a
     weight that was never written.  Returns the names of the replaced modules."""
-    named, bufs = _check_unpack(pm, model)
+    named, bufs = _check_target(pm, model)
     index = {id(p): k for k, (_, p) in enumerate(named)}
     holders = {}                                 # parameter -> registrations in the module tree, every path counted
     for _, mod in model.named_modules(remove_duplicate=False):
@@ -1094,7 +1041,7 @@ def attach_packed_linear_(pm: PackedModel, model) -> list:
                 raise ValueError(f"{mname}: a PackedLinear runs on a CUDA device, the Linear is on {mod.weight.device}")
             parent_name, _, attr = mname.rpartition(".")
             targets.append((mname, model.get_submodule(parent_name) if parent_name else model, attr, mod, index[id(mod.weight)]))
-    _unpack_into(pm, named, bufs, skip={k for *_, k in targets})
+    _write_into(pm, named, bufs, skip={k for *_, k in targets})
     movers = {}
     for mname, parent, attr, lin, k in targets:
         dev = lin.weight.device
@@ -1111,133 +1058,14 @@ def attach_packed_linear_(pm: PackedModel, model) -> list:
 def save_packed(pm: PackedModel, path) -> int:
     """Writes the fixed-width container: magic QDPACK, version 1, JSON header, 16-byte-aligned little-endian sections
     (packed codes as bytes).  Returns the file size in bytes."""
-    header, sections, data_bytes = _packed_layout(pm)
-    return _write_container(path, PACKED_MAGIC, PACKED_VERSION, header, sections, data_bytes)
-
-
-def _bad_packed(msg):
-    raise ValueError(f"not a valid fixed-width model file: {msg}")
+    return _write_container(pm, path)
 
 
 def load_packed(path, device=None) -> PackedModel:
     """Reads and validates a file written by save_packed; everything is checked on the host before anything reaches a
     device.  Every section is a view into one tensor holding the file's data region.  device=None keeps it in host
     memory (unpack_ moves it to the GPU in one copy); a device gets it in one copy here."""
-    bad = _bad_packed
-    with open(path, "rb") as f:
-        buf = bytearray(f.read())
-    if len(buf) < _PREFIX.size:
-        bad("shorter than its prefix")
-    magic, version, reserved, hlen = _PREFIX.unpack_from(buf)
-    if magic != PACKED_MAGIC:
-        bad("bad magic")
-    if version != PACKED_VERSION:
-        bad(f"format version {version}, this reader knows {PACKED_VERSION}")
-    if reserved != 0:
-        bad("reserved prefix field is not 0")
-    if _PREFIX.size + hlen > len(buf):
-        bad("header runs past the end of the file")
-    try:
-        h = json.loads(buf[_PREFIX.size:_PREFIX.size + hlen].decode("utf-8"))
-        kind, levels, bucket, entries, data_bytes = h["kind"], h["levels"], h["bucket"], h["tensors"], h["data_bytes"]
-    except (ValueError, KeyError, TypeError) as e:
-        bad(f"unreadable header ({e})")
-    if not isinstance(data_bytes, int) or not isinstance(entries, list):
-        bad("data_bytes must be an integer and tensors a list")
-    start = _align(_PREFIX.size + hlen)
-    if data_bytes < 0 or start + data_bytes != len(buf):
-        bad(f"{len(buf)} bytes, the header describes {start + data_bytes}")
-    if kind not in ("uniform", "nonuniform"):
-        bad(f"unknown kind {kind!r}")
-    if kind == "uniform" and not (isinstance(levels, int) and not isinstance(levels, bool) and 2 <= levels <= 256):
-        bad("uniform levels must be in [2, 256]")
-    if kind == "nonuniform" and levels is not None:
-        bad("a non-uniform model has no levels")
-    if bucket is not None and not (isinstance(bucket, int) and not isinstance(bucket, bool) and bucket > 0):
-        bad("bucket must be a positive integer or null")
-    region = torch.from_numpy(np.frombuffer(buf, np.uint8, count=data_bytes, offset=start)) if data_bytes else \
-        torch.empty(0, dtype=torch.uint8)
-    spans = []
-
-    def view(off, nb, dtype, shape):
-        return region[off:off + nb].view(dtype).view(shape)
-
-    def section(e, name, dtype, nbytes):
-        try:
-            off, nb = (int(v) for v in e["sections"][name])
-        except (KeyError, TypeError, ValueError):
-            bad(f"{e.get('name')}: section {name} missing")
-        if nb != nbytes:
-            bad(f"{e.get('name')}: section {name} holds {nb} bytes, {nbytes} expected")
-        if off < 0 or off % _ALIGN or off + nb > data_bytes:
-            bad(f"{e.get('name')}: section {name} out of range")
-        spans.append((off, nb))
-        return view(off, nb, dtype, (nbytes // dtype.itemsize,))
-
-    tensors, names = [], set()
-    for e in entries:
-        try:
-            name, shape, quantized = str(e["name"]), tuple(int(d) for d in e["shape"]), e["quantized"]
-        except (KeyError, TypeError, ValueError):
-            bad("tensor entry without name / shape / quantized")
-        if not isinstance(quantized, bool) or e.get("dtype") != "float32" or any(d < 0 for d in shape):
-            bad(f"{name}: bad dtype, shape or quantized flag")
-        if name in names:
-            bad(f"tensor {name} appears twice")
-        names.add(name)
-        if not isinstance(e.get("sections"), dict) or set(e["sections"]) != ({"packed", "alpha", "beta"} if quantized else {"raw"}):
-            bad(f"{name}: unexpected sections")
-        n = int(math.prod(shape))
-        if not quantized:
-            tensors.append(PackedEntry(name, shape, raw=section(e, "raw", torch.float32, 4 * n)))
-            continue
-        if n == 0:
-            bad(f"{name}: empty quantized tensor")
-        bits = e.get("bits")
-        if bits not in (1, 2, 4, 8) or isinstance(bits, bool):
-            bad(f"{name}: bits must be 1, 2, 4 or 8")
-        pts = None
-        if kind == "uniform":
-            if "points" in e:
-                bad(f"{name}: a uniform tensor has no points")
-            if levels > 1 << bits:
-                bad(f"{name}: {levels} levels do not fit in {bits}-bit codes")
-        else:
-            try:
-                pts = torch.tensor([float(v) for v in e["points"]], dtype=torch.float32)
-            except (KeyError, TypeError, ValueError):
-                bad(f"{name}: non-uniform tensor without points")
-            if not 1 <= pts.numel() <= 1 << bits:
-                bad(f"{name}: {pts.numel()} points do not fit in {bits}-bit codes")
-        rows = _rows(n, bucket)
-        tensors.append(PackedEntry(name, shape, bits=bits, packed=section(e, "packed", torch.uint8, (n * bits + 7) // 8),
-                                   alpha=section(e, "alpha", torch.float32, 4 * rows),
-                                   beta=section(e, "beta", torch.float32, 4 * rows), points=pts))
-    if not any(t.quantized for t in tensors):
-        bad("no quantized tensor")
-    buffers = None
-    if "buffers" in h:
-        buffers = _read_buffers(h["buffers"], view, data_bytes, bad, spans)
-    spans.sort()
-    for (o1, n1), (o2, _) in zip(spans, spans[1:]):
-        if o1 + n1 > o2:
-            bad(f"sections at {o1} and {o2} overlap")
-    pm = PackedModel(kind, levels, bucket, tensors, buffers=buffers)
-    pm._data = region
-    if device is not None:                       # everything is validated before anything reaches the GPU
-        move = _mover(pm, torch.device(device))
-        pts = [t.points for t in tensors if t.points is not None]
-        flat = torch.cat(pts).to(device) if pts else None          # every tensor's points in one upload too
-        at = 0
-        for t in tensors:
-            for f_ in ("packed", "alpha", "beta", "raw"):
-                setattr(t, f_, move(getattr(t, f_)))
-            if t.points is not None:
-                t.points, at = flat[at:at + t.points.numel()], at + t.points.numel()
-        if buffers is not None:
-            pm.buffers = [(name, move(b)) for name, b in buffers]
-        pm._data = move(region)
-    return pm
+    return _read_container(PackedModel, path, device)
 
 
 def get_size_reduction(effective_number_bits, bucket_size=256, full_precision_bits=32):

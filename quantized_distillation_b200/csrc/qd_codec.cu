@@ -289,12 +289,7 @@ __global__ void __launch_bounds__(256, 4) unpack_dequant_model_kernel(const qd_p
                                                                   int64_t bucket, float S) {
     __shared__ float s_unit[256];
     const int b = (int)blockIdx.x;
-    int lo = 0, hi = count;                       // cta_start[lo] <= b < cta_start[hi]
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(cta_start + mid) <= b) lo = mid;
-        else hi = mid;
-    }
+    const int lo = model_tensor_of(cta_start, count, b);
     const qd_packed_tensor& t = tensors[lo];
     load_unit_table<UNIFORM>(s_unit, t.points, t.num_points, S);
     __syncthreads();
@@ -312,30 +307,56 @@ __global__ void __launch_bounds__(256, 4) unpack_dequant_model_kernel(const qd_p
     }
 }
 
-// workspace of the model unpack: the tensor array, then cta_start[count + 1] (int32)
-static_assert(sizeof(qd_packed_tensor) == 56 && sizeof(qd_packed_tensor) % alignof(int32_t) == 0,
-              "qd_packed_tensor layout is shared with codec.py");
-
-extern "C" size_t qd_unpack_model_workspace_bytes(int count) {
-    return count < 1 ? 0 : (size_t)count * sizeof(qd_packed_tensor) + ((size_t)count + 1) * sizeof(int32_t);
+// ------------------------------------------------------------------ whole-model launches
+// qd_unpack_dequant_model and qd_huffman_decode_dequant_model read one workspace: the caller's descriptor array, then
+// cta_start[count + 1] (int32); the kernel finds a CTA's tensor with model_tensor_of.
+template <typename Desc>
+static size_t model_workspace_bytes(int count) {
+    static_assert(sizeof(Desc) % alignof(int32_t) == 0, "cta_start follows the descriptors");
+    return count < 1 ? 0 : (size_t)count * sizeof(Desc) + ((size_t)count + 1) * sizeof(int32_t);
 }
+
+// Checks the workspace and every tensor -- ctas_of(i, tensors[i], &ctas) returns QD_OK with the tensor's CTA count, or
+// the status of fail() -- refuses grids of more than 2^31 - 1 CTAs (each `unit` of `size` `what`), then uploads the
+// image with one copy on `st`.  On QD_OK, *grid is the launch's CTA count and *dev_start the device cta_start; the
+// descriptors are at the start of the workspace.
+template <typename Desc, typename CtasOf>
+static int upload_model(const Desc* tensors, int count, void* workspace, size_t workspace_bytes, cudaStream_t st, CtasOf ctas_of,
+                        const char* unit, int size, const char* what, unsigned* grid, const int32_t** dev_start) {
+    const size_t need = model_workspace_bytes<Desc>(count);
+    if (workspace == nullptr || (reinterpret_cast<uintptr_t>(workspace) & 15) || workspace_bytes < need)
+        return fail(QD_ERR_WORKSPACE, "workspace must be 16-byte aligned and hold %zu bytes (got %zu)", need, workspace_bytes);
+    // host image of the workspace, consumed by the pageable copy before it returns (kept per thread: no allocation once grown)
+    thread_local std::vector<unsigned char> image;
+    image.resize(need);
+    int32_t* cta_start = reinterpret_cast<int32_t*>(image.data() + (size_t)count * sizeof(Desc));
+    int64_t ctas = 0;
+    for (int i = 0; i < count; ++i) {
+        int64_t c = 0;
+        if (const int rc = ctas_of(i, tensors[i], &c)) return rc;
+        cta_start[i] = (int32_t)ctas;
+        ctas += c;
+        if (ctas > INT32_MAX) return fail(QD_ERR_INVALID_ARG, "the model has more than 2^31 - 1 %s of %d %s", unit, size, what);
+    }
+    cta_start[count] = (int32_t)ctas;
+    memcpy(image.data(), tensors, (size_t)count * sizeof(Desc));
+    QD_CUDA(cudaMemcpyAsync(workspace, image.data(), need, cudaMemcpyHostToDevice, st));
+    *grid = (unsigned)ctas;
+    *dev_start = reinterpret_cast<const int32_t*>(static_cast<const unsigned char*>(workspace) + (size_t)count * sizeof(Desc));
+    return QD_OK;
+}
+
+static_assert(sizeof(qd_packed_tensor) == 56, "qd_packed_tensor layout is shared with codec.py");
+
+extern "C" size_t qd_unpack_model_workspace_bytes(int count) { return model_workspace_bytes<qd_packed_tensor>(count); }
 
 extern "C" int qd_unpack_dequant_model(const qd_packed_tensor* tensors, int count, int64_t bucket, int levels, void* workspace,
                                        size_t workspace_bytes, qd_stream_t stream) {
     if (tensors == nullptr || count < 1) return fail(QD_ERR_INVALID_ARG, "NULL tensors or count < 1");
     if (bucket < 0) return fail(QD_ERR_INVALID_ARG, "bucket must be >= 0");
     if (levels != 0 && (levels < 2 || levels > 256)) return fail(QD_ERR_INVALID_ARG, "levels must be in [2, 256] (uniform) or 0 (non-uniform)");
-    const size_t need = qd_unpack_model_workspace_bytes(count);
-    if (workspace == nullptr || (reinterpret_cast<uintptr_t>(workspace) & 15) || workspace_bytes < need)
-        return fail(QD_ERR_WORKSPACE, "workspace must be 16-byte aligned and hold %zu bytes (got %zu)", need, workspace_bytes);
     const bool uniform = levels != 0;
-    // host image of the workspace, consumed by the pageable copy before it returns (kept per thread: no allocation once grown)
-    thread_local std::vector<unsigned char> image;
-    image.resize(need);
-    int32_t* cta_start = reinterpret_cast<int32_t*>(image.data() + (size_t)count * sizeof(qd_packed_tensor));
-    int64_t ctas = 0;
-    for (int i = 0; i < count; ++i) {
-        const qd_packed_tensor& t = tensors[i];
+    auto ctas_of = [&](int i, const qd_packed_tensor& t, int64_t* ctas) {
         if (t.packed == nullptr || t.alpha == nullptr || t.beta == nullptr || t.q == nullptr)
             return fail(QD_ERR_INVALID_ARG, "tensor %d: NULL argument", i);
         if (t.n < 1) return fail(QD_ERR_INVALID_ARG, "tensor %d: n must be >= 1", i);
@@ -345,20 +366,20 @@ extern "C" int qd_unpack_dequant_model(const qd_packed_tensor* tensors, int coun
         if (uniform && levels > (1 << t.bits)) return fail(QD_ERR_INVALID_ARG, "tensor %d: %d levels do not fit in %d-bit codes", i, levels, t.bits);
         if (!uniform && (t.points == nullptr || t.num_points < 1 || t.num_points > (1 << t.bits)))
             return fail(QD_ERR_INVALID_ARG, "tensor %d: num_points must be in [1, 2^bits]", i);
-        cta_start[i] = (int32_t)ctas;
-        ctas += ((t.n + 3) / 4 + kTileGroups - 1) / kTileGroups;
-        if (ctas > INT32_MAX) return fail(QD_ERR_INVALID_ARG, "the model has more than 2^31 - 1 tiles of %d elements", kTileGroups * 4);
-    }
-    cta_start[count] = (int32_t)ctas;
-    memcpy(image.data(), tensors, (size_t)count * sizeof(qd_packed_tensor));
+        *ctas = ((t.n + 3) / 4 + kTileGroups - 1) / kTileGroups;
+        return (int)QD_OK;
+    };
     cudaStream_t st = as_stream(stream);
-    QD_CUDA(cudaMemcpyAsync(workspace, image.data(), need, cudaMemcpyHostToDevice, st));
+    unsigned ctas;
+    const int32_t* dev_start;
+    if (const int rc = upload_model(tensors, count, workspace, workspace_bytes, st, ctas_of, "tiles", kTileGroups * 4, "elements",
+                                    &ctas, &dev_start))
+        return rc;
     const qd_packed_tensor* dev_tensors = static_cast<const qd_packed_tensor*>(workspace);
-    const int32_t* dev_start = reinterpret_cast<const int32_t*>(static_cast<const unsigned char*>(workspace) + (size_t)count * sizeof(qd_packed_tensor));
     if (uniform)
-        unpack_dequant_model_kernel<true><<<(unsigned)ctas, 256, 0, st>>>(dev_tensors, dev_start, count, bucket, (float)(levels - 1));
+        unpack_dequant_model_kernel<true><<<ctas, 256, 0, st>>>(dev_tensors, dev_start, count, bucket, (float)(levels - 1));
     else
-        unpack_dequant_model_kernel<false><<<(unsigned)ctas, 256, 0, st>>>(dev_tensors, dev_start, count, bucket, 0.f);
+        unpack_dequant_model_kernel<false><<<ctas, 256, 0, st>>>(dev_tensors, dev_start, count, bucket, 0.f);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }
@@ -693,13 +714,9 @@ extern "C" int qd_huffman_decode_dequant_nonuniform(const uint32_t* words, int64
                                       stream);
 }
 
-// workspace of the model decode: the tensor array, then cta_start[count + 1] (int32)
-static_assert(sizeof(qd_huffman_tensor) == 72 && sizeof(qd_huffman_tensor) % alignof(int32_t) == 0,
-              "qd_huffman_tensor layout is shared with codec.py");
+static_assert(sizeof(qd_huffman_tensor) == 72, "qd_huffman_tensor layout is shared with codec.py");
 
-extern "C" size_t qd_huffman_model_workspace_bytes(int count) {
-    return count < 1 ? 0 : (size_t)count * sizeof(qd_huffman_tensor) + ((size_t)count + 1) * sizeof(int32_t);
-}
+extern "C" size_t qd_huffman_model_workspace_bytes(int count) { return model_workspace_bytes<qd_huffman_tensor>(count); }
 
 extern "C" int qd_huffman_decode_dequant_model(const qd_huffman_tensor* tensors, int count, const qd_huffman_table* table,
                                                int64_t bucket, int levels, void* workspace, size_t workspace_bytes,
@@ -707,17 +724,8 @@ extern "C" int qd_huffman_decode_dequant_model(const qd_huffman_tensor* tensors,
     if (tensors == nullptr || count < 1 || table == nullptr) return fail(QD_ERR_INVALID_ARG, "NULL tensors / table or count < 1");
     if (bucket < 0) return fail(QD_ERR_INVALID_ARG, "bucket must be >= 0");
     if (levels != 0 && (levels < 2 || levels > 256)) return fail(QD_ERR_INVALID_ARG, "levels must be in [2, 256] (uniform) or 0 (non-uniform)");
-    const size_t need = qd_huffman_model_workspace_bytes(count);
-    if (workspace == nullptr || (reinterpret_cast<uintptr_t>(workspace) & 15) || workspace_bytes < need)
-        return fail(QD_ERR_WORKSPACE, "workspace must be 16-byte aligned and hold %zu bytes (got %zu)", need, workspace_bytes);
     const bool uniform = levels != 0;
-    // host image of the workspace, consumed by the pageable copy before it returns (kept per thread: no allocation once grown)
-    thread_local std::vector<unsigned char> image;
-    image.resize(need);
-    int32_t* cta_start = reinterpret_cast<int32_t*>(image.data() + (size_t)count * sizeof(qd_huffman_tensor));
-    int64_t ctas = 0;
-    for (int i = 0; i < count; ++i) {
-        const qd_huffman_tensor& t = tensors[i];
+    auto ctas_of = [&](int i, const qd_huffman_tensor& t, int64_t* ctas) {
         if (t.chunk_offsets == nullptr || t.alpha == nullptr || t.beta == nullptr || t.q == nullptr)
             return fail(QD_ERR_INVALID_ARG, "tensor %d: NULL argument", i);
         if (t.num_words < 0 || (t.num_words > 0 && t.words == nullptr)) return fail(QD_ERR_INVALID_ARG, "tensor %d: bad words / num_words", i);
@@ -727,21 +735,21 @@ extern "C" int qd_huffman_decode_dequant_model(const qd_huffman_tensor* tensors,
             return fail(QD_ERR_INVALID_ARG, "tensor %d: a uniform model has no points (points NULL, num_points 0)", i);
         if (!uniform && (t.points == nullptr || t.num_points < 1 || t.num_points > 256))
             return fail(QD_ERR_INVALID_ARG, "tensor %d: num_points must be in [1, 256]", i);
-        cta_start[i] = (int32_t)ctas;
-        ctas += ((t.n + kHuffChunk - 1) / kHuffChunk + kHuffDecThreads - 1) / kHuffDecThreads;
-        if (ctas > INT32_MAX) return fail(QD_ERR_INVALID_ARG, "the model has more than 2^31 - 1 blocks of %d chunks", kHuffDecThreads);
-    }
-    cta_start[count] = (int32_t)ctas;
-    memcpy(image.data(), tensors, (size_t)count * sizeof(qd_huffman_tensor));
+        *ctas = ((t.n + kHuffChunk - 1) / kHuffChunk + kHuffDecThreads - 1) / kHuffDecThreads;
+        return (int)QD_OK;
+    };
     cudaStream_t st = as_stream(stream);
-    QD_CUDA(cudaMemcpyAsync(workspace, image.data(), need, cudaMemcpyHostToDevice, st));
+    unsigned ctas;
+    const int32_t* dev_start;
+    if (const int rc = upload_model(tensors, count, workspace, workspace_bytes, st, ctas_of, "blocks", kHuffDecThreads, "chunks",
+                                    &ctas, &dev_start))
+        return rc;
     const qd_huffman_tensor* dev_tensors = static_cast<const qd_huffman_tensor*>(workspace);
-    const int32_t* dev_start = reinterpret_cast<const int32_t*>(static_cast<const unsigned char*>(workspace) + (size_t)count * sizeof(qd_huffman_tensor));
     if (uniform)
-        huff_decode_dequant_model_kernel<true><<<(unsigned)ctas, kHuffDecThreads, 0, st>>>(dev_tensors, dev_start, count, table, bucket,
-                                                                                           (float)(levels - 1));
+        huff_decode_dequant_model_kernel<true><<<ctas, kHuffDecThreads, 0, st>>>(dev_tensors, dev_start, count, table, bucket,
+                                                                                 (float)(levels - 1));
     else
-        huff_decode_dequant_model_kernel<false><<<(unsigned)ctas, kHuffDecThreads, 0, st>>>(dev_tensors, dev_start, count, table, bucket, 0.f);
+        huff_decode_dequant_model_kernel<false><<<ctas, kHuffDecThreads, 0, st>>>(dev_tensors, dev_start, count, table, bucket, 0.f);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }

@@ -179,4 +179,16 @@ inline int geometry_of(int64_t n, int64_t bucket, Geometry* g) {
     return QD_OK;
 }
 
+// Whole-model launches: tensor t owns CTAs [cta_start[t], cta_start[t + 1]) of one grid.  The tensor of CTA b, found by
+// binary search over cta_start[0..count].
+__device__ __forceinline__ int model_tensor_of(const int32_t* __restrict__ cta_start, int count, int b) {
+    int lo = 0, hi = count;                       // cta_start[lo] <= b < cta_start[hi]
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(cta_start + mid) <= b) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+
 }  // namespace qd

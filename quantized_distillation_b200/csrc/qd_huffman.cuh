@@ -302,12 +302,7 @@ __global__ void __launch_bounds__(kHuffDecThreads, 10) huff_decode_dequant_model
     const qd_huffman_table* __restrict__ tab, int64_t bucket, float S) {
     __shared__ HuffDecodeShared s;
     const int b = (int)blockIdx.x;
-    int lo = 0, hi = count;                       // cta_start[lo] <= b < cta_start[hi]
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(cta_start + mid) <= b) lo = mid;
-        else hi = mid;
-    }
+    const int lo = model_tensor_of(cta_start, count, b);
     const qd_huffman_tensor& t = tensors[lo];
     huff_load_tables<UNIFORM>(s, tab, S, t.points, t.num_points);
     const int max_len = (int)tab->max_length;

@@ -186,7 +186,29 @@ def test_malformed_files_are_rejected(tmp_path):
     def incomplete(h):
         h["code"] = [[0, 1], [1, 3]]
     rejected(_rewrite_header(good, incomplete), "Kraft")
+
+    # the checks both containers share: the Huffman reader refuses what the fixed-width reader refuses
+    def edit(fn):
+        return _rewrite_header(good, fn)
+    rejected(good[:12] + struct.pack("<I", 1) + good[16:], "reserved")
+    rejected(edit(lambda h: h.__setitem__("data_bytes", float(h["data_bytes"]))), "data_bytes")
+    rejected(edit(lambda h: h["tensors"][2].__setitem__("name", "t0")), "twice")                     # duplicate tensor name
+    rejected(edit(lambda h: h["tensors"][0].__setitem__("quantized", 0)), "quantized flag")
+    rejected(edit(lambda h: h["tensors"][1]["sections"].__setitem__("packed", [0, 0])), "sections")  # unexpected section
+    rejected(edit(lambda h: h["tensors"][1].__setitem__("points", [0.0, 1.0])), "no points")        # points on a uniform model
+    rejected(edit(lambda h: h["tensors"][2]["sections"].__setitem__(
+        "alpha", [h["tensors"][1]["sections"]["words"][0], h["tensors"][2]["sections"]["alpha"][1]])), "overlap")
+    codec.save_compressed(_oracle_model("nonuniform", None), path)
+    rejected(_rewrite_header(path.read_bytes(), lambda h: h.__setitem__("levels", 16)), "no levels")
+    codec.save_compressed(_oracle_model(bucket=1), path)       # bucket true would read as 1
+    rejected(_rewrite_header(path.read_bytes(), lambda h: h.__setitem__("bucket", True)), "bucket")
+    codec.save_compressed(_oracle_model(), path)
     assert codec.load_compressed(path).tensors[1].numel == 2000
+
+
+def test_compress_model_refuses_an_unknown_rule_before_device_work():
+    with pytest.raises(ValueError, match="rule"):
+        codec.compress_model(torch.nn.Linear(4, 4), points=[0.0, 0.5, 1.0], rule="midpiont")
 
 
 def test_decoding_needs_a_gpu(tmp_path):

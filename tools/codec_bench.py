@@ -65,7 +65,7 @@ def run(out_path, reps, numBits=2, bucket=256):
     from quantized_distillation_b200 import _native as N
     dev = outs[0].device
     items = [(t, d) for t, d in zip(cm.tensors, outs) if t.quantized]
-    args, keep = codec._model_decode_args(cm, items, dev, codec._mover(cm, dev))
+    args, keep = codec._decode_args(cm, items, dev, codec._mover(cm, dev))
     launches = 50
     for _ in range(5):
         N.check(N.lib().qd_huffman_decode_dequant_model(*args))

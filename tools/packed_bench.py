@@ -128,9 +128,9 @@ def model(launches, rounds, numBits=2, bucket=256):
     outs = [p.data for p in fresh.parameters()]
     dev = outs[0].device
     items = [(t, d) for t, d in zip(pm.tensors, outs) if t.quantized]
-    args, keep = codec._packed_decode_args(pm, items, dev, codec._mover(pm, dev))
+    args, keep = codec._decode_args(pm, items, dev, codec._mover(pm, dev))
     h_items = [(t, d) for t, d in zip(cm.tensors, outs) if t.quantized]
-    h_args, h_keep = codec._model_decode_args(cm, h_items, dev, codec._mover(cm, dev))
+    h_args, h_keep = codec._decode_args(cm, h_items, dev, codec._mover(cm, dev))
     lib, sp, s = N.lib(), N.stream_ptr(), 2 ** numBits
 
     def per_tensor():
