@@ -254,11 +254,19 @@ extern "C" int qd_plan_uniform_fwd_save(const qd_plan* p, qd_stream_t stream) {
 extern "C" int qd_plan_uniform_bwd(const qd_plan* p, float* const* grad, int mode, qd_stream_t stream) {
     if (p == nullptr || grad == nullptr) return fail(QD_ERR_INVALID_ARG, "plan or grad is NULL");
     if (mode == QD_BWD_STE) return QD_OK;  // identity
+    if (mode != QD_BWD_TRUNCATED && mode != QD_BWD_MINMAX) return fail(QD_ERR_INVALID_ARG, "unknown backward mode %d", mode);
+    // Every refusal comes before the first launch, so a refused call leaves every gradient untouched: the per-tensor
+    // fallback below fixes the tensors up in place one after the other, and the op refuses min/max rows beyond the
+    // staged path (qd_quant.cu run_rows) only when it reaches them.
+    if (mode == QD_BWD_MINMAX && p->bucket == 0)
+        return fail(QD_ERR_UNSUPPORTED, "minmax backward needs a bucket size (quant_functions.py:332-334)");
+    if (mode == QD_BWD_MINMAX && p->max_row_len > QD_MAX_STAGED_BUCKET)
+        return fail(QD_ERR_UNSUPPORTED, "minmax backward needs rows of at most %d elements (plan has %lld)", QD_MAX_STAGED_BUCKET,
+                    (long long)p->max_row_len);
+    for (int i = 0; i < p->count; ++i)
+        if (grad[i] == nullptr) return fail(QD_ERR_INVALID_ARG, "grad[%d] is NULL", i);
     cudaStream_t s = as_stream(stream);
     if (p->long_path) {
-        if (mode == QD_BWD_MINMAX)
-            return fail(QD_ERR_UNSUPPORTED, "minmax backward needs a bucket size (quant_functions.py:332-334)");
-        if (mode != QD_BWD_TRUNCATED) return fail(QD_ERR_INVALID_ARG, "unknown backward mode %d", mode);
         int grid;
         int rc = capped_grid(p->long_chunks, 4, &grid);
         if (rc) return rc;
@@ -277,11 +285,6 @@ extern "C" int qd_plan_uniform_bwd(const qd_plan* p, float* const* grad, int mod
         }
         return QD_OK;
     }
-    if (mode == QD_BWD_MINMAX && p->bucket == 0)
-        return fail(QD_ERR_UNSUPPORTED, "minmax backward needs a bucket size (quant_functions.py:332-334)");
-    if (mode != QD_BWD_TRUNCATED && mode != QD_BWD_MINMAX) return fail(QD_ERR_INVALID_ARG, "unknown backward mode %d", mode);
-    for (int i = 0; i < p->count; ++i)
-        if (grad[i] == nullptr) return fail(QD_ERR_INVALID_ARG, "grad[%d] is NULL", i);
     GradTable gt;
     float* const* dev_grads;
     int rc = plan_grads(p, grad, s, &gt, &dev_grads);
