@@ -209,6 +209,22 @@ int qd_packed_linear(const float* x, int64_t m, int64_t in_features, int64_t out
                      const float* alpha, const float* beta, const float* points, int num_points, int levels, int64_t bucket,
                      const float* bias, float* y, qd_stream_t stream);
 
+/* Convolution on packed weights: y = conv2d(x, W) (+ bias) for x float32[batch, in_channels, height, width] and
+ * y float32[batch, out_channels, Ho, Wo] (NCHW, C order), groups 1, dilation 1, zero padding pad_h / pad_w on both
+ * sides, Ho = (height + 2*pad_h - kernel_h) / stride_h + 1 (Wo likewise).  W is the tensor of
+ * out_channels*in_channels*kernel_h*kernel_w elements (flattened [O, C, kh, kw]) that qd_unpack_dequant_* writes from
+ * (packed, alpha, beta) at this bucket: the weights are the stored ones, bit for bit.  levels, points, num_points and
+ * bias as for qd_packed_linear.  Each output is one float32 fmaf chain over k = (c*kh + r)*kw + s in increasing order,
+ * the bias added last: the order depends on (in_channels, kernel_h, kernel_w) alone, so an image gives the same bits
+ * alone or in any batch, and repeated calls and replicas agree.  QD_ERR_INVALID_ARG: NULL pointers, sizes < 1,
+ * strides < 1, padding < 0, an empty output, bits too narrow, y overlapping x.  QD_ERR_UNSUPPORTED: sides or padding
+ * of 2^29 or more, K = in_channels*kernel_h*kernel_w of 2^31 or more, more output tiles than one launch holds.  Needs
+ * no workspace; only enqueues work on `stream`. */
+int qd_packed_conv2d(const float* x, int64_t batch, int64_t in_channels, int64_t height, int64_t width, int64_t out_channels,
+                     int kernel_h, int kernel_w, int stride_h, int stride_w, int pad_h, int pad_w, const uint8_t* packed,
+                     int bits, const float* alpha, const float* beta, const float* points, int num_points, int levels,
+                     int64_t bucket, const float* bias, float* y, qd_stream_t stream);
+
 /* ---- next row f2: Huffman-coded storage (the model helpers/functions.py:226-262 only sizes) ----------
  * Canonical code over uint8 symbols, codes of 1..QD_HUFFMAN_MAX_LENGTH bits (built on the host: codec.py).
  * Stream: a tensor's symbols are cut into chunks of QD_HUFFMAN_CHUNK; each chunk's codes are written MSB-first

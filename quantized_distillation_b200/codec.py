@@ -940,6 +940,55 @@ def unpack_(pm: PackedModel, model) -> None:
     _write_into(pm, *_check_target(pm, model))
 
 
+def _hold_sections(layer, entry: PackedEntry, kind: str, levels, bucket_size, bias, out: int) -> None:
+    """Registers one quantized tensor's packed sections (and the layer's bias of ``out`` elements) as non-persistent
+    buffers of ``layer`` on the sections' CUDA device: what PackedLinear and PackedConv2d hold in place of a float32
+    weight."""
+    if kind not in ("uniform", "nonuniform"):
+        raise ValueError(f"unknown kind {kind!r}")
+    layer.kind, layer.bits, layer.bucket_size = kind, int(entry.bits), bucket_size
+    layer.levels = int(levels) if kind == "uniform" else 0
+    dev = entry.packed.device
+    if not dev.type == "cuda":
+        raise ValueError(f"{entry.name}: the packed sections must be on a CUDA device")
+
+    def own(t):                                  # a view into a loaded file's region is copied out of it
+        t = t.to(dev).contiguous()
+        return t.clone() if t.untyped_storage().nbytes() > t.numel() * t.element_size() else t
+    layer.register_buffer("packed", own(entry.packed), persistent=False)
+    layer.register_buffer("alpha", own(entry.alpha.to(torch.float32)), persistent=False)
+    layer.register_buffer("beta", own(entry.beta.to(torch.float32)), persistent=False)
+    layer.register_buffer("points", None if kind == "uniform" else own(entry.points.reshape(-1).to(torch.float32)), persistent=False)
+    if bias is not None:
+        if tuple(bias.shape) != (out,):
+            raise ValueError(f"{entry.name}: bias of shape {tuple(bias.shape)}, expected ({out},)")
+        bias = bias.detach().to(dev, torch.float32).contiguous()
+    layer.register_buffer("bias", bias, persistent=False)
+
+
+def _check_input(layer, x, what: str) -> None:
+    if not torch.is_tensor(x) or not x.is_cuda or x.dtype != torch.float32:
+        raise ValueError(f"{what} takes a float32 CUDA tensor")
+    if x.device != layer.packed.device:
+        raise ValueError(f"input on {x.device}, the packed weight on {layer.packed.device}")
+
+
+def _check_state(layer, x, what: str) -> None:
+    """Refusals after the input's shape: sections cast away from uint8 / float32, an input that needs a gradient in
+    grad mode."""
+    if layer.packed.dtype != torch.uint8 or any(t is not None and t.dtype != torch.float32 for t in (layer.alpha, layer.beta, layer.points, layer.bias)):
+        raise RuntimeError(f"{what}'s sections must stay uint8 codes and float32 scales, points and bias "
+                           "(the module was cast, e.g. by .half() or .double())")
+    if torch.is_grad_enabled() and x.requires_grad:
+        raise RuntimeError(f"{what} is forward only: it cannot propagate a gradient to its input "
+                           "(run it under torch.no_grad() or torch.inference_mode())")
+
+
+def _decoded(layer, shape) -> torch.Tensor:
+    w = torch.empty(*shape, dtype=torch.float32, device=layer.packed.device)
+    return _unpack(layer.packed, layer.bits, layer.alpha, layer.beta, layer.points, layer.levels, layer.bucket_size, w)
+
+
 class PackedLinear(torch.nn.Module):
     """Inference replacement of an ``nn.Linear`` whose weight stays in its fixed-width stored form (one PackedEntry of
     a PackedModel: codes, alpha and beta per bucket, points) on the device.  For batches of at most CROSSOVER_ROWS
@@ -957,27 +1006,8 @@ class PackedLinear(torch.nn.Module):
         super().__init__()
         if not entry.quantized or len(entry.shape) != 2:
             raise ValueError(f"{entry.name}: a PackedLinear needs a quantized two-dimensional weight")
-        if kind not in ("uniform", "nonuniform"):
-            raise ValueError(f"unknown kind {kind!r}")
         self.out_features, self.in_features = (int(d) for d in entry.shape)
-        self.kind, self.bits, self.bucket_size = kind, int(entry.bits), bucket_size
-        self.levels = int(levels) if kind == "uniform" else 0
-        dev = entry.packed.device
-        if not dev.type == "cuda":
-            raise ValueError(f"{entry.name}: the packed sections must be on a CUDA device")
-
-        def own(t):                              # a view into a loaded file's region is copied out of it
-            t = t.to(dev).contiguous()
-            return t.clone() if t.untyped_storage().nbytes() > t.numel() * t.element_size() else t
-        self.register_buffer("packed", own(entry.packed), persistent=False)
-        self.register_buffer("alpha", own(entry.alpha.to(torch.float32)), persistent=False)
-        self.register_buffer("beta", own(entry.beta.to(torch.float32)), persistent=False)
-        self.register_buffer("points", None if kind == "uniform" else own(entry.points.reshape(-1).to(torch.float32)), persistent=False)
-        if bias is not None:
-            if tuple(bias.shape) != (self.out_features,):
-                raise ValueError(f"{entry.name}: bias of shape {tuple(bias.shape)}, expected ({self.out_features},)")
-            bias = bias.detach().to(dev, torch.float32).contiguous()
-        self.register_buffer("bias", bias, persistent=False)
+        _hold_sections(self, entry, kind, levels, bucket_size, bias, self.out_features)
 
     def extra_repr(self) -> str:
         return (f"in_features={self.in_features}, out_features={self.out_features}, bias={self.bias is not None}, "
@@ -985,22 +1015,13 @@ class PackedLinear(torch.nn.Module):
 
     def decoded_weight(self) -> torch.Tensor:
         """The decoded float32 weight [out_features, in_features], bit for bit what unpack_ writes."""
-        w = torch.empty(self.out_features, self.in_features, dtype=torch.float32, device=self.packed.device)
-        return _unpack(self.packed, self.bits, self.alpha, self.beta, self.points, self.levels, self.bucket_size, w)
+        return _decoded(self, (self.out_features, self.in_features))
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if not torch.is_tensor(x) or not x.is_cuda or x.dtype != torch.float32:
-            raise ValueError("PackedLinear takes a float32 CUDA tensor")
-        if x.device != self.packed.device:
-            raise ValueError(f"input on {x.device}, the packed weight on {self.packed.device}")
+        _check_input(self, x, "PackedLinear")
         if x.dim() < 1 or x.shape[-1] != self.in_features:
             raise ValueError(f"input of shape {tuple(x.shape)}, expected (..., {self.in_features})")
-        if self.packed.dtype != torch.uint8 or any(t is not None and t.dtype != torch.float32 for t in (self.alpha, self.beta, self.points, self.bias)):
-            raise RuntimeError("PackedLinear's sections must stay uint8 codes and float32 scales, points and bias "
-                               "(the module was cast, e.g. by .half() or .double())")
-        if torch.is_grad_enabled() and x.requires_grad:
-            raise RuntimeError("PackedLinear is forward only: it cannot propagate a gradient to its input "
-                               "(run it under torch.no_grad() or torch.inference_mode())")
+        _check_state(self, x, "PackedLinear")
         lead = x.shape[:-1]
         x2 = x.reshape(-1, self.in_features).contiguous()
         m = x2.shape[0]
@@ -1017,6 +1038,145 @@ class PackedLinear(torch.nn.Module):
         return y.view(*lead, self.out_features)
 
 
+def _pair(v, what: str) -> tuple:
+    p = (v, v) if isinstance(v, int) else tuple(v)
+    if len(p) != 2 or not all(isinstance(i, int) and not isinstance(i, bool) for i in p):
+        raise ValueError(f"{what} must be an int or a pair of ints, got {v!r}")
+    return p
+
+
+class PackedConv2d(torch.nn.Module):
+    """Inference replacement of an ``nn.Conv2d`` (groups 1, dilation 1, symmetric zero padding) whose weight stays in
+    its fixed-width stored form (one PackedEntry of a PackedModel with a [O, C, kh, kw] shape) on the device.  Takes
+    NCHW float32 input, or one CHW image.  When the layer has K = C*kh*kw <= KERNEL_MAX_TAPS and a call's work,
+    N*Ho*Wo*O*K multiply-adds, is at most CROSSOVER_MACS (runs_kernel), forward runs qd_packed_conv2d, which reads the codes and never materialises the float32 weight; its
+    weights are the decoded ones bit for bit, each output is one float32 fmaf chain in a fixed order.  Above it, the
+    weight is decoded into a scratch tensor (qd_unpack_dequant_*), F.conv2d is called and the scratch is freed: exactly
+    what an unpack_-loaded nn.Conv2d computes, TF32 setting and input strides included (the kernel path reads a
+    contiguous copy of a non-contiguous input).  Forward only: an input that needs a gradient in
+    grad mode is refused.  No host synchronisation, so it can be captured in a CUDA graph."""
+    # Measured (DESIGN.md section 3.7.3): the kernel beats decode + F.conv2d (TF32 on) by 5-25 % on layers of 16 and
+    # 27 taps up to 8.4 M multiply-adds (WRN's 16->352 shortcut at batch 1, its stem up to batch 8); on every layer of
+    # 144 taps or more it loses at every batch, by up to 10x, since one CTA walks the whole K chain.
+    KERNEL_MAX_TAPS = 32
+    CROSSOVER_MACS = 1 << 23
+
+    def __init__(self, entry: PackedEntry, kind: str, levels, bucket_size, stride=1, padding=0, bias: torch.Tensor = None):
+        super().__init__()
+        if not entry.quantized or len(entry.shape) != 4:
+            raise ValueError(f"{entry.name}: a PackedConv2d needs a quantized four-dimensional weight")
+        self.out_channels, self.in_channels, kh, kw = (int(d) for d in entry.shape)
+        self.kernel_size = (kh, kw)
+        self.stride, self.padding = _pair(stride, "stride"), _pair(padding, "padding")
+        if min(self.stride) < 1 or min(self.padding) < 0:
+            raise ValueError(f"{entry.name}: stride must be >= 1 and padding >= 0")
+        _hold_sections(self, entry, kind, levels, bucket_size, bias, self.out_channels)
+
+    def extra_repr(self) -> str:
+        return (f"{self.in_channels}, {self.out_channels}, kernel_size={self.kernel_size}, stride={self.stride}, "
+                f"padding={self.padding}, bias={self.bias is not None}, {self.kind}, bits={self.bits}, bucket_size={self.bucket_size}")
+
+    def decoded_weight(self) -> torch.Tensor:
+        """The decoded float32 weight [out_channels, in_channels, kh, kw], bit for bit what unpack_ writes."""
+        return _decoded(self, (self.out_channels, self.in_channels, *self.kernel_size))
+
+    def runs_kernel(self, n: int, ho: int, wo: int) -> bool:
+        """True when a call with batch n and output Ho x Wo runs qd_packed_conv2d, False when it decodes."""
+        k = self.in_channels * self.kernel_size[0] * self.kernel_size[1]
+        return k <= self.KERNEL_MAX_TAPS and n * ho * wo * self.out_channels * k <= self.CROSSOVER_MACS
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        _check_input(self, x, "PackedConv2d")
+        if x.dim() not in (3, 4) or x.shape[-3] != self.in_channels:
+            raise ValueError(f"input of shape {tuple(x.shape)}, expected (N, {self.in_channels}, H, W) or ({self.in_channels}, H, W)")
+        _check_state(self, x, "PackedConv2d")
+        (kh, kw), (sh, sw), (ph, pw) = self.kernel_size, self.stride, self.padding
+        n, (h, w) = (x.shape[0] if x.dim() == 4 else 1), x.shape[-2:]
+        if h + 2 * ph < kh or w + 2 * pw < kw:
+            raise ValueError(f"input of shape {tuple(x.shape)} is smaller than the {kh}x{kw} kernel after padding {self.padding}")
+        ho, wo = (h + 2 * ph - kh) // sh + 1, (w + 2 * pw - kw) // sw + 1
+        with torch.cuda.device(x.device):
+            if not self.runs_kernel(n, ho, wo):
+                return torch.nn.functional.conv2d(x, self.decoded_weight(), self.bias, self.stride, self.padding)
+            xc = x.contiguous()
+            y = torch.empty(n, self.out_channels, ho, wo, dtype=torch.float32, device=x.device)
+            if n:
+                b = 0 if self.bucket_size is None else int(self.bucket_size)
+                N.check(N.lib().qd_packed_conv2d(N.ptr(xc), n, self.in_channels, h, w, self.out_channels, kh, kw, sh, sw, ph, pw,
+                                                 N.ptr(self.packed), self.bits, N.ptr(self.alpha), N.ptr(self.beta), N.ptr(self.points),
+                                                 0 if self.points is None else self.points.numel(), self.levels, b, N.ptr(self.bias),
+                                                 N.ptr(y), N.stream_ptr(x.device)))
+        return y if x.dim() == 4 else y[0]
+
+
+def _conv_padding(conv) -> tuple:
+    """(pad_h, pad_w) of an nn.Conv2d's padding when it is symmetric: an int pair, "valid", or "same" whose total
+    padding per side is even; None otherwise."""
+    p = conv.padding
+    if p == "valid":
+        return (0, 0)
+    if p == "same":
+        total = [d * (k - 1) for k, d in zip(conv.kernel_size, conv.dilation)]
+        return None if any(t % 2 for t in total) else tuple(t // 2 for t in total)
+    if isinstance(p, tuple) and len(p) == 2 and all(isinstance(v, int) for v in p):
+        return p
+    return None
+
+
+def _linear_target(mod) -> bool:
+    return isinstance(mod, torch.nn.Linear)
+
+
+def _conv_target(mod) -> bool:
+    # type, not isinstance: a subclass may override forward
+    return (type(mod) is torch.nn.Conv2d and mod.groups == 1 and tuple(mod.dilation) == (1, 1) and mod.padding_mode == "zeros"
+            and _conv_padding(mod) is not None)
+
+
+def _packed_linear(entry, pm, lin):
+    return PackedLinear(entry, pm.kind, pm.levels, pm.bucket_size, None if lin.bias is None else lin.bias.data)
+
+
+def _packed_conv(entry, pm, conv):
+    return PackedConv2d(entry, pm.kind, pm.levels, pm.bucket_size, conv.stride, _conv_padding(conv),
+                        None if conv.bias is None else conv.bias.data)
+
+
+def _attach(pm: PackedModel, model, kinds) -> list:
+    """unpack_, except that every module accepted by the ``accept`` of one of ``kinds`` -- (accept, make, what) -- whose
+    weight ``pm`` stores quantized and which is that weight's only holder is replaced in its parent by make(entry, pm,
+    module); the float32 weight is released.  Returns the names of the replaced modules."""
+    named, bufs = _check_target(pm, model)
+    index = {id(p): k for k, (_, p) in enumerate(named)}
+    holders = {}                                 # parameter -> registrations in the module tree, every path counted
+    for _, mod in model.named_modules(remove_duplicate=False):
+        for p in mod._parameters.values():
+            if p is not None:
+                holders[id(p)] = holders.get(id(p), 0) + 1
+    targets = []                                 # (module name, parent, attribute, module, weight index, make)
+    for mname, mod in model.named_modules():
+        for accept, make, what in kinds:
+            if accept(mod) and id(mod.weight) in index and pm.tensors[index[id(mod.weight)]].quantized \
+                    and holders[id(mod.weight)] == 1:
+                if not mod.weight.is_cuda:
+                    raise ValueError(f"{mname}: a Packed{what} runs on a CUDA device, the {what} is on {mod.weight.device}")
+                parent_name, _, attr = mname.rpartition(".")
+                targets.append((mname, model.get_submodule(parent_name) if parent_name else model, attr, mod, index[id(mod.weight)], make))
+                break
+    _write_into(pm, named, bufs, skip={t[4] for t in targets})
+    movers = {}
+    for mname, parent, attr, mod, k, make in targets:
+        dev = mod.weight.device
+        t = pm.tensors[k]
+        with torch.cuda.device(dev):
+            move = movers.setdefault(dev, _mover(pm, dev))
+            entry = PackedEntry(t.name, t.shape, bits=t.bits, packed=move(t.packed), alpha=move(t.alpha), beta=move(t.beta),
+                                points=None if t.points is None else t.points.to(dev))
+            layer = make(entry, pm, mod)
+        setattr(parent, attr, layer)
+    return [t[0] for t in targets]
+
+
 def attach_packed_linear_(pm: PackedModel, model) -> list:
     """unpack_, except that every ``nn.Linear`` whose weight ``pm`` stores quantized is replaced in its parent module
     by a PackedLinear holding that weight's packed sections (and the Linear's bias, decoded as unpack_ decodes it);
@@ -1026,33 +1186,18 @@ def attach_packed_linear_(pm: PackedModel, model) -> list:
     generator sharing the embedding's matrix) or the Linear itself registered under two parents -- stays an nn.Linear
     and its weight is decoded as unpack_ decodes it: replacing it in one place would leave the other holder with a
     weight that was never written.  Returns the names of the replaced modules."""
-    named, bufs = _check_target(pm, model)
-    index = {id(p): k for k, (_, p) in enumerate(named)}
-    holders = {}                                 # parameter -> registrations in the module tree, every path counted
-    for _, mod in model.named_modules(remove_duplicate=False):
-        for p in mod._parameters.values():
-            if p is not None:
-                holders[id(p)] = holders.get(id(p), 0) + 1
-    targets = []                                 # (module name, parent, attribute, Linear, weight index)
-    for mname, mod in model.named_modules():
-        if isinstance(mod, torch.nn.Linear) and id(mod.weight) in index and pm.tensors[index[id(mod.weight)]].quantized \
-                and holders[id(mod.weight)] == 1:
-            if not mod.weight.is_cuda:
-                raise ValueError(f"{mname}: a PackedLinear runs on a CUDA device, the Linear is on {mod.weight.device}")
-            parent_name, _, attr = mname.rpartition(".")
-            targets.append((mname, model.get_submodule(parent_name) if parent_name else model, attr, mod, index[id(mod.weight)]))
-    _write_into(pm, named, bufs, skip={k for *_, k in targets})
-    movers = {}
-    for mname, parent, attr, lin, k in targets:
-        dev = lin.weight.device
-        t = pm.tensors[k]
-        with torch.cuda.device(dev):
-            move = movers.setdefault(dev, _mover(pm, dev))
-            entry = PackedEntry(t.name, t.shape, bits=t.bits, packed=move(t.packed), alpha=move(t.alpha), beta=move(t.beta),
-                                points=None if t.points is None else t.points.to(dev))
-            layer = PackedLinear(entry, pm.kind, pm.levels, pm.bucket_size, None if lin.bias is None else lin.bias.data)
-        setattr(parent, attr, layer)
-    return [mname for mname, *_ in targets]
+    return _attach(pm, model, [(_linear_target, _packed_linear, "Linear")])
+
+
+def attach_packed_(pm: PackedModel, model) -> list:
+    """attach_packed_linear_ for Linear and convolution layers: every nn.Linear it would replace becomes a
+    PackedLinear, and every ``nn.Conv2d`` (the class itself, not a subclass) with groups 1, dilation 1, zero padding
+    that is symmetric (int padding, "valid", or "same" that resolves to equal sides) and a weight ``pm`` stores
+    quantized and it alone holds becomes a PackedConv2d with that weight's packed sections, its stride, padding and
+    bias.  The replaced float32 weights are released; every other parameter and layer, and the stored buffers, are
+    written exactly as unpack_ writes them, quantized tensors in one launch per device.  Everything is checked before
+    anything is written.  Returns the names of the replaced modules, in module order."""
+    return _attach(pm, model, [(_linear_target, _packed_linear, "Linear"), (_conv_target, _packed_conv, "Conv2d")])
 
 
 def save_packed(pm: PackedModel, path) -> int:

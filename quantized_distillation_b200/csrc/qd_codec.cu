@@ -657,6 +657,216 @@ extern "C" int qd_packed_linear(const float* x, int64_t m, int64_t in_features, 
     return go(std::integral_constant<int, 8>{});
 }
 
+// ------------------------------------------------------------------ f2: convolution on packed weights
+// y[n, o, ho, wo] = sum_k x[n, c, ho*sh - ph + r, wo*sw - pw + s] * q[o*K + k] (+ bias[o]), k = (c*kh + r)*kw + s,
+// K = C*kh*kw, taps outside the input read 0.  q is the tensor qd_unpack_dequant_* writes: every weight is
+// from_unit(unit[code], alpha[bucket], beta[bucket]) with the unit table of load_unit_table.
+//
+// Implicit GEMM over M = N*Ho*Wo output positions x O channels x K taps.  A CTA owns a tile of kPcBM positions and
+// kPcBO channels and walks K in slabs of kPcBK taps: it decodes the slab's weights from the codes into shared memory
+// (each thread four consecutive taps of one channel, a bucket cursor instead of a division), gathers the matching
+// input patch (each thread four consecutive taps of one position, a (c, r, s) cursor, padding zero-filled), then every
+// thread runs a 4 x 4 register micro-tile.  Each output is one fmaf chain over k = 0 .. K-1 in order, the bias added
+// last: the order depends on the layer alone, not on N, H, W, the grid or timing.
+constexpr int kPcBM = 64, kPcBO = 64, kPcBK = 16;
+constexpr int kPcThreads = 256;
+
+struct PackedConvArgs {
+    const float* x;
+    const uint8_t* packed;
+    const float* alpha;
+    const float* beta;
+    const float* points;
+    const float* bias;
+    float* y;
+    int64_t M, O, C, HW, HoWo;  // positions, channels, input channels, input and output plane sizes
+    int64_t L, rows;            // bucket row length and bucket count (geometry_of)
+    int64_t step_q, step_r;     // kPcBK / L and kPcBK % L: a bucket cursor from one slab to the next
+    int K, H, W, Wo, kh, kw, sh, sw, ph, pw;
+    int step_c, step_rr, step_s;  // kPcBK taps as (channels, rows, columns) of the window
+    int num_points;
+    float S;
+};
+
+template <bool UNIFORM, int BITS>
+__global__ void __launch_bounds__(kPcThreads, 2) packed_conv2d_kernel(PackedConvArgs a) {
+    constexpr unsigned mask = (1u << BITS) - 1u;
+    __shared__ float s_unit[256];
+    __shared__ __align__(16) float s_x[kPcBK][kPcBM];
+    __shared__ __align__(16) float s_w[kPcBK][kPcBO];
+    const int t = threadIdx.x;
+    const int64_t m0 = (int64_t)blockIdx.x * kPcBM, o0 = (int64_t)blockIdx.y * kPcBO;
+    const int lane4 = (t >> 6) * 4;     // first of the four taps this thread gathers and decodes per slab
+
+    // gather role: position m0 + (t & 63); tap cursor (gc, gr, gs) of tap lane4 of the slab
+    const int64_t gpos = m0 + (t & 63);
+    const bool gvalid = gpos < a.M;
+    const float* xb = a.x;
+    int hi0 = 0, wi0 = 0;
+    if (gvalid) {
+        const int64_t n = gpos / a.HoWo;
+        const int p = (int)(gpos - n * a.HoWo);
+        const int ho = p / a.Wo, wo = p - ho * a.Wo;
+        xb = a.x + n * a.C * a.HW;
+        hi0 = ho * a.sh - a.ph;
+        wi0 = wo * a.sw - a.pw;
+    }
+    int gc = lane4 / (a.kh * a.kw), gr = lane4 - gc * a.kh * a.kw, gs = gr % a.kw;
+    gr /= a.kw;
+
+    // decode role: channel o0 + (t & 63), elements o*K + k0 + lane4 .. +3; bucket cursor (bc, rc) of the first
+    const int64_t o = o0 + (t & 63);
+    const bool ovalid = o < a.O;
+    const int64_t e_first = (ovalid ? o : 0) * a.K + lane4;
+    int64_t bc = e_first / a.L, rc = e_first - bc * a.L;
+
+    load_unit_table<UNIFORM>(s_unit, a.points, a.num_points, a.S);
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    const int tx = t & 15, ty = t >> 4;   // micro-tile: positions m0 + 4*tx .. +3, channels o0 + 4*ty .. +3
+
+    for (int k0 = 0; k0 < a.K; k0 += kPcBK) {
+        __syncthreads();                  // the previous slab is consumed (and, at the first, the unit table written)
+        {   // input patch: taps k0 + lane4 + j of position gpos
+            int c = gc, r = gr, s = gs;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int hi = hi0 + r, wi = wi0 + s;
+                float v = 0.f;
+                if (gvalid && c < a.C && (unsigned)hi < (unsigned)a.H && (unsigned)wi < (unsigned)a.W)
+                    v = __ldg(xb + (int64_t)c * a.HW + (int64_t)hi * a.W + wi);
+                s_x[lane4 + j][t & 63] = v;
+                if (++s == a.kw) {
+                    s = 0;
+                    if (++r == a.kh) { r = 0; ++c; }
+                }
+            }
+        }
+        {   // weights: elements o*K + k0 + lane4 + j, walked with the bucket cursor
+            int64_t b = bc, rr = rc;
+            float al = __ldg(a.alpha + min(b, a.rows - 1)), be = __ldg(a.beta + min(b, a.rows - 1));
+            const int64_t e0 = o * a.K + k0 + lane4;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                float w = 0.f;
+                if (ovalid && k0 + lane4 + j < a.K) {
+                    const int64_t bit = (e0 + j) * BITS;
+                    const unsigned code = ((unsigned)__ldg(a.packed + (bit >> 3)) >> (unsigned)(bit & 7)) & mask;
+                    w = from_unit(s_unit[code], al, be);
+                }
+                s_w[lane4 + j][t & 63] = w;
+                if (++rr == a.L) {        // next element starts bucket b + 1
+                    rr = 0;
+                    ++b;
+                    al = __ldg(a.alpha + min(b, a.rows - 1));
+                    be = __ldg(a.beta + min(b, a.rows - 1));
+                }
+            }
+        }
+        // advance both cursors by one slab
+        bc += a.step_q;
+        rc += a.step_r;
+        if (rc >= a.L) { rc -= a.L; ++bc; }
+        gs += a.step_s;
+        if (gs >= a.kw) { gs -= a.kw; ++gr; }
+        gr += a.step_rr;
+        if (gr >= a.kh) { gr -= a.kh; ++gc; }
+        gc += a.step_c;
+        __syncthreads();
+        const int kn = min(kPcBK, a.K - k0);
+#pragma unroll
+        for (int kk = 0; kk < kPcBK; ++kk) {
+            if (kk < kn) {
+                const float4 xv = *reinterpret_cast<const float4*>(&s_x[kk][4 * tx]);
+                const float4 wv = *reinterpret_cast<const float4*>(&s_w[kk][4 * ty]);
+                const float xs[4] = {xv.x, xv.y, xv.z, xv.w}, ws[4] = {wv.x, wv.y, wv.z, wv.w};
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) acc[i][j] = __fmaf_rn(xs[i], ws[j], acc[i][j]);
+            }
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int64_t m = m0 + 4 * tx + i;
+        if (m >= a.M) break;
+        const int64_t n = m / a.HoWo;
+        float* yb = a.y + n * a.O * a.HoWo + (m - n * a.HoWo);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int64_t oc = o0 + 4 * ty + j;
+            if (oc < a.O) yb[oc * a.HoWo] = a.bias != nullptr ? __fadd_rn(acc[i][j], __ldg(a.bias + oc)) : acc[i][j];
+        }
+    }
+}
+
+static bool mul_ok(int64_t p, int64_t q, int64_t* out) { return !__builtin_mul_overflow(p, q, out); }
+
+extern "C" int qd_packed_conv2d(const float* x, int64_t batch, int64_t in_channels, int64_t height, int64_t width,
+                                int64_t out_channels, int kernel_h, int kernel_w, int stride_h, int stride_w, int pad_h, int pad_w,
+                                const uint8_t* packed, int bits, const float* alpha, const float* beta, const float* points,
+                                int num_points, int levels, int64_t bucket, const float* bias, float* y, qd_stream_t stream) {
+    if (x == nullptr || packed == nullptr || alpha == nullptr || beta == nullptr || y == nullptr)
+        return fail(QD_ERR_INVALID_ARG, "NULL argument");
+    if (batch < 1 || in_channels < 1 || height < 1 || width < 1 || out_channels < 1 || kernel_h < 1 || kernel_w < 1)
+        return fail(QD_ERR_INVALID_ARG, "batch, channels, input and kernel sizes must be >= 1");
+    if (stride_h < 1 || stride_w < 1 || pad_h < 0 || pad_w < 0) return fail(QD_ERR_INVALID_ARG, "strides must be >= 1 and padding >= 0");
+    if (height > INT32_MAX / 4 || width > INT32_MAX / 4 || pad_h > INT32_MAX / 4 || pad_w > INT32_MAX / 4)
+        return fail(QD_ERR_UNSUPPORTED, "input sides and padding must be below 2^29");
+    const int64_t hp = height + 2 * (int64_t)pad_h, wp = width + 2 * (int64_t)pad_w;
+    if (hp < kernel_h || wp < kernel_w)
+        return fail(QD_ERR_INVALID_ARG, "the %dx%d kernel is larger than the padded %lldx%lld input: the output is empty", kernel_h,
+                    kernel_w, (long long)hp, (long long)wp);
+    const int64_t ho = (hp - kernel_h) / stride_h + 1, wo = (wp - kernel_w) / stride_w + 1;
+    int64_t K, n, hw, howo, x_n, y_n, m;
+    if (!mul_ok(in_channels, (int64_t)kernel_h * kernel_w, &K) || !mul_ok(K, out_channels, &n) || n > INT64_MAX / 8 ||
+        !mul_ok(height, width, &hw) || !mul_ok(ho, wo, &howo) || !mul_ok(hw, in_channels, &x_n) || !mul_ok(x_n, batch, &x_n) ||
+        !mul_ok(howo, out_channels, &y_n) || !mul_ok(y_n, batch, &y_n) || !mul_ok(howo, batch, &m) || x_n > INT64_MAX / 4 ||
+        y_n > INT64_MAX / 4)
+        return fail(QD_ERR_INVALID_ARG, "the layer's sizes overflow 64-bit indexing");
+    if (K > INT32_MAX) return fail(QD_ERR_UNSUPPORTED, "K = in_channels * kernel_h * kernel_w = %lld: at most 2^31 - 1", (long long)K);
+    const int64_t m_tiles = (m + kPcBM - 1) / kPcBM, o_tiles = (out_channels + kPcBO - 1) / kPcBO;
+    if (m_tiles > INT32_MAX || o_tiles > 65535)
+        return fail(QD_ERR_UNSUPPORTED, "%lld output positions x %lld channels: more tiles than one launch holds", (long long)m,
+                    (long long)out_channels);
+    if (!bits_ok(bits)) return fail(QD_ERR_INVALID_ARG, "bits must be 1, 2, 4 or 8");
+    const bool uniform = levels != 0;
+    if (uniform) {
+        if (points != nullptr || num_points != 0) return fail(QD_ERR_INVALID_ARG, "uniform weights have no points (points NULL, num_points 0)");
+        if (levels < 2 || levels > (1 << bits)) return fail(QD_ERR_INVALID_ARG, "levels must be in [2, 2^bits]");
+    } else if (points == nullptr || num_points < 1 || num_points > (1 << bits)) {
+        return fail(QD_ERR_INVALID_ARG, "num_points must be in [1, 2^bits]");
+    }
+    Geometry geo;
+    if (geometry_of(n, bucket, &geo)) return fail(QD_ERR_INVALID_ARG, "bucket must be >= 0");
+    const uintptr_t xb = reinterpret_cast<uintptr_t>(x), xe = xb + (uintptr_t)x_n * sizeof(float);
+    const uintptr_t yb = reinterpret_cast<uintptr_t>(y), ye = yb + (uintptr_t)y_n * sizeof(float);
+    if (xb < ye && yb < xe) return fail(QD_ERR_INVALID_ARG, "y must not overlap x");
+    PackedConvArgs a{};
+    a.x = x, a.packed = packed, a.alpha = alpha, a.beta = beta, a.points = points, a.bias = bias, a.y = y;
+    a.M = m, a.O = out_channels, a.C = in_channels, a.HW = hw, a.HoWo = howo;
+    a.L = geo.row_len, a.rows = geo.rows;
+    a.step_q = kPcBK / a.L, a.step_r = kPcBK % a.L;
+    a.K = (int)K, a.H = (int)height, a.W = (int)width, a.Wo = (int)wo;
+    a.kh = kernel_h, a.kw = kernel_w, a.sh = stride_h, a.sw = stride_w, a.ph = pad_h, a.pw = pad_w;
+    const int taps = kernel_h * kernel_w;
+    a.step_c = kPcBK / taps, a.step_rr = (kPcBK % taps) / kernel_w, a.step_s = (kPcBK % taps) % kernel_w;
+    a.num_points = num_points;
+    a.S = uniform ? (float)(levels - 1) : 0.f;
+    const dim3 grid((unsigned)m_tiles, (unsigned)o_tiles);
+    cudaStream_t st = as_stream(stream);
+    with_bits(bits, [&](auto b) {
+        if (uniform) packed_conv2d_kernel<true, b><<<grid, kPcThreads, 0, st>>>(a);
+        else packed_conv2d_kernel<false, b><<<grid, kPcThreads, 0, st>>>(a);
+    });
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
 // ------------------------------------------------------------------ f2: Huffman-coded storage (qd_huffman.cuh)
 extern "C" int qd_huffman_encode(const uint8_t* idx_u8, int64_t n, const qd_huffman_table* table, uint32_t* words_out,
                                  int64_t words_capacity, uint32_t* chunk_offsets, uint64_t* total_words, qd_stream_t stream) {
