@@ -157,6 +157,8 @@ int qd_index_histogram(const uint8_t* idx_u8, int64_t n, int num_bins, int64_t* 
  * accounts for: helpers/functions.py:216-262).  bits in {1, 2, 4, 8}; code i of element e sits in
  * byte e*bits/8 at bit offset (e*bits)%8 (little endian).  packed has ceil(n*bits/8) bytes. */
 int qd_pack_indices(const uint8_t* idx_u8, uint8_t* packed, int64_t n, int bits, qd_stream_t stream);
+/* the inverse: idx_u8[e] = code of element e (any alignment of either pointer) */
+int qd_unpack_indices(const uint8_t* packed, int bits, uint8_t* idx_u8, int64_t n, qd_stream_t stream);
 /* q[n] rebuilt from packed uniform levels and the per-row (alpha, beta): bit-identical to the
  * output of qd_uniform_fwd that produced the levels. */
 int qd_unpack_dequant_uniform(const uint8_t* packed, int bits, const float* alpha, const float* beta, float* q,
@@ -282,6 +284,27 @@ int qd_huffman_decode_dequant_model(const qd_huffman_tensor* tensors /* HOST arr
                                     const qd_huffman_table* table, int64_t bucket,
                                     int levels /* uniform: s in [2,256]; 0: non-uniform */,
                                     void* workspace, size_t workspace_bytes, qd_stream_t stream);
+
+/* Transcoding, Huffman stream -> fixed-width codes, a whole model in one launch: every tensor's symbols are decoded
+ * with the model-wide table and written to `packed` at the tensor's own width, byte-identical to qd_pack_indices of
+ * the decoded levels (the high bits of the last byte included).  A symbol >= the tensor's limit is counted into
+ * out_of_range[t] (device int64[count], zeroed by the caller); that tensor's bytes are then unspecified.  Same
+ * protocol as qd_huffman_decode_dequant_model: the host array is validated, then copied into `workspace` (device,
+ * 16-byte aligned, >= qd_huffman_repack_model_workspace_bytes(count) bytes, else QD_ERR_WORKSPACE) with a
+ * stream-ordered copy; the call neither allocates nor synchronises. */
+typedef struct {                 /* one quantized tensor; every pointer is DEVICE memory */
+    const uint32_t* words;       /* may be NULL when num_words == 0 (single-symbol code) */
+    const uint32_t* chunk_offsets;
+    uint8_t* packed;             /* out: ceil(n*bits/8) bytes, the qd_pack_indices layout */
+    int64_t num_words;
+    int64_t n;                   /* >= 1 */
+    int32_t bits;                /* 1, 2, 4 or 8 */
+    int32_t limit;               /* every symbol must be < limit: uniform s, non-uniform K_t; 1 <= limit <= 2^bits */
+} qd_huffman_repack_tensor;
+size_t qd_huffman_repack_model_workspace_bytes(int count);
+int qd_huffman_decode_packed_model(const qd_huffman_repack_tensor* tensors /* HOST array */, int count,
+                                   const qd_huffman_table* table, int64_t* out_of_range, void* workspace,
+                                   size_t workspace_bytes, qd_stream_t stream);
 
 /* ---- next row f1: one launch over every parameter tensor of a model ------
  * (replaces the per-tensor loop of cnn_models/conv_forward_model.py:236-247).

@@ -43,6 +43,7 @@ SIGNATURES = {
     "qd_centroid_index": (C.c_int, [_p, _p, _i32, _i32, _p, _p, _p, _i64, _p]),
     "qd_index_histogram": (C.c_int, [_p, _i64, _i32, _p, _p]),
     "qd_pack_indices": (C.c_int, [_p, _p, _i64, _i32, _p]),
+    "qd_unpack_indices": (C.c_int, [_p, _i32, _p, _i64, _p]),
     "qd_unpack_dequant_uniform": (C.c_int, [_p, _i32, _p, _p, _p, _i64, _i64, _i32, _p]),
     "qd_unpack_dequant_nonuniform": (C.c_int, [_p, _i32, _p, _i32, _p, _p, _p, _i64, _i64, _p]),
     "qd_packed_workspace_bytes": (_sz, [_i64, _i64]),
@@ -58,6 +59,8 @@ SIGNATURES = {
     "qd_huffman_decode_dequant_nonuniform": (C.c_int, [_p, _i64, _p, _p, _p, _i32, _p, _p, _p, _i64, _i64, _p]),
     "qd_huffman_model_workspace_bytes": (_sz, [_i32]),
     "qd_huffman_decode_dequant_model": (C.c_int, [_p, _i32, _p, _i64, _i32, _p, _sz, _p]),
+    "qd_huffman_repack_model_workspace_bytes": (_sz, [_i32]),
+    "qd_huffman_decode_packed_model": (C.c_int, [_p, _i32, _p, _p, _p, _sz, _p]),
     "qd_plan_create": (C.c_int, [C.POINTER(_p), _i32, _p, _p, _p, _p, _i64]),
     "qd_plan_destroy": (C.c_int, [_p]),
     "qd_plan_set_shadow": (C.c_int, [_p, _p]),

@@ -147,6 +147,10 @@ assert _MODEL_TENSOR.itemsize == 72
 _PACKED_TENSOR = np.dtype([("packed", "<u8"), ("alpha", "<u8"), ("beta", "<u8"), ("points", "<u8"), ("q", "<u8"), ("n", "<i8"),
                            ("bits", "<i4"), ("num_points", "<i4")])
 assert _PACKED_TENSOR.itemsize == 56
+# qd_huffman_repack_tensor (include/qd_b200.h): one entry of the whole-model Huffman -> fixed-width transcode
+_REPACK_TENSOR = np.dtype([("words", "<u8"), ("chunk_offsets", "<u8"), ("packed", "<u8"), ("num_words", "<i8"), ("n", "<i8"),
+                           ("bits", "<i4"), ("limit", "<i4")])
+assert _REPACK_TENSOR.itemsize == 48
 
 
 def huffman_code_lengths(counts) -> dict:
@@ -804,7 +808,6 @@ def compress_model(model, numBits=None, bucket_size=256, quantize_first_and_last
     that decompress_ into a freshly built network gives back the whole eval-mode model."""
     named, quantized, s, buffers, dev = _quantization_plan(model, numBits, quantize_first_and_last_layer, points, rule, include_buffers)
     sp = N.stream_ptr(dev)
-    counts = torch.zeros(len(quantized), 256, dtype=torch.int64, device=dev)
     tensors, idxs = [], []
     with torch.cuda.device(dev):
         for i, (name, p) in enumerate(named):
@@ -813,34 +816,50 @@ def compress_model(model, numBits=None, bucket_size=256, quantize_first_and_last
                 continue
             pts = None if s is not None else _points(quantized[i], dev)
             idx, alpha, beta = _levels(_flat(p, dev), s, pts, bucket_size, rule, sp)
-            N.check(N.lib().qd_index_histogram(N.ptr(idx), idx.numel(), 256 if s is None else s, N.ptr(counts[len(idxs)]), sp))
             idxs.append(idx)
             tensors.append(HuffmanTensor(name, tuple(p.shape), alpha=alpha, beta=beta, points=pts))
-        lengths = huffman_code_lengths(counts.sum(0).cpu().numpy())
-        cm = CompressedModel("uniform" if s is not None else "nonuniform", s, bucket_size, lengths, tensors, buffers=buffers)
-        table = cm.table(dev)
-        len_vec = torch.zeros(256, dtype=torch.int64)
-        for sym, l in lengths.items():
-            len_vec[sym] = l
-        code_bits = (counts.cpu() * len_vec).sum(1).tolist()
-        quantized = [t for t in tensors if t.quantized]
-        totals, bufs = torch.zeros(len(idxs), dtype=torch.int64, device=dev), []
-        for k, (t, idx) in enumerate(zip(quantized, idxs)):
-            n = idx.numel()
-            chunks = -(-n // HUFFMAN_CHUNK)
-            capacity = -(-int(code_bits[k]) // 32) + chunks
-            if capacity - chunks > 1 << 32:
-                raise ValueError(f"{t.name}: its Huffman stream would exceed 2^32 words")
-            capacity = min(capacity, 1 << 32)
-            words = torch.empty(max(capacity, 1), dtype=torch.int32, device=dev)
-            offs = torch.empty(chunks, dtype=torch.int32, device=dev)
-            N.check(N.lib().qd_huffman_encode(N.ptr(idx), n, N.ptr(table), N.ptr(words), capacity, N.ptr(offs), N.ptr(totals[k:k + 1]), sp))
-            t.chunk_offsets, t.code_bits = offs, int(code_bits[k])
-            bufs.append((words, capacity))
-        for (t, (words, capacity)), total in zip(zip(quantized, bufs), totals.cpu().tolist()):
-            if total > capacity:
-                raise ValueError(f"{t.name}: its Huffman stream would exceed 2^32 words")
-            t.words = words[:total]
+        return _huffman_coded("uniform" if s is not None else "nonuniform", s, bucket_size, tensors, idxs,
+                              [256 if s is None else s] * len(idxs), buffers, dev)
+
+
+def _huffman_coded(kind, levels, bucket_size, tensors, idxs, bins, buffers, dev) -> CompressedModel:
+    """What compress_model and compress_packed run once every quantized tensor of ``tensors`` (HuffmanTensor, in order)
+    has its uint8 level indices in ``idxs`` on ``dev`` (the current device): one level histogram over all of them
+    gives the code, then each stream is encoded into a capacity bounded by its code bits and trimmed to its length.
+    ``bins``: each tensor's number of levels; a tensor with an index >= its bins raises ValueError naming it."""
+    sp = N.stream_ptr(dev)
+    counts = torch.zeros(len(idxs), 256, dtype=torch.int64, device=dev)
+    for k, (idx, b) in enumerate(zip(idxs, bins)):
+        N.check(N.lib().qd_index_histogram(N.ptr(idx), idx.numel(), b, N.ptr(counts[k]), sp))
+    counts = counts.cpu()
+    quantized = [t for t in tensors if t.quantized]
+    for t, idx, b, seen in zip(quantized, idxs, bins, counts.sum(1).tolist()):
+        if seen != idx.numel():
+            raise ValueError(f"{t.name}: {idx.numel() - seen} codes are not among its {b} levels")
+    lengths = huffman_code_lengths(counts.sum(0).numpy())
+    cm = CompressedModel(kind, levels, bucket_size, lengths, tensors, buffers=buffers)
+    table = cm.table(dev)
+    len_vec = torch.zeros(256, dtype=torch.int64)
+    for sym, l in lengths.items():
+        len_vec[sym] = l
+    code_bits = (counts * len_vec).sum(1).tolist()
+    totals, bufs = torch.zeros(len(idxs), dtype=torch.int64, device=dev), []
+    for k, (t, idx) in enumerate(zip(quantized, idxs)):
+        n = idx.numel()
+        chunks = -(-n // HUFFMAN_CHUNK)
+        capacity = -(-int(code_bits[k]) // 32) + chunks
+        if capacity - chunks > 1 << 32:
+            raise ValueError(f"{t.name}: its Huffman stream would exceed 2^32 words")
+        capacity = min(capacity, 1 << 32)
+        words = torch.empty(max(capacity, 1), dtype=torch.int32, device=dev)
+        offs = torch.empty(chunks, dtype=torch.int32, device=dev)
+        N.check(N.lib().qd_huffman_encode(N.ptr(idx), n, N.ptr(table), N.ptr(words), capacity, N.ptr(offs), N.ptr(totals[k:k + 1]), sp))
+        t.chunk_offsets, t.code_bits = offs, int(code_bits[k])
+        bufs.append((words, capacity))
+    for (t, (words, capacity)), total in zip(zip(quantized, bufs), totals.cpu().tolist()):
+        if total > capacity:
+            raise ValueError(f"{t.name}: its Huffman stream would exceed 2^32 words")
+        t.words = words[:total]
     return cm
 
 
@@ -1211,6 +1230,104 @@ def load_packed(path, device=None) -> PackedModel:
     device.  Every section is a view into one tensor holding the file's data region.  device=None keeps it in host
     memory (unpack_ moves it to the GPU in one copy); a device gets it in one copy here."""
     return _read_container(PackedModel, path, device)
+
+
+def _transcode_limits(m) -> list:
+    """Host-side checks of a model about to change container (pack_compressed, compress_packed), before any device
+    work: [(quantized entry, number of levels it may use: uniform s, non-uniform K_t)]; ValueError otherwise."""
+    if m.kind not in ("uniform", "nonuniform"):
+        raise ValueError(f"unknown kind {m.kind!r}")
+    if m.kind == "uniform" and not (isinstance(m.levels, int) and 2 <= m.levels <= 256):
+        raise ValueError("uniform levels must be in [2, 256]")
+    q = [t for t in m.tensors if t.quantized]
+    if not q:
+        raise ValueError(f"the {m._WHAT} has no quantized tensor")
+    out = []
+    for t in q:
+        limit = int(m.levels) if m.kind == "uniform" else (0 if t.points is None else t.points.numel())
+        if not 1 <= limit <= 256:
+            raise ValueError(f"{t.name}: {limit} points, expected 1 to 256")
+        out.append((t, limit))
+    return out
+
+
+def _own_points(limits, dev) -> list:
+    """Every non-uniform entry's points on ``dev`` in one upload, in new storage; None for a uniform model."""
+    pts = [t.points for t, _ in limits if t.points is not None]
+    if not pts:
+        return [None] * len(limits)
+    flat = torch.cat([p.reshape(-1).to(pts[0].device, torch.float32) for p in pts]).to(dev)
+    return list(flat.split([p.numel() for p in pts]))
+
+
+def pack_compressed(cm: CompressedModel, device=None) -> PackedModel:
+    """The fixed-width model holding exactly what the Huffman-coded ``cm`` holds: same kind, levels, bucket, names,
+    shapes, points, (alpha, beta), unquantized tensors and buffers, each tensor's codes at pack_model's width
+    (bits_for(levels), or bits_for(K_t) for tensor t of a non-uniform model).  Every stream is decoded straight to
+    packed codes in one launch (qd_huffman_decode_packed_model); nothing is re-quantized, so unpack_ of the result
+    writes the parameters decompress_ of ``cm`` writes, bit for bit.  A host-loaded file reaches the device in one
+    copy of its data region; the result shares no storage with ``cm``.  One synchronise reads the count of
+    out-of-range symbols: a stream that emits a symbol >= s or >= K_t raises ValueError naming its tensor.  Runs
+    attach_packed_ on a Huffman-coded file: attach_packed_(pack_compressed(load_compressed(path, "cuda")), net)."""
+    limits = _transcode_limits(cm)
+    for t, _ in limits:
+        if t.chunk_offsets.numel() != -(-t.numel // HUFFMAN_CHUNK):
+            raise ValueError(f"{t.name}: {t.chunk_offsets.numel()} chunk offsets for {t.numel} symbols")
+    dev = _device_of(cm, device)
+    with torch.cuda.device(dev):
+        move = _mover(cm, dev)
+        points = iter(_own_points(limits, dev))
+        tensors, desc, keep = [], np.zeros(len(limits), _REPACK_TENSOR), []
+        for t in cm.tensors:
+            if not t.quantized:
+                tensors.append(PackedEntry(t.name, tuple(t.shape), raw=move(t.raw).clone()))
+                continue
+            k = len(keep) // 2
+            limit = limits[k][1]
+            bits = bits_for(limit)
+            words, offs = move(t.words).contiguous(), move(t.chunk_offsets).contiguous()
+            packed = torch.empty((t.numel * bits + 7) // 8, dtype=torch.uint8, device=dev)
+            desc[k] = (N.ptr(words) if words.numel() else 0, N.ptr(offs), N.ptr(packed), words.numel(), t.numel, bits, limit)
+            keep += [words, offs]
+            tensors.append(PackedEntry(t.name, tuple(t.shape), bits=bits, packed=packed, alpha=move(t.alpha).clone(),
+                                       beta=move(t.beta).clone(), points=next(points)))
+        buffers = None if cm.buffers is None else [(name, move(b).clone()) for name, b in cm.buffers]
+        ws = torch.empty(int(N.lib().qd_huffman_repack_model_workspace_bytes(len(limits))), dtype=torch.uint8, device=dev)
+        bad = torch.zeros(len(limits), dtype=torch.int64, device=dev)
+        N.check(N.lib().qd_huffman_decode_packed_model(desc.ctypes.data, len(limits), N.ptr(cm.table(dev)), N.ptr(bad), N.ptr(ws),
+                                                       ws.numel(), N.stream_ptr(dev)))
+        for (t, limit), count in zip(limits, bad.cpu().tolist()):
+            if count:
+                raise ValueError(f"{t.name}: its Huffman stream emits {count} symbols that are not among its {limit} levels")
+    return PackedModel(cm.kind, cm.levels, cm.bucket_size, tensors, buffers=buffers)
+
+
+def compress_packed(pm: PackedModel, device=None) -> CompressedModel:
+    """The Huffman-coded model holding exactly what the fixed-width ``pm`` holds: every tensor's codes are unpacked to
+    levels (qd_unpack_indices), then compress_model's histogram, code and encoder run on them, so that for a model
+    compress_packed(pack_model(model, ...)) saves to the bytes compress_model(model, ...) saves to.  (alpha, beta),
+    points, unquantized tensors and buffers are carried over.  A code >= s (uniform) or >= K_t (non-uniform tensor t)
+    raises ValueError naming its tensor, as does a code longer than HUFFMAN_MAX_LENGTH bits."""
+    limits = _transcode_limits(pm)
+    for t, limit in limits:
+        if t.bits not in (1, 2, 4, 8) or limit > 1 << t.bits or t.packed.numel() != (t.numel * t.bits + 7) // 8:
+            raise ValueError(f"{t.name}: {t.packed.numel()} bytes of {t.bits}-bit codes cannot hold {t.numel} codes of {limit} levels")
+    dev = _device_of(pm, device)
+    with torch.cuda.device(dev):
+        move, sp = _mover(pm, dev), N.stream_ptr(dev)
+        points = iter(_own_points(limits, dev))
+        tensors, idxs = [], []
+        for t in pm.tensors:
+            if not t.quantized:
+                tensors.append(HuffmanTensor(t.name, tuple(t.shape), raw=move(t.raw).clone()))
+                continue
+            idx = torch.empty(t.numel, dtype=torch.uint8, device=dev)
+            N.check(N.lib().qd_unpack_indices(N.ptr(move(t.packed).contiguous()), t.bits, N.ptr(idx), t.numel, sp))
+            idxs.append(idx)
+            tensors.append(HuffmanTensor(t.name, tuple(t.shape), alpha=move(t.alpha).clone(), beta=move(t.beta).clone(),
+                                         points=next(points)))
+        buffers = None if pm.buffers is None else [(name, move(b).clone()) for name, b in pm.buffers]
+        return _huffman_coded(pm.kind, pm.levels, pm.bucket_size, tensors, idxs, [limit for _, limit in limits], buffers, dev)
 
 
 def get_size_reduction(effective_number_bits, bucket_size=256, full_precision_bits=32):

@@ -51,12 +51,6 @@ extern "C" int qd_index_histogram(const uint8_t* idx_u8, int64_t n, int num_bins
 // one thread-group = 16 consecutive codes in (one 128-bit load), 2*BITS bytes out (one store of that width); BITS is a
 // template parameter so that every shift, mask and access width is a compile-time constant
 template <int BITS>
-__device__ __forceinline__ uint32_t squeeze4(uint32_t w) {  // four codes in four bytes -> 4*BITS bits
-    constexpr unsigned mask = (1u << BITS) - 1u;
-    return (w & mask) | (((w >> 8) & mask) << BITS) | (((w >> 16) & mask) << (2 * BITS)) | (((w >> 24) & mask) << (3 * BITS));
-}
-
-template <int BITS>
 __global__ void __launch_bounds__(256) pack_kernel(const uint8_t* __restrict__ idx, uint8_t* __restrict__ packed, int64_t n) {
     const int64_t groups = (n + 15) / 16;
     const int64_t full = n / 16;   // groups with all sixteen codes present
@@ -150,6 +144,42 @@ __device__ __forceinline__ uint32_t load_codes4_fast(const uint8_t* __restrict__
     else if constexpr (BITS == 4) return __ldcs(reinterpret_cast<const uint16_t*>(packed) + g);
     else if constexpr (BITS == 2) return __ldcs(packed + g);
     else return (uint32_t)__ldcs(packed + (g >> 1)) >> (unsigned)((g & 1) * 4);
+}
+
+// inverse of pack_kernel: one thread-group = 16 consecutive codes, read as four load_codes4 groups, written as one
+// 128-bit store when the output is 16-byte aligned and the group complete, else byte by byte
+template <int BITS>
+__global__ void __launch_bounds__(256) unpack_indices_kernel(const uint8_t* __restrict__ packed, uint8_t* __restrict__ idx, int64_t n) {
+    constexpr uint32_t mask = (1u << BITS) - 1u;
+    const int64_t groups = (n + 15) / 16;
+    const int64_t in_bytes = (n * BITS + 7) / 8;
+    const bool ivec = (reinterpret_cast<uintptr_t>(packed) & 3) == 0;
+    const bool ovec = (reinterpret_cast<uintptr_t>(idx) & 15) == 0;
+    for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += (int64_t)gridDim.x * blockDim.x) {
+        uint32_t w[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const int64_t e0 = g * 16 + u * 4;
+            const uint32_t c = e0 < n ? load_codes4<BITS>(packed, e0, in_bytes, ivec) : 0u;
+            w[u] = (c & mask) | (((c >> BITS) & mask) << 8) | (((c >> (2 * BITS)) & mask) << 16) | (((c >> (3 * BITS)) & mask) << 24);
+        }
+        if (ovec && g * 16 + 16 <= n) {
+            __stcs(reinterpret_cast<uint4*>(idx + g * 16), make_uint4(w[0], w[1], w[2], w[3]));
+        } else {
+            for (int j = 0; j < 16 && g * 16 + j < n; ++j) idx[g * 16 + j] = (uint8_t)(w[j >> 2] >> (8 * (j & 3)));
+        }
+    }
+}
+
+extern "C" int qd_unpack_indices(const uint8_t* packed, int bits, uint8_t* idx_u8, int64_t n, qd_stream_t stream) {
+    if (packed == nullptr || idx_u8 == nullptr || n <= 0) return fail(QD_ERR_INVALID_ARG, "NULL argument or n <= 0");
+    if (!bits_ok(bits)) return fail(QD_ERR_INVALID_ARG, "bits must be 1, 2, 4 or 8");
+    int grid;
+    int rc = capped_grid(((n + 15) / 16 + 255) / 256, 8, &grid);
+    if (rc) return rc;
+    with_bits(bits, [&](auto b) { unpack_indices_kernel<b><<<grid, 256, 0, as_stream(stream)>>>(packed, idx_u8, n); });
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
 }
 
 template <bool UNIFORM>
@@ -308,7 +338,7 @@ __global__ void __launch_bounds__(256, 4) unpack_dequant_model_kernel(const qd_p
 }
 
 // ------------------------------------------------------------------ whole-model launches
-// qd_unpack_dequant_model and qd_huffman_decode_dequant_model read one workspace: the caller's descriptor array, then
+// qd_unpack_dequant_model, qd_huffman_decode_dequant_model and qd_huffman_decode_packed_model read one workspace: the caller's descriptor array, then
 // cta_start[count + 1] (int32); the kernel finds a CTA's tensor with model_tensor_of.
 template <typename Desc>
 static size_t model_workspace_bytes(int count) {
@@ -960,6 +990,35 @@ extern "C" int qd_huffman_decode_dequant_model(const qd_huffman_tensor* tensors,
                                                                                  (float)(levels - 1));
     else
         huff_decode_dequant_model_kernel<false><<<ctas, kHuffDecThreads, 0, st>>>(dev_tensors, dev_start, count, table, bucket, 0.f);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+static_assert(sizeof(qd_huffman_repack_tensor) == 48, "qd_huffman_repack_tensor layout is shared with codec.py");
+
+extern "C" size_t qd_huffman_repack_model_workspace_bytes(int count) { return model_workspace_bytes<qd_huffman_repack_tensor>(count); }
+
+extern "C" int qd_huffman_decode_packed_model(const qd_huffman_repack_tensor* tensors, int count, const qd_huffman_table* table,
+                                              int64_t* out_of_range, void* workspace, size_t workspace_bytes, qd_stream_t stream) {
+    if (tensors == nullptr || count < 1 || table == nullptr || out_of_range == nullptr)
+        return fail(QD_ERR_INVALID_ARG, "NULL tensors / table / out_of_range or count < 1");
+    auto ctas_of = [&](int i, const qd_huffman_repack_tensor& t, int64_t* ctas) {
+        if (t.chunk_offsets == nullptr || t.packed == nullptr) return fail(QD_ERR_INVALID_ARG, "tensor %d: NULL argument", i);
+        if (t.num_words < 0 || (t.num_words > 0 && t.words == nullptr)) return fail(QD_ERR_INVALID_ARG, "tensor %d: bad words / num_words", i);
+        if (t.n < 1) return fail(QD_ERR_INVALID_ARG, "tensor %d: n must be >= 1", i);
+        if (!bits_ok(t.bits)) return fail(QD_ERR_INVALID_ARG, "tensor %d: bits must be 1, 2, 4 or 8", i);
+        if (t.limit < 1 || t.limit > (1 << t.bits)) return fail(QD_ERR_INVALID_ARG, "tensor %d: limit must be in [1, 2^bits]", i);
+        *ctas = ((t.n + kHuffChunk - 1) / kHuffChunk + kHuffDecThreads - 1) / kHuffDecThreads;
+        return (int)QD_OK;
+    };
+    cudaStream_t st = as_stream(stream);
+    unsigned ctas;
+    const int32_t* dev_start;
+    if (const int rc = upload_model(tensors, count, workspace, workspace_bytes, st, ctas_of, "blocks", kHuffDecThreads, "chunks",
+                                    &ctas, &dev_start))
+        return rc;
+    huff_decode_packed_model_kernel<<<ctas, kHuffDecThreads, 0, st>>>(static_cast<const qd_huffman_repack_tensor*>(workspace), dev_start,
+                                                                      count, table, reinterpret_cast<unsigned long long*>(out_of_range));
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }

@@ -179,6 +179,14 @@ inline int geometry_of(int64_t n, int64_t bucket, Geometry* g) {
     return QD_OK;
 }
 
+// ---------------------------------------------------------------- fixed-width codes
+// four codes in four bytes -> 4*BITS bits, low code first (the qd_pack_indices layout)
+template <int BITS>
+__device__ __forceinline__ uint32_t squeeze4(uint32_t w) {
+    constexpr unsigned mask = (1u << BITS) - 1u;
+    return (w & mask) | (((w >> 8) & mask) << BITS) | (((w >> 16) & mask) << (2 * BITS)) | (((w >> 24) & mask) << (3 * BITS));
+}
+
 // Whole-model launches: tensor t owns CTAs [cta_start[t], cta_start[t + 1]) of one grid.  The tensor of CTA b, found by
 // binary search over cta_start[0..count].
 __device__ __forceinline__ int model_tensor_of(const int32_t* __restrict__ cta_start, int count, int b) {

@@ -1,5 +1,6 @@
 // qd_huffman.cuh -- Huffman-coded model storage: encoder (uint8 levels -> canonical-code bit stream) and
-// decoder fused with the dequantization (bit stream -> float32 q).
+// decoder fused with the dequantization (bit stream -> float32 q) or with the fixed-width packing (bit stream ->
+// 1/2/4/8-bit codes).
 //
 // Stream format (include/qd_b200.h, codec.py): every tensor's symbols are cut into chunks of QD_HUFFMAN_CHUNK;
 // each chunk's codes are written MSB-first into 32-bit words starting on a fresh word, chunk_offsets[c] is the
@@ -153,12 +154,13 @@ __global__ void __launch_bounds__(kHuffEncWarps * 32) huff_encode_kernel(const u
     }
 }
 
-// ---- decoder fused with dequantization --------------------------------------------------------------------------
+// ---- decoder fused with dequantization, or with packing ---------------------------------------------------------
 // One thread decodes one chunk sequentially from a 64-bit bit buffer (refilled a word at a time, >= 33 valid bits
 // after a refill): the next 11 bits index a lookup table in shared memory; a miss (code longer than 11 bits) walks
 // the canonical per-length ranges.  After every 32 symbols the CTA's decoded codes (staged in shared memory as
-// bytes) are dequantized with the same unit table and (unit*alpha)+beta arithmetic as unpack_dequant_kernel and
-// leave as 128-bit stores: 8 threads write one chunk's 128 contiguous bytes.
+// bytes) are either dequantized with the same unit table and (unit*alpha)+beta arithmetic as unpack_dequant_kernel and
+// leave as 128-bit stores (8 threads write one chunk's 128 contiguous bytes), or packed into the fixed-width layout
+// of qd_pack_indices.
 struct HuffDecodeShared {
     uint32_t lut[1 << kHuffLutBits];
     unsigned long long first[64];
@@ -208,16 +210,16 @@ __device__ __forceinline__ uint32_t huff_decode_one(const HuffDecodeShared& s, i
     return sym;
 }
 
-// the code (model-wide) and the unit table (per tensor: level / S, or the tensor's points) into shared memory; the
-// caller synchronises the CTA before decoding
-template <bool UNIFORM>
+// the code (model-wide) and, with UNIT, the unit table (per tensor: level / S, or the tensor's points) into shared
+// memory; the caller synchronises the CTA before decoding
+template <bool UNIFORM, bool UNIT = true>
 __device__ __forceinline__ void huff_load_tables(HuffDecodeShared& s, const qd_huffman_table* __restrict__ tab, float S,
                                                  const float* __restrict__ points, int K) {
     for (int i = threadIdx.x; i < (1 << kHuffLutBits); i += blockDim.x) s.lut[i] = tab->lut[i];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) {
         s.symbols[i] = tab->symbols[i];
-        if (UNIFORM) s.unit[i] = ((float)i <= S) ? level_to_unit((float)i, S) : 0.f;
-        else s.unit[i] = (i < K) ? points[i] : 0.f;
+        if (UNIT && UNIFORM) s.unit[i] = ((float)i <= S) ? level_to_unit((float)i, S) : 0.f;
+        else if (UNIT) s.unit[i] = (i < K) ? points[i] : 0.f;
     }
     for (int i = threadIdx.x; i < 64; i += blockDim.x) {
         s.first[i] = tab->first[i];
@@ -226,13 +228,54 @@ __device__ __forceinline__ void huff_load_tables(HuffDecodeShared& s, const qd_h
     }
 }
 
+// Output of the packing decode: one tensor's codes in the qd_pack_indices layout at `bits` per code.
+struct HuffPackOut {
+    uint8_t* packed;
+    int64_t bytes;       // ceil(n * bits / 8)
+    uint32_t limit;      // symbols >= limit are counted into `bad`
+    int bits;
+    uint32_t bad;
+};
+
+// Store stage of the packing decode, after one round: chunk c0 + cl's kHuffDecRound codes are 4*BITS bytes at byte
+// (c0 + cl) * 128*BITS + r*BITS/8 (a chunk fills 128*BITS bytes, so chunks never share a byte).  Thread i writes
+// 32-bit word i % BITS of chunk i / BITS: consecutive threads write consecutive words of a chunk's piece.  Codes past n
+// are staged as 0, so the last byte's high bits are 0, and no byte past the tensor is written.  Every staged symbol
+// >= limit is added to o.bad.
+template <int BITS>
+__device__ __forceinline__ void huff_store_packed(const HuffDecodeShared& s, HuffPackOut& o, int64_t c0, int r) {
+    constexpr int per = 8 / BITS;                 // staged words (four codes each) per output word (32 / BITS codes)
+    const bool vec = (reinterpret_cast<uintptr_t>(o.packed) & 3) == 0;
+    for (int i = threadIdx.x; i < kHuffDecThreads * BITS; i += kHuffDecThreads) {
+        const int cl = i / BITS, part = i % BITS;
+        const int64_t b = (c0 + cl) * (kHuffChunk / 8 * BITS) + (r / kHuffDecRound) * (kHuffDecRound / 8 * BITS) + part * 4;
+        if (b >= o.bytes) continue;
+        uint32_t w = 0u;
+#pragma unroll
+        for (int j = 0; j < per; ++j) {
+            const uint32_t codes = s.stage[cl * kHuffStageStride + part * per + j];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) o.bad += ((codes >> (8 * k)) & 0xffu) >= o.limit;
+            w |= (BITS == 8 ? codes : squeeze4<BITS>(codes)) << (4 * BITS * j);
+        }
+        if (vec && b + 4 <= o.bytes) {
+            __stcs(reinterpret_cast<uint32_t*>(o.packed + b), w);
+        } else {
+            for (int k = 0; k < 4 && b + k < o.bytes; ++k) o.packed[b + k] = (uint8_t)(w >> (8 * k));
+        }
+    }
+}
+
 // Decodes chunks [c0, c0 + kHuffDecThreads) of one tensor (c0 < chunks), one chunk per thread.  Every thread of the
-// CTA calls it with the same arguments (the staging rounds synchronise the CTA).
+// CTA calls it with the same arguments (the staging rounds synchronise the CTA).  The decode loop is shared; the store
+// stage that follows every round is chosen at compile time: PACK = false dequantizes into q (alpha, beta, L,
+// single_row; pk is NULL), PACK = true writes the codes to *pk and counts out-of-range symbols into pk->bad.
+template <bool PACK>
 __device__ __forceinline__ void huff_decode_chunks(HuffDecodeShared& s, int max_len, const uint32_t* __restrict__ words,
                                                    int64_t num_words, const uint32_t* __restrict__ offs,
                                                    const float* __restrict__ alpha, const float* __restrict__ beta,
                                                    float* __restrict__ q, int64_t n, int64_t L, bool single_row, int64_t chunks,
-                                                   int64_t c0) {
+                                                   int64_t c0, HuffPackOut* pk) {
     const bool qvec = (reinterpret_cast<uintptr_t>(q) & 15) == 0;
     const int64_t c = c0 + threadIdx.x;
     const int64_t e0 = c * kHuffChunk;
@@ -256,21 +299,30 @@ __device__ __forceinline__ void huff_decode_chunks(HuffDecodeShared& s, int max_
             s.stage[threadIdx.x * kHuffStageStride + g] = acc;
         }
         __syncthreads();
+        if constexpr (PACK) {
+            switch (pk->bits) {
+                case 8: huff_store_packed<8>(s, *pk, c0, r); break;
+                case 4: huff_store_packed<4>(s, *pk, c0, r); break;
+                case 2: huff_store_packed<2>(s, *pk, c0, r); break;
+                default: huff_store_packed<1>(s, *pk, c0, r); break;
+            }
+        } else {
 #pragma unroll 2
-        for (int i = threadIdx.x; i < kHuffDecThreads * (kHuffDecRound / 4); i += kHuffDecThreads) {
-            const int cl = i / (kHuffDecRound / 4), part = i % (kHuffDecRound / 4);
-            const int64_t e = (c0 + cl) * kHuffChunk + r + part * 4;
-            if (c0 + cl >= chunks || e >= n || r + part * 4 >= kHuffChunk) continue;
-            const uint32_t codes = s.stage[cl * kHuffStageStride + part];
-            if (qvec && e + 4 <= n && (single_row || L % 4 == 0)) {
-                const int64_t row = single_row ? 0 : e / L;
-                const float a = __ldg(alpha + row), b = __ldg(beta + row);
-                st_stream4(q + e, make_float4(from_unit(s.unit[codes & 0xffu], a, b), from_unit(s.unit[(codes >> 8) & 0xffu], a, b),
-                                              from_unit(s.unit[(codes >> 16) & 0xffu], a, b), from_unit(s.unit[codes >> 24], a, b)));
-            } else {
-                for (int j = 0; j < 4 && e + j < n; ++j) {
-                    const int64_t row = single_row ? 0 : (e + j) / L;
-                    q[e + j] = from_unit(s.unit[(codes >> (8 * j)) & 0xffu], __ldg(alpha + row), __ldg(beta + row));
+            for (int i = threadIdx.x; i < kHuffDecThreads * (kHuffDecRound / 4); i += kHuffDecThreads) {
+                const int cl = i / (kHuffDecRound / 4), part = i % (kHuffDecRound / 4);
+                const int64_t e = (c0 + cl) * kHuffChunk + r + part * 4;
+                if (c0 + cl >= chunks || e >= n || r + part * 4 >= kHuffChunk) continue;
+                const uint32_t codes = s.stage[cl * kHuffStageStride + part];
+                if (qvec && e + 4 <= n && (single_row || L % 4 == 0)) {
+                    const int64_t row = single_row ? 0 : e / L;
+                    const float a = __ldg(alpha + row), b = __ldg(beta + row);
+                    st_stream4(q + e, make_float4(from_unit(s.unit[codes & 0xffu], a, b), from_unit(s.unit[(codes >> 8) & 0xffu], a, b),
+                                                  from_unit(s.unit[(codes >> 16) & 0xffu], a, b), from_unit(s.unit[codes >> 24], a, b)));
+                } else {
+                    for (int j = 0; j < 4 && e + j < n; ++j) {
+                        const int64_t row = single_row ? 0 : (e + j) / L;
+                        q[e + j] = from_unit(s.unit[(codes >> (8 * j)) & 0xffu], __ldg(alpha + row), __ldg(beta + row));
+                    }
                 }
             }
         }
@@ -289,7 +341,8 @@ __global__ void __launch_bounds__(kHuffDecThreads) huff_decode_dequant_kernel(
     const int max_len = (int)tab->max_length;
     __syncthreads();
     for (int64_t c0 = (int64_t)blockIdx.x * kHuffDecThreads; c0 < chunks; c0 += (int64_t)gridDim.x * kHuffDecThreads)
-        huff_decode_chunks(s, max_len, words, num_words, offs, alpha, beta, q, geo.n, geo.row_len, geo.rows == 1, chunks, c0);
+        huff_decode_chunks<false>(s, max_len, words, num_words, offs, alpha, beta, q, geo.n, geo.row_len, geo.rows == 1, chunks, c0,
+                                  nullptr);
 }
 
 // A whole model in one launch.  Tensor t owns CTAs [cta_start[t], cta_start[t + 1]), ceil(chunks_t / kHuffDecThreads)
@@ -310,8 +363,29 @@ __global__ void __launch_bounds__(kHuffDecThreads, 10) huff_decode_dequant_model
     const int64_t n = t.n;
     const int64_t L = (bucket == 0 || n < bucket) ? n : bucket;   // geometry_of; one row exactly when L == n
     const int64_t chunks = (n + kHuffChunk - 1) / kHuffChunk;
-    huff_decode_chunks(s, max_len, t.words, t.num_words, t.chunk_offsets, t.alpha, t.beta, t.q, n, L, L == n, chunks,
-                       (int64_t)(b - __ldg(cta_start + lo)) * kHuffDecThreads);
+    huff_decode_chunks<false>(s, max_len, t.words, t.num_words, t.chunk_offsets, t.alpha, t.beta, t.q, n, L, L == n, chunks,
+                              (int64_t)(b - __ldg(cta_start + lo)) * kHuffDecThreads, nullptr);
+}
+
+// A whole model's streams to fixed-width codes in one launch: the CTA map of huff_decode_dequant_model_kernel, no
+// unit table, and the packing store stage at the tensor's own width.  A CTA that staged symbols >= the tensor's limit
+// adds their count to out_of_range[t].
+__global__ void __launch_bounds__(kHuffDecThreads, 10) huff_decode_packed_model_kernel(
+    const qd_huffman_repack_tensor* __restrict__ tensors, const int32_t* __restrict__ cta_start, int count,
+    const qd_huffman_table* __restrict__ tab, unsigned long long* __restrict__ out_of_range) {
+    __shared__ HuffDecodeShared s;
+    const int b = (int)blockIdx.x;
+    const int lo = model_tensor_of(cta_start, count, b);
+    const qd_huffman_repack_tensor& t = tensors[lo];
+    huff_load_tables<true, false>(s, tab, 0.f, nullptr, 0);
+    const int max_len = (int)tab->max_length;
+    __syncthreads();
+    const int64_t n = t.n;
+    const int64_t chunks = (n + kHuffChunk - 1) / kHuffChunk;
+    HuffPackOut pk{t.packed, (n * t.bits + 7) / 8, (uint32_t)t.limit, t.bits, 0u};
+    huff_decode_chunks<true>(s, max_len, t.words, t.num_words, t.chunk_offsets, nullptr, nullptr, nullptr, n, n, true, chunks,
+                             (int64_t)(b - __ldg(cta_start + lo)) * kHuffDecThreads, &pk);
+    if (pk.bad) atomicAdd(out_of_range + lo, (unsigned long long)pk.bad);
 }
 
 }  // namespace qd
