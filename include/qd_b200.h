@@ -351,6 +351,15 @@ int qd_plan_nonuniform_destroy(qd_nu_plan* plan);
 int qd_plan_nonuniform_fwd(const qd_nu_plan* plan, qd_stream_t stream);
 /* grad[i]: dLoss/d(quantized tensor i), float[n[i]] */
 int qd_plan_nonuniform_bwd(const qd_nu_plan* plan, const float* const* grad, qd_stream_t stream);
+/* The same backward split in two for data-parallel training, where the centroid gradient of the global
+ * batch is the rank average of the per-rank ones.  _partial runs the same launches and writes each tensor's
+ * float64 sum into sums, a caller-owned device table double[count][32] (zeros past num_points[i]) instead
+ * of casting it; the caller may reduce that table across ranks.  _finish writes
+ * grad_points[i][k] = (float)(sums[i][k] * scale).  _partial then _finish(scale = 1) equals
+ * qd_plan_nonuniform_bwd bit for bit.  Both are stream-ordered only (no allocation, no synchronisation),
+ * so they can be captured in a CUDA graph. */
+int qd_plan_nonuniform_bwd_partial(const qd_nu_plan* plan, const float* const* grad, double* sums, qd_stream_t stream);
+int qd_plan_nonuniform_bwd_finish(const qd_nu_plan* plan, const double* sums, double scale, qd_stream_t stream);
 
 /* ---- next row f3: the reductions of the differentiable-quantization setup -----------------
  * Exact order statistics without a sort: out[r] = the ranks[r]-th smallest element of v (0-based; ranks

@@ -73,6 +73,8 @@ SIGNATURES = {
     "qd_plan_nonuniform_destroy": (C.c_int, [_p]),
     "qd_plan_nonuniform_fwd": (C.c_int, [_p, _p]),
     "qd_plan_nonuniform_bwd": (C.c_int, [_p, _p, _p]),
+    "qd_plan_nonuniform_bwd_partial": (C.c_int, [_p, _p, _p, _p]),
+    "qd_plan_nonuniform_bwd_finish": (C.c_int, [_p, _p, C.c_double, _p]),
     "qd_order_statistics_workspace_bytes": (_sz, [_i64]),
     "qd_order_statistics": (C.c_int, [_p, _i64, _p, _i32, _p, _p, _sz, _p]),
     "qd_multi_l2norm": (C.c_int, [_p, _p, _i32, _p, _p]),

@@ -17,10 +17,12 @@ swallowed.
 """
 from __future__ import annotations
 
+import contextlib
 import copy
 import time
 
 import torch
+import torch.distributed as dist
 import torch.nn as nn
 import torch.nn.functional as F
 import torch.optim as optim
@@ -438,7 +440,8 @@ def train_model(model, train_loader, test_loader, initial_learning_rate=0.001, u
                     assignBitsAutomatically=True, bucket_size=bucket_size, use_distillation_loss=True,
                     initialize_method="quantiles", quantize_first_and_last_layer=quantize_first_and_last_layer,
                     verbose=verbose, evaluate=evaluate, max_steps=max_steps)[0]
-                model.load_state_dict(quantized_state_dict)
+                inner = _data_parallel_module(model)                       # wrapped: unprefixed keys of the network
+                (model if inner is None else inner).load_state_dict(quantized_state_dict)
                 if fused:
                     quantizer.quantize_weights_model()                     # master <- the loaded weights, live <- quantized
                 losses_epochs.append(last_loss_saved)
@@ -510,6 +513,66 @@ def _capture_point_graphs(quantize_all, point_gradients, device):
         return False
 
 
+def _data_parallel_module(model):
+    """The wrapped network when ``model`` is a :class:`FlatDataParallel` or stock DDP wrapper, else None."""
+    from ..distributed import FlatDataParallel
+    if isinstance(model, (FlatDataParallel, nn.parallel.DistributedDataParallel)):
+        return model.module
+    return None
+
+
+class _RankGroup:
+    """The collectives of the data-parallel differentiable-quantization loop.  Without an initialised
+    process group (a wrapper built in a single process) every call is the identity."""
+
+    def __init__(self, wrapper):
+        self.group = getattr(wrapper, "process_group", None)
+        self.active = dist.is_available() and dist.is_initialized()
+        self.world = dist.get_world_size(self.group) if self.active else 1
+        self.nccl = self.active and dist.get_backend(self.group) == "nccl"
+        self.src = (0 if self.group is None else dist.get_global_rank(self.group, 0)) if self.active else 0
+
+    def average(self, tensors):
+        """Rank average of a list of float32 tensors with ONE all-reduce; returns views of the reduced buffer."""
+        if not self.active:
+            return tensors
+        flat = torch.cat([t.reshape(-1) for t in tensors])
+        dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=self.group)
+        flat.mul_(1.0 / self.world)
+        return [v.view(t.shape) for v, t in zip(flat.split([t.numel() for t in tensors]), tensors)]
+
+    def check_point_counts(self, counts, device):
+        """Raises ValueError on every rank unless all ranks quantize the same tensors with the same point
+        counts (all-reduce MIN of (c, -c): min and max of every count at once)."""
+        if not self.active:
+            return
+        n = torch.tensor([len(counts), -len(counts)], dtype=torch.int64, device=device)
+        dist.all_reduce(n, op=dist.ReduceOp.MIN, group=self.group)
+        lo, hi = n.tolist()
+        if lo != -hi:
+            raise ValueError(f"ranks quantize different numbers of tensors ({lo} to {-hi})")
+        c = torch.tensor([int(k) for k in counts], dtype=torch.int64, device=device)
+        both = torch.cat([c, -c])
+        dist.all_reduce(both, op=dist.ReduceOp.MIN, group=self.group)
+        lo, hi = both[:len(counts)].tolist(), [-v for v in both[len(counts):].tolist()]
+        bad = [i for i, (a, b) in enumerate(zip(lo, hi)) if a != b]
+        if bad:
+            i = bad[0]
+            raise ValueError(f"ranks chose different numbers of points for {len(bad)} tensor(s); tensor {i}: "
+                             f"{lo[i]} to {hi[i]} points")
+
+    def broadcast_buffers(self, model):
+        if self.active:
+            for b in model.buffers():
+                dist.broadcast(b.data, self.src, group=self.group)
+
+    def mean(self, value, device):
+        if not self.active:
+            return value
+        t = torch.tensor([value], dtype=torch.float64, device=device)
+        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
+        return float(t.item()) / self.world
+
 
 def optimize_quantization_points(modelToQuantize, train_loader, test_loader, initial_learning_rate=1e-5,
                                  initial_momentum=0.9, epochs_to_train=30, print_every=500, use_nesterov=True,
@@ -519,7 +582,21 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
                                  step_hook=None, use_cuda_graphs=True, cuda_graph_step=False, use_plan=True):
     """Learn the quantization points of every tensor by SGD on the loss of the
     quantized network, the unquantized network acting as teacher (reference
-    :395-592).  Returns ``(quantizedModel.state_dict(), pointsPerTensor, informationDict)``."""
+    :395-592).  Returns ``(quantizedModel.state_dict(), pointsPerTensor, informationDict)``.
+
+    Data parallel: pass the :class:`FlatDataParallel` or DDP wrapper (one process per GPU, each with its
+    shard of every batch).  The quantized copy is built from the wrapped network and is not wrapped; per
+    step the ranks reduce only the centroid gradients, as float64 sums with ONE all-reduce of a
+    ``(tensors x 32)`` table, and round them to float32 once, so points, quantized weights and the
+    returned (unprefixed) state dict are bit-identical on every rank.  ``assignBitsAutomatically`` uses the
+    rank-averaged gradients; the point counts are checked to agree across ranks (``ValueError`` otherwise).
+    Batch-norm buffers of the quantized copy are broadcast from rank 0 before each evaluation and before
+    returning, and the evaluated accuracy is the mean over ranks.  ``cuda_graph_step=True`` captures the
+    step with its collective on NCCL with ``FlatDataParallel``; stock DDP and gloo run eagerly."""
+    dp_net = _data_parallel_module(modelToQuantize)
+    dp = dp_net is not None
+    ranks = _RankGroup(modelToQuantize) if dp else None
+    net = dp_net if dp else modelToQuantize          # the network itself: teacher and source of the quantized copy
     numTensorsNetwork = sum(1 for _ in modelToQuantize.parameters())
     initialize_method = initialize_method.lower()
     if initialize_method not in ("quantiles", "uniform"):
@@ -536,17 +613,22 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
     if assignBitsAutomatically:                                             # :424-448
         num_to_estimate_grad = 5
         modelToQuantize.zero_grad()
-        for idx_minibatch, batch in enumerate(train_loader, start=1):
-            cnn_hf.forward_and_backward(modelToQuantize, batch, idx_batch=idx_minibatch, epoch=0,
-                                        use_distillation_loss=False, return_tensor=True)
-            if idx_minibatch >= num_to_estimate_grad:
-                break
+        with (modelToQuantize.no_sync() if dp else contextlib.nullcontext()):     # data parallel: accumulate locally
+            for idx_minibatch, batch in enumerate(train_loader, start=1):
+                cnn_hf.forward_and_backward(modelToQuantize, batch, idx_batch=idx_minibatch, epoch=0,
+                                            use_distillation_loss=False, return_tensor=True)
+                if idx_minibatch >= num_to_estimate_grad:
+                    break
         # ||grad / num||_2 of every selected tensor: one multi-tensor launch, one device->host copy
         sel_grads = [p.grad for p in _selected_parameters(modelToQuantize, quantize_first_and_last_layer)]
+        if dp:
+            sel_grads = ranks.average(sel_grads)          # every rank takes the norms of the same averaged gradients
         norms = (quantization.help_functions.gradient_norms(sel_grads) / num_to_estimate_grad).tolist()
         modelToQuantize.zero_grad()
         numPointsPerTensor = quantization.help_functions.assign_bits_automatically(norms, numPointsPerTensor,
                                                                                    input_is_point=True)
+    if dp:
+        ranks.check_point_counts(numPointsPerTensor, device)     # before anything is sized by the counts
 
     selected = _selected_parameters(modelToQuantize, quantize_first_and_last_layer)
     pointsPerTensor = []
@@ -575,7 +657,7 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
         print_every = max(batches_per_epoch // 2, 1)
 
     modelToQuantize.eval()
-    quantizedModel = copy.deepcopy(modelToQuantize)                           # :497-498
+    quantizedModel = copy.deepcopy(net)                                       # :497-498
     q_selected = _selected_parameters(quantizedModel, quantize_first_and_last_layer)
     quantizationFunctions = [quantization.nonUniformQuantization_variable(
         max_element=False, subtract_mean=False, modify_in_place=False, bucket_size=bucket_size,
@@ -591,6 +673,9 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
                                 [pts.data for pts in pointsPerTensor], bucket_size)
         except NotImplementedError:
             plan = None
+    # data parallel: the float64 centroid-gradient sums of every tensor, reduced in place across ranks each step
+    sums = torch.zeros((len(q_selected), CentroidPlan.MAX_POINTS), dtype=torch.float64, device=device) \
+        if (dp and plan is not None) else None
 
     def quantize_all():                                                       # :525-532
         if plan is not None:
@@ -601,7 +686,13 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
 
     def point_gradients():                                                    # :539-545
         if plan is not None:
-            return plan.backward_([p_q.grad.data if p_q.grad.is_contiguous() else p_q.grad.data.contiguous() for p_q in q_selected])
+            q_grads = [p_q.grad.data if p_q.grad.is_contiguous() else p_q.grad.data.contiguous() for p_q in q_selected]
+            if sums is not None:              # global-batch gradient = rank average; rounded to float32 once, after the sum
+                plan.backward_partial_(q_grads, sums)
+                if ranks.active:
+                    dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=ranks.group)
+                return plan.finish_(sums, 1.0 / ranks.world)
+            return plan.backward_(q_grads)
         return [fun.backward(p_q.grad.data)[1] for fun, p_q in zip(quantizationFunctions, q_selected)]
 
     # Without the plan the per-step quantization work is 3 small launches per tensor (22-60 tensors),
@@ -624,13 +715,15 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
         else:
             quantize_all()
         loss = cnn_hf.forward_and_backward(quantizedModel, data, idx_minibatch, epoch,
-                                           use_distillation_loss=use_distillation_loss, teacher_model=modelToQuantize,
+                                           use_distillation_loss=use_distillation_loss, teacher_model=net,
                                            return_tensor=True)
         if graphs:
             graphs[1].replay()
             grads = graphs[2]
         else:
             grads = point_gradients()
+        if dp and plan is None:                   # per-tensor fallback: its float32 gradients, ONE all-reduce (average)
+            grads = ranks.average(grads)
         for pts, gp in zip(pointsPerTensor, grads):
             pts.grad = gp
         optimizer.step()
@@ -639,6 +732,11 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
 
     # whole-step capture (opt-in), same mechanism as train_model(cuda_graph_step=True)
     whole_ok = bool(cuda_graph_step and device.type == "cuda")
+    # data parallel: the collective is captured with the step only on NCCL behind FlatDataParallel (stock DDP and
+    # gloo run eagerly), and the step is replayed only if EVERY rank captured it (the rule of train_model)
+    collective = dp and ranks.active
+    if collective and (not ranks.nccl or isinstance(modelToQuantize, nn.parallel.DistributedDataParallel)):
+        whole_ok = False
     side_stream = torch.cuda.Stream(device) if whole_ok else None
     graphed = None
 
@@ -648,8 +746,13 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
         running = torch.zeros((), device=device)
         for idx_minibatch, data in enumerate(train_loader, start=1):
             if whole_ok and graphed is None and total_steps >= 3:
-                graphed = _GraphedStep(one_step, data, device, side_stream, optimizer)
-                if not graphed.ok:
+                graphed = _GraphedStep(one_step, data, device, side_stream, optimizer, collective=collective)
+                captured = graphed.ok
+                if collective:
+                    flag = torch.tensor([1 if captured else 0], dtype=torch.int32, device=device)
+                    dist.all_reduce(flag, op=dist.ReduceOp.MIN, group=ranks.group)
+                    captured = bool(flag.item())
+                if not captured:
                     whole_ok, graphed = False, None
             if graphed is not None and graphed.matches(data):
                 loss = graphed.run(data)[0]
@@ -674,7 +777,11 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
                 break
         losses_epochs.append(last_loss_saved)
         if evaluate:
-            pred_accuracy_epochs.append(cnn_hf.evaluateModel(quantizedModel, test_loader, fastEvaluation=False))
+            if dp:
+                ranks.broadcast_buffers(quantizedModel)                    # every rank evaluates rank 0's statistics
+            accuracy = cnn_hf.evaluateModel(quantizedModel, test_loader, fastEvaluation=False)
+            # data parallel: one accuracy for all ranks, so that they take the same learning-rate decisions
+            pred_accuracy_epochs.append(ranks.mean(accuracy, device) if dp else accuracy)
             if verbose:
                 print(" === Epoch: {} - prediction accuracy {:2f}% === ".format(epoch + 1, pred_accuracy_epochs[-1] * 100))
         if stop:
@@ -691,5 +798,8 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
                        "lossSaved": losses_epochs, "numStepsTrained": total_steps,
                        "cuda_graph_step": graphed is not None, "cuda_graph_quantization": bool(graphs),
                        "multi_tensor_plan": plan is not None}
+    if dp:
+        informationDict["data_parallel_world"] = ranks.world
+        ranks.broadcast_buffers(quantizedModel)                            # one state dict on every rank
     # the state dict also carries the batch-norm running statistics of the quantized model (:579-592)
     return quantizedModel.state_dict(), pointsPerTensor, informationDict

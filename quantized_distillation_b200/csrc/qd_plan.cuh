@@ -293,18 +293,53 @@ __global__ void __launch_bounds__(kPgThreads) plan_points_grad_partial(const NuE
     }
 }
 
+// Fold of one tensor's gradient blocks, shared by both outputs of the backward.  Lane k < K sums
+// centroid k's block partials in index order; the store stage is picked at compile time:
+//   NU_FOLD_POINTS  grad_points[k] = (float)s                     (the single-process backward)
+//   NU_FOLD_SUMS    sums[t][k] = s, zeros for k >= K              (data parallel: reduced across ranks
+//                                                                  in float64, cast once by the finish)
+enum { NU_FOLD_POINTS = 0, NU_FOLD_SUMS = 1 };
+
+template <int OUT>
+__device__ __forceinline__ void nu_fold_tensor(const NuEntry& en, int t, const double* __restrict__ partial,
+                                               double* __restrict__ sums) {
+    const int lane = threadIdx.x & 31;   // read here, not passed in: keeps plan_points_grad_final's code as it was
+    if (lane < en.K) {
+        double s = 0.0;
+        for (int64_t b = 0; b < en.blocks; ++b) s += partial[(en.blk_start + b) * kNuMaxK + lane];
+        if constexpr (OUT == NU_FOLD_POINTS) en.grad_points[lane] = (float)s;
+        else sums[(int64_t)t * kNuMaxK + lane] = s;
+    } else if constexpr (OUT == NU_FOLD_SUMS) {
+        sums[(int64_t)t * kNuMaxK + lane] = 0.0;
+    }
+}
+
 // one warp per tensor: lane k folds the tensor's blocks in index order
 __global__ void __launch_bounds__(256) plan_points_grad_final(const NuEntry* __restrict__ entries, int count,
                                                               const double* __restrict__ partial) {
+    const int t = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (t >= count) return;
+    const NuEntry en = entries[t];
+    nu_fold_tensor<NU_FOLD_POINTS>(en, t, partial, nullptr);
+}
+
+// the same fold, float64 sums into a caller-owned [count][32] table
+__global__ void __launch_bounds__(256) plan_points_grad_sums(const NuEntry* __restrict__ entries, int count,
+                                                             const double* __restrict__ partial, double* __restrict__ sums) {
+    const int t = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (t >= count) return;
+    const NuEntry en = entries[t];
+    nu_fold_tensor<NU_FOLD_SUMS>(en, t, partial, sums);
+}
+
+// grad_points[t][k] = (float)(sums[t][k] * scale): the one float32 rounding of a reduced table
+__global__ void __launch_bounds__(256) plan_points_grad_finish(const NuEntry* __restrict__ entries, int count,
+                                                               const double* __restrict__ sums, double scale) {
     const int lane = threadIdx.x & 31;
     const int t = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (t >= count) return;
     const NuEntry en = entries[t];
-    if (lane < en.K) {
-        double s = 0.0;
-        for (int64_t b = 0; b < en.blocks; ++b) s += partial[(en.blk_start + b) * kNuMaxK + lane];
-        en.grad_points[lane] = (float)s;
-    }
+    if (lane < en.K) en.grad_points[lane] = (float)(sums[(int64_t)t * kNuMaxK + lane] * scale);
 }
 
 }  // namespace qd

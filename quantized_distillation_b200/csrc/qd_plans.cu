@@ -382,21 +382,48 @@ extern "C" int qd_plan_nonuniform_fwd(const qd_nu_plan* p, qd_stream_t stream) {
     });
 }
 
-extern "C" int qd_plan_nonuniform_bwd(const qd_nu_plan* p, const float* const* grad, qd_stream_t stream) {
-    if (p == nullptr || grad == nullptr) return fail(QD_ERR_INVALID_ARG, "plan or grad is NULL");
+// the gradient blocks of every tensor -> p->partial (first launch of every backward entry point)
+static int nu_grad_partials(const qd_nu_plan* p, const float* const* grad, cudaStream_t s) {
+    if (grad == nullptr) return fail(QD_ERR_INVALID_ARG, "grad is NULL");
     for (int i = 0; i < p->count; ++i)
         if (grad[i] == nullptr) return fail(QD_ERR_INVALID_ARG, "grad[%d] is NULL", i);
     int grid;
     int rc = capped_grid((p->total_blocks + kPgWarps - 1) / kPgWarps, 4, &grid);
     if (rc) return rc;
-    cudaStream_t s = as_stream(stream);
     GradTable gt;
     float* const* dev_grads;
     rc = plan_grads(p, grad, s, &gt, &dev_grads);
     if (rc) return rc;
     plan_points_grad_partial<0><<<grid, kPgThreads, 0, s>>>(p->dev, p->count, p->total_blocks, p->block_tiles, gt, dev_grads, p->partial);
     QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+extern "C" int qd_plan_nonuniform_bwd(const qd_nu_plan* p, const float* const* grad, qd_stream_t stream) {
+    if (p == nullptr) return fail(QD_ERR_INVALID_ARG, "plan is NULL");
+    cudaStream_t s = as_stream(stream);
+    int rc = nu_grad_partials(p, grad, s);
+    if (rc) return rc;
     plan_points_grad_final<<<(p->count + 7) / 8, 256, 0, s>>>(p->dev, p->count, p->partial);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+extern "C" int qd_plan_nonuniform_bwd_partial(const qd_nu_plan* p, const float* const* grad, double* sums, qd_stream_t stream) {
+    if (p == nullptr || sums == nullptr) return fail(QD_ERR_INVALID_ARG, "plan or sums is NULL");
+    if ((reinterpret_cast<uintptr_t>(sums) & 7) != 0) return fail(QD_ERR_INVALID_ARG, "sums must be 8-byte aligned");
+    cudaStream_t s = as_stream(stream);
+    int rc = nu_grad_partials(p, grad, s);
+    if (rc) return rc;
+    plan_points_grad_sums<<<(p->count + 7) / 8, 256, 0, s>>>(p->dev, p->count, p->partial, sums);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+extern "C" int qd_plan_nonuniform_bwd_finish(const qd_nu_plan* p, const double* sums, double scale, qd_stream_t stream) {
+    if (p == nullptr || sums == nullptr) return fail(QD_ERR_INVALID_ARG, "plan or sums is NULL");
+    if ((reinterpret_cast<uintptr_t>(sums) & 7) != 0) return fail(QD_ERR_INVALID_ARG, "sums must be 8-byte aligned");
+    plan_points_grad_finish<<<(p->count + 7) / 8, 256, 0, as_stream(stream)>>>(p->dev, p->count, sums, scale);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }

@@ -22,6 +22,7 @@ fix-up kernels run after it, on the already reduced gradients, like the referenc
 runs them on its single reduced copy (conv_forward_model.py:315)."""
 from __future__ import annotations
 
+import contextlib
 import os
 from collections import OrderedDict
 
@@ -100,6 +101,7 @@ class FlatDataParallel(torch.nn.Module):
             spans.append((off, off + pad(p.numel())))
             off += pad(p.numel())
         self._params = params
+        self._paused = False
         self._nccl = self.world > 1 and dist.get_backend(process_group) == "nccl"
         # buckets: contiguous runs of parameters, in registration order, of >= bucket_mb each
         limit = int(bucket_mb * (1 << 20) / self.flat_grad.element_size())
@@ -123,6 +125,8 @@ class FlatDataParallel(torch.nn.Module):
     # ---- bucketed, overlapped reduction ---------------------------------------------------------
     def _make_hook(self, index):
         def hook(_param):
+            if self._paused:
+                return
             bucket = self._buckets[self._bucket_of[index]]
             bucket["pending"] -= 1
             if bucket["pending"] == 0 and not bucket["sent"]:
@@ -155,6 +159,18 @@ class FlatDataParallel(torch.nn.Module):
         self.flat_grad.zero_()
         for bucket in self._buckets:
             bucket["pending"], bucket["sent"] = len(bucket["members"]), False
+
+    @contextlib.contextmanager
+    def no_sync(self):
+        """Backward passes inside the block accumulate into the flat buffer without any reduction, like
+        DDP's ``no_sync()``; the caller reduces what it needs afterwards.  Every bucket is re-armed on exit."""
+        self._paused = True
+        try:
+            yield
+        finally:
+            self._paused = False
+            for bucket in self._buckets:
+                bucket["pending"], bucket["sent"] = len(bucket["members"]), False
 
     def views_intact(self) -> bool:
         """True while every ``p.grad`` still aliases the flat buffer (an optimizer's

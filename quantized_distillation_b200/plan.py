@@ -187,17 +187,44 @@ class CentroidPlan:
         with torch.cuda.device(self.device):
             N.check(N.lib().qd_plan_nonuniform_fwd(self._handle, N.stream_ptr(self.device)))
 
-    def backward_(self, grads):
-        """Every tensor's dLoss/dpoints from dLoss/d(quantized tensor) (:539-545); returns views of one
-        flat buffer, overwritten by the next call."""
+    def _grad_ptrs(self, grads):
         if len(grads) != len(self.sources):
             raise ValueError("one gradient per tensor expected")
         for g, s in zip(grads, self.sources):
             if not (g.is_cuda and g.dtype == torch.float32 and g.is_contiguous() and g.numel() == s.numel()):
                 raise ValueError("gradients must be contiguous float32 CUDA tensors matching the tensors")
-        gp = (C.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
+        return (C.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
+
+    def _check_sums(self, sums):
+        if not (sums.is_cuda and sums.device == self.device and sums.dtype == torch.float64 and sums.is_contiguous()
+                and tuple(sums.shape) == (len(self.sources), self.MAX_POINTS)):
+            raise ValueError(f"sums must be a contiguous float64 CUDA tensor of shape ({len(self.sources)}, {self.MAX_POINTS}) "
+                             "on the plan's device")
+
+    def backward_(self, grads):
+        """Every tensor's dLoss/dpoints from dLoss/d(quantized tensor) (:539-545); returns views of one
+        flat buffer, overwritten by the next call."""
+        gp = self._grad_ptrs(grads)
         with torch.cuda.device(self.device):
             N.check(N.lib().qd_plan_nonuniform_bwd(self._handle, gp, N.stream_ptr(self.device)))
+        return self.grad_points
+
+    def backward_partial_(self, grads, sums):
+        """``backward_`` up to its last rounding: writes every tensor's float64 centroid-gradient sums into
+        ``sums`` (float64, shape ``(tensors, 32)``, zeros past each tensor's point count) and leaves
+        ``grad_points`` alone.  Data-parallel training reduces ``sums`` across ranks, then calls ``finish_``."""
+        gp = self._grad_ptrs(grads)
+        self._check_sums(sums)
+        with torch.cuda.device(self.device):
+            N.check(N.lib().qd_plan_nonuniform_bwd_partial(self._handle, gp, N.ptr(sums), N.stream_ptr(self.device)))
+        return sums
+
+    def finish_(self, sums, scale=1.0):
+        """``grad_points[t][k] = float32(sums[t][k] * scale)``; returns ``grad_points``.  ``backward_partial_``
+        followed by ``finish_(sums, 1.0)`` gives ``backward_``'s result bit for bit."""
+        self._check_sums(sums)
+        with torch.cuda.device(self.device):
+            N.check(N.lib().qd_plan_nonuniform_bwd_finish(self._handle, N.ptr(sums), float(scale), N.stream_ptr(self.device)))
         return self.grad_points
 
     def close(self):
