@@ -20,6 +20,7 @@ from __future__ import annotations
 import contextlib
 import copy
 import time
+import warnings
 
 import torch
 import torch.distributed as dist
@@ -105,49 +106,175 @@ class ConvolForwardNet(nn.Module):
 
 
 # ------------------------------------------------------------------------------------------
+# data parallelism and CUDA-graph capture of a whole step, shared by both training loops
+# ------------------------------------------------------------------------------------------
+def _data_parallel_module(model):
+    """The wrapped network when ``model`` is a :class:`FlatDataParallel` or stock DDP wrapper, else None."""
+    from ..distributed import FlatDataParallel
+    if isinstance(model, (FlatDataParallel, nn.parallel.DistributedDataParallel)):
+        return model.module
+    return None
+
+
+class _RankGroup:
+    """The collectives of the data-parallel training loops, on the wrapper's process group.  Without an
+    initialised process group (a wrapper built in a single process) every call is the identity."""
+
+    def __init__(self, wrapper):
+        self.group = getattr(wrapper, "process_group", None)
+        self.active = dist.is_available() and dist.is_initialized()
+        self.world = dist.get_world_size(self.group) if self.active else 1
+        self.nccl = self.active and dist.get_backend(self.group) == "nccl"
+        self.src = (0 if self.group is None else dist.get_global_rank(self.group, 0)) if self.active else 0
+
+    def average(self, tensors):
+        """Rank average of a list of float32 tensors with ONE all-reduce; returns views of the reduced buffer."""
+        if not self.active:
+            return tensors
+        flat = torch.cat([t.reshape(-1) for t in tensors])
+        dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=self.group)
+        flat.mul_(1.0 / self.world)
+        return [v.view(t.shape) for v, t in zip(flat.split([t.numel() for t in tensors]), tensors)]
+
+    def check_point_counts(self, counts, device):
+        """Raises ValueError on every rank unless all ranks quantize the same tensors with the same point
+        counts (all-reduce MIN of (c, -c): min and max of every count at once)."""
+        if not self.active:
+            return
+        n = torch.tensor([len(counts), -len(counts)], dtype=torch.int64, device=device)
+        dist.all_reduce(n, op=dist.ReduceOp.MIN, group=self.group)
+        lo, hi = n.tolist()
+        if lo != -hi:
+            raise ValueError(f"ranks quantize different numbers of tensors ({lo} to {-hi})")
+        c = torch.tensor([int(k) for k in counts], dtype=torch.int64, device=device)
+        both = torch.cat([c, -c])
+        dist.all_reduce(both, op=dist.ReduceOp.MIN, group=self.group)
+        lo, hi = both[:len(counts)].tolist(), [-v for v in both[len(counts):].tolist()]
+        bad = [i for i, (a, b) in enumerate(zip(lo, hi)) if a != b]
+        if bad:
+            i = bad[0]
+            raise ValueError(f"ranks chose different numbers of points for {len(bad)} tensor(s); tensor {i}: "
+                             f"{lo[i]} to {hi[i]} points")
+
+    def broadcast_buffers(self, model):
+        if self.active:
+            for b in model.buffers():
+                dist.broadcast(b.data, self.src, group=self.group)
+
+    def mean(self, value, device):
+        if not self.active:
+            return value
+        t = torch.tensor([value], dtype=torch.float64, device=device)
+        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
+        return float(t.item()) / self.world
+
+
+def _step_capturable(model, ranks, device):
+    """The one rule for capturing a whole step in a CUDA graph (``ranks``: None for an unwrapped model).  Not data
+    parallel (no wrapper, or no process group): always.  Data parallel: only on NCCL behind FlatDataParallel,
+    whose collectives are stream-ordered device work; stock DDP (host-side reducer hooks) and gloo run eagerly."""
+    from ..distributed import FlatDataParallel
+    return device.type == "cuda" and (ranks is None or not ranks.active
+                                      or (ranks.nccl and isinstance(model, FlatDataParallel)))
+
+
+def _side_stream(device):
+    """A CUDA stream, and a context that runs work on it after the current stream's work, then makes the
+    current stream wait for it."""
+    stream = torch.cuda.Stream(device)
+
+    @contextlib.contextmanager
+    def on_side():
+        stream.wait_stream(torch.cuda.current_stream(device))
+        with torch.cuda.stream(stream):
+            yield
+        torch.cuda.current_stream(device).wait_stream(stream)
+    return stream, on_side
+
+
+def _capture(fn, device, stream=None, thread_local=False, what="the training step"):
+    """``(graph, fn())`` with ``fn`` captured on ``stream``, or None after a warning when capture fails.  A step
+    that holds an NCCL collective needs ``thread_local``: the NCCL watchdog thread may call CUDA meanwhile."""
+    try:
+        torch.cuda.synchronize(device)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, stream=stream, capture_error_mode="thread_local" if thread_local else "global"):
+            out = fn()
+        return graph, out
+    except Exception as e:                                   # pragma: no cover - depends on driver / torch build
+        warnings.warn(f"CUDA graph capture of {what} failed, running eagerly: {e}")
+        with contextlib.suppress(Exception):
+            torch.cuda.synchronize(device)
+        return None
+
+
+class _CapturedStep:
+    """Runs a loop's ``step(batch, idx_minibatch, epoch) -> (loss, asked, total)``, eagerly or as a CUDA graph.
+
+    Enabled, the first three steps run eagerly on the side stream the capture uses (warm pools and workspaces);
+    the fourth is captured, and every batch of the captured shapes is then copied into static buffers and
+    replayed.  A batch of another shape runs eagerly and the graph is kept.  With a process group every rank
+    must have captured, or all stay eager; after a failed capture the run stays eager.  ``invalidate()`` (the
+    graph holds the learning rate) makes the next step capture again.  ``captured``: every rank agreed once."""
+
+    def __init__(self, step, optimizer, device, enabled, ranks=None, static_grads=False):
+        self.step, self.optimizer, self.device, self.enabled = step, optimizer, device, enabled
+        self.ranks = ranks if ranks is not None and ranks.active else None
+        self.static_grads = static_grads          # FlatDataParallel's gradient views: allocated once, address-stable
+        self.stream, self.on_side = _side_stream(device) if enabled else (None, None)
+        self.steps, self.captured = 0, False
+        self.invalidate()
+
+    def invalidate(self):
+        self.graph = self.x = self.y = self.out = None
+
+    def _try_capture(self, batch):
+        x, y = batch
+        self.x = torch.empty(x.shape, dtype=x.dtype, device=self.device).copy_(x, non_blocking=True)
+        self.y = torch.empty(y.shape, dtype=y.dtype, device=self.device).copy_(y, non_blocking=True)
+        if not self.static_grads:
+            self.optimizer.zero_grad(set_to_none=True)     # gradients are re-created inside the graph's pool
+        got = _capture(lambda: self.step((self.x, self.y), 1, 0), self.device, self.stream,
+                       thread_local=self.ranks is not None)
+        ok = got is not None
+        if self.ranks is not None:                          # a replayed collective needs every peer to replay it
+            flag = torch.tensor([int(ok)], dtype=torch.int32, device=self.device)
+            dist.all_reduce(flag, op=dist.ReduceOp.MIN, group=self.ranks.group)
+            ok = bool(flag.item())
+        if ok:
+            self.graph, self.out = got
+            self.captured = True
+        else:
+            self.invalidate()
+            self.enabled = False
+
+    def run(self, batch, idx_minibatch, epoch):
+        if self.enabled and self.graph is None and self.steps >= 3:
+            self._try_capture(batch)
+        self.steps += 1
+        if self.graph is not None and batch[0].shape == self.x.shape and batch[1].shape == self.y.shape:
+            self.x.copy_(batch[0], non_blocking=True)
+            self.y.copy_(batch[1], non_blocking=True)
+            self.graph.replay()
+            return self.out
+        if not self.enabled:
+            return self.step(batch, idx_minibatch, epoch)
+        with self.on_side():
+            return self.step(batch, idx_minibatch, epoch)
+
+
+def _set_learning_rate(optimizers, lr, runner):
+    """Sets ``lr`` in every parameter group; a change invalidates the captured step, which holds the old rate."""
+    for opt in optimizers:
+        for group in opt.param_groups:
+            if group["lr"] != lr:
+                runner.invalidate()
+            group["lr"] = lr
+
+
+# ------------------------------------------------------------------------------------------
 # quantized distillation
 # ------------------------------------------------------------------------------------------
-class _GraphedStep:
-    """One whole training step captured in a CUDA graph: static input buffers, one replay per step."""
-
-    def __init__(self, step_fn, example_batch, device, stream, optimizer, static_grads=False, collective=False):
-        self.ok = False
-        try:
-            x, y = example_batch
-            self.x = torch.empty(x.shape, dtype=x.dtype, device=device)
-            self.y = torch.empty(y.shape, dtype=y.dtype, device=device)
-            self.x.copy_(x, non_blocking=True)
-            self.y.copy_(y, non_blocking=True)
-            torch.cuda.synchronize(device)
-            if not static_grads:
-                optimizer.zero_grad(set_to_none=True)        # gradients are re-created inside the graph's pool
-            # (static_grads: they are views of FlatDataParallel's flat buffer, allocated once, address-stable)
-            self.graph = torch.cuda.CUDAGraph()
-            # a captured step that holds an NCCL collective: other threads of the process (the NCCL
-            # watchdog) may touch the CUDA API meanwhile, which only thread-local capture tolerates
-            mode = {"capture_error_mode": "thread_local"} if collective else {}
-            with torch.cuda.graph(self.graph, stream=stream, **mode):
-                self.loss, self.asked, self.total = step_fn((self.x, self.y))
-            self.ok = True
-        except Exception as e:                               # pragma: no cover - depends on driver / torch build
-            import warnings
-            warnings.warn(f"CUDA graph capture of the training step failed, running eagerly: {e}")
-            try:
-                torch.cuda.synchronize(device)
-            except Exception:
-                pass
-
-    def matches(self, batch):
-        return batch[0].shape == self.x.shape and batch[1].shape == self.y.shape
-
-    def run(self, batch):
-        self.x.copy_(batch[0], non_blocking=True)
-        self.y.copy_(batch[1], non_blocking=True)
-        self.graph.replay()
-        return self.loss, self.asked, self.total
-
-
-
 def _selected_parameters(model, quantize_first_and_last_layer):
     params = list(model.parameters())
     if quantize_first_and_last_layer is False:
@@ -268,12 +395,12 @@ def train_model(model, train_loader, test_loader, initial_learning_rate=0.001, u
     quantization (reference :165-393; same positional/keyword arguments, the
     keyword-only ones after ``*`` are additions).
 
-    ``cuda_graph_step=True`` (single process, ``ask_teacher_strategy`` 'always',
-    ``estimate_quant_grad_every`` 1): after three eager steps the whole step --
-    save+quantize, student/teacher forward, backward, restore, gradient fix-up,
-    SGD update -- is captured once in a CUDA graph and replayed; each step then
-    costs one H2D copy of the batch and one graph launch.  Same arithmetic, same
-    kernels; the graph is re-captured when the learning rate changes.
+    ``cuda_graph_step=True`` (``ask_teacher_strategy`` 'always', ``estimate_quant_grad_every`` 1, no gradient
+    noise; data parallel only on NCCL behind ``FlatDataParallel``): after three eager steps the whole step --
+    save+quantize, student/teacher forward, backward, all-reduce, restore, gradient fix-up, SGD update -- is
+    captured once in a CUDA graph and replayed (:class:`_CapturedStep`); each step then costs one H2D copy of
+    the batch and one graph launch.  Same arithmetic, same kernels; the graph is re-captured when the learning
+    rate changes.  ``informationDict["cuda_graph_step"]``: every rank captured the step at least once.
 
     ``fused_optimizer_step=True`` (quantized training, bucket of at most 512, no gradient noise /
     clipping): restore, gradient fix-up, the SGD update and the NEXT step's save-and-quantize become
@@ -308,7 +435,6 @@ def train_model(model, train_loader, test_loader, initial_learning_rate=0.001, u
     state = {"since": steps_since_estimate}
     # data parallelism: FlatDataParallel exposes reduce_gradients(); DDP reduces inside backward
     reduce_gradients = getattr(model, "reduce_gradients", None)
-    flat_dp = reduce_gradients is not None
 
     fused = bool(fused_optimizer_step and quantizer is not None and device.type == "cuda" and estimate_quant_grad_every == 1
                  and not add_gradient_noise and grad_clipping_threshold is False
@@ -373,38 +499,17 @@ def train_model(model, train_loader, test_loader, initial_learning_rate=0.001, u
         return loss, c_teach, c_total
 
     strategy_name = (ask_teacher_strategy[0] if isinstance(ask_teacher_strategy, tuple) else ask_teacher_strategy).lower()
-    multi = torch.distributed.is_available() and torch.distributed.is_initialized() and torch.distributed.get_world_size() > 1
-    # stock DDP drives its reducer from autograd hooks on the host and cannot be replayed; the flat
-    # wrapper's single all-reduce can, so a captured step is available for any world size with it
-    graph_ok = bool(cuda_graph_step and device.type == "cuda" and estimate_quant_grad_every == 1 and not add_gradient_noise
-                    and strategy_name == "always" and (not multi or flat_dp))
-    side_stream = torch.cuda.Stream(device) if graph_ok else None
-    graphed = None
+    ranks = _RankGroup(model) if _data_parallel_module(model) is not None else None
+    runner = _CapturedStep(one_step, optimizer, device, static_grads=reduce_gradients is not None, ranks=ranks, enabled=bool(
+        cuda_graph_step and estimate_quant_grad_every == 1 and not add_gradient_noise and strategy_name == "always"
+        and _step_capturable(model, ranks, device)))
     try:
         for epoch in range(start_epoch, epochs_to_train + start_epoch):
             model.train()
             running = torch.zeros((), device=cnn_hf._device_of(model))
             asked, seen = 0, 0
             for idx_minibatch, data in enumerate(train_loader, start=1):
-                if graph_ok and graphed is None and total_steps >= 3:
-                    graphed = _GraphedStep(one_step, data, device, side_stream, optimizer, static_grads=flat_dp,
-                                           collective=flat_dp and multi)
-                    captured = graphed.ok
-                    if multi:                                      # replay a collective only if EVERY rank captured it
-                        flag = torch.tensor([1 if captured else 0], dtype=torch.int32, device=device)
-                        torch.distributed.all_reduce(flag, op=torch.distributed.ReduceOp.MIN)
-                        captured = bool(flag.item())
-                    informationDict["cuda_graph_step"] = captured
-                    if not captured:
-                        graph_ok, graphed = False, None
-                if graphed is not None and graphed.matches(data):
-                    loss, c_teach, c_total = graphed.run(data)
-                elif graph_ok:
-                    with torch.cuda.stream(side_stream):           # warm-up steps run where the capture will
-                        loss, c_teach, c_total = one_step(data, idx_minibatch, epoch)
-                    torch.cuda.current_stream(device).wait_stream(side_stream)
-                else:
-                    loss, c_teach, c_total = one_step(data, idx_minibatch, epoch)
+                loss, c_teach, c_total = runner.run(data, idx_minibatch, epoch)
                 asked += c_teach
                 seen += c_total
                 running += loss
@@ -451,11 +556,7 @@ def train_model(model, train_loader, test_loader, initial_learning_rate=0.001, u
             new_learning_rate, stop_training = lr_scheduler.update_learning_rate(epoch, error)
             if stop_training is True:
                 break
-            for opt in (optimizer, rest_optimizer):
-                for group in (opt.param_groups if opt is not None else []):
-                    if group["lr"] != new_learning_rate:
-                        graphed = None                                     # the captured SGD update holds the old rate
-                    group["lr"] = new_learning_rate
+            _set_learning_rate([opt for opt in (optimizer, rest_optimizer) if opt is not None], new_learning_rate, runner)
             state["lr"] = new_learning_rate
     except KeyboardInterrupt:
         informationDict["errorFlag"] = False
@@ -466,6 +567,7 @@ def train_model(model, train_loader, test_loader, initial_learning_rate=0.001, u
     if quantizer is not None and not fused:                                # (fused: the live weights already are)
         quantizer.quantize_weights_model(save=False)                       # final weights are returned quantized (:384-385)
     informationDict["fused_optimizer_step"] = fused
+    informationDict["cuda_graph_step"] = runner.captured
     if mix_with_differentiable_quantization:
         informationDict["numEpochsTrained"] *= 2
     informationDict["percentages_asked_teacher"] = percentages_asked_teacher
@@ -487,91 +589,14 @@ def train_model_quantized(model, train_loader, test_loader, numBits=8, bucket_si
 # ------------------------------------------------------------------------------------------
 def _capture_point_graphs(quantize_all, point_gradients, device):
     """Captures the two per-step launch sequences of the differentiable-quantization loop.
-    Returns (forward_graph, backward_graph, gradient tensors) or False when capture fails."""
-    try:
-        torch.cuda.synchronize(device)
-        side = torch.cuda.Stream(device)
-        side.wait_stream(torch.cuda.current_stream(device))
-        with torch.cuda.stream(side):                       # warm the capture stream's workspace / caches
-            quantize_all()
-            point_gradients()
-        torch.cuda.current_stream(device).wait_stream(side)
-        torch.cuda.synchronize(device)
-        g_fwd, g_bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g_fwd):
-            quantize_all()
-        with torch.cuda.graph(g_bwd):
-            grads = point_gradients()
-        return g_fwd, g_bwd, grads
-    except Exception as e:                                   # pragma: no cover - depends on driver / torch build
-        import warnings
-        warnings.warn(f"CUDA graph capture of the quantization step failed, running eagerly: {e}")
-        try:
-            torch.cuda.synchronize(device)
-        except Exception:
-            pass
-        return False
-
-
-def _data_parallel_module(model):
-    """The wrapped network when ``model`` is a :class:`FlatDataParallel` or stock DDP wrapper, else None."""
-    from ..distributed import FlatDataParallel
-    if isinstance(model, (FlatDataParallel, nn.parallel.DistributedDataParallel)):
-        return model.module
-    return None
-
-
-class _RankGroup:
-    """The collectives of the data-parallel differentiable-quantization loop.  Without an initialised
-    process group (a wrapper built in a single process) every call is the identity."""
-
-    def __init__(self, wrapper):
-        self.group = getattr(wrapper, "process_group", None)
-        self.active = dist.is_available() and dist.is_initialized()
-        self.world = dist.get_world_size(self.group) if self.active else 1
-        self.nccl = self.active and dist.get_backend(self.group) == "nccl"
-        self.src = (0 if self.group is None else dist.get_global_rank(self.group, 0)) if self.active else 0
-
-    def average(self, tensors):
-        """Rank average of a list of float32 tensors with ONE all-reduce; returns views of the reduced buffer."""
-        if not self.active:
-            return tensors
-        flat = torch.cat([t.reshape(-1) for t in tensors])
-        dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=self.group)
-        flat.mul_(1.0 / self.world)
-        return [v.view(t.shape) for v, t in zip(flat.split([t.numel() for t in tensors]), tensors)]
-
-    def check_point_counts(self, counts, device):
-        """Raises ValueError on every rank unless all ranks quantize the same tensors with the same point
-        counts (all-reduce MIN of (c, -c): min and max of every count at once)."""
-        if not self.active:
-            return
-        n = torch.tensor([len(counts), -len(counts)], dtype=torch.int64, device=device)
-        dist.all_reduce(n, op=dist.ReduceOp.MIN, group=self.group)
-        lo, hi = n.tolist()
-        if lo != -hi:
-            raise ValueError(f"ranks quantize different numbers of tensors ({lo} to {-hi})")
-        c = torch.tensor([int(k) for k in counts], dtype=torch.int64, device=device)
-        both = torch.cat([c, -c])
-        dist.all_reduce(both, op=dist.ReduceOp.MIN, group=self.group)
-        lo, hi = both[:len(counts)].tolist(), [-v for v in both[len(counts):].tolist()]
-        bad = [i for i, (a, b) in enumerate(zip(lo, hi)) if a != b]
-        if bad:
-            i = bad[0]
-            raise ValueError(f"ranks chose different numbers of points for {len(bad)} tensor(s); tensor {i}: "
-                             f"{lo[i]} to {hi[i]} points")
-
-    def broadcast_buffers(self, model):
-        if self.active:
-            for b in model.buffers():
-                dist.broadcast(b.data, self.src, group=self.group)
-
-    def mean(self, value, device):
-        if not self.active:
-            return value
-        t = torch.tensor([value], dtype=torch.float64, device=device)
-        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
-        return float(t.item()) / self.world
+    Returns (forward_graph, backward_graph, gradient tensors), or None when capture fails."""
+    _, on_side = _side_stream(device)
+    with on_side():                                          # warm the capture stream's workspace / caches
+        quantize_all()
+        point_gradients()
+    fwd = _capture(quantize_all, device, what="the quantization step")
+    bwd = fwd and _capture(point_gradients, device, what="the quantization step")
+    return (fwd[0], bwd[0], bwd[1]) if bwd else None
 
 
 def optimize_quantization_points(modelToQuantize, train_loader, test_loader, initial_learning_rate=1e-5,
@@ -708,8 +733,8 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
         optimizer.zero_grad(set_to_none=False)
         if graphs is None and graph_after is not None and total_steps >= graph_after:
             graphs = _capture_point_graphs(quantize_all, point_gradients, device)
-            if graphs is False:
-                graph_after, graphs = None, None                          # capture unavailable: stay eager
+            if graphs is None:
+                graph_after = None                                        # capture unavailable: stay eager
         if graphs:
             graphs[0].replay()
         else:
@@ -730,38 +755,15 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
         points_table.copy_(torch.sort(points_table, dim=1)[0])            # :550-551, every list at once, in place
         return loss, 0, 0
 
-    # whole-step capture (opt-in), same mechanism as train_model(cuda_graph_step=True)
-    whole_ok = bool(cuda_graph_step and device.type == "cuda")
-    # data parallel: the collective is captured with the step only on NCCL behind FlatDataParallel (stock DDP and
-    # gloo run eagerly), and the step is replayed only if EVERY rank captured it (the rule of train_model)
-    collective = dp and ranks.active
-    if collective and (not ranks.nccl or isinstance(modelToQuantize, nn.parallel.DistributedDataParallel)):
-        whole_ok = False
-    side_stream = torch.cuda.Stream(device) if whole_ok else None
-    graphed = None
+    runner = _CapturedStep(one_step, optimizer, device, ranks=ranks,
+                           enabled=bool(cuda_graph_step and _step_capturable(modelToQuantize, ranks, device)))
 
     total_steps, epoch, stop = 0, 0, False
     for epoch in range(epochs_to_train):
         quantizedModel.train()
         running = torch.zeros((), device=device)
         for idx_minibatch, data in enumerate(train_loader, start=1):
-            if whole_ok and graphed is None and total_steps >= 3:
-                graphed = _GraphedStep(one_step, data, device, side_stream, optimizer, collective=collective)
-                captured = graphed.ok
-                if collective:
-                    flag = torch.tensor([1 if captured else 0], dtype=torch.int32, device=device)
-                    dist.all_reduce(flag, op=dist.ReduceOp.MIN, group=ranks.group)
-                    captured = bool(flag.item())
-                if not captured:
-                    whole_ok, graphed = False, None
-            if graphed is not None and graphed.matches(data):
-                loss = graphed.run(data)[0]
-            elif whole_ok:
-                with torch.cuda.stream(side_stream):
-                    loss = one_step(data, idx_minibatch, epoch)[0]
-                torch.cuda.current_stream(device).wait_stream(side_stream)
-            else:
-                loss = one_step(data, idx_minibatch, epoch)[0]
+            loss = runner.run(data, idx_minibatch, epoch)[0]
             running += loss
             total_steps += 1
             if step_hook is not None:
@@ -790,13 +792,10 @@ def optimize_quantization_points(modelToQuantize, train_loader, test_loader, ini
         new_learning_rate, stop_training = lr_scheduler.update_learning_rate(epoch, error)
         if stop_training is True:
             break
-        for group in optimizer.param_groups:
-            if group["lr"] != new_learning_rate:
-                graphed = None                                             # the captured update holds the old rate
-            group["lr"] = new_learning_rate
+        _set_learning_rate([optimizer], new_learning_rate, runner)
     informationDict = {"predictionAccuracy": pred_accuracy_epochs, "numEpochsTrained": epoch + 1,
                        "lossSaved": losses_epochs, "numStepsTrained": total_steps,
-                       "cuda_graph_step": graphed is not None, "cuda_graph_quantization": bool(graphs),
+                       "cuda_graph_step": runner.captured, "cuda_graph_quantization": bool(graphs),
                        "multi_tensor_plan": plan is not None}
     if dp:
         informationDict["data_parallel_world"] = ranks.world
