@@ -385,18 +385,6 @@ int qd_uniform_fwd_host(const float* x_host, float* q_host, int64_t n, int64_t b
 int qd_uniform_fwd_bwd_host(const float* x_host, const float* g_host, float* q_host, float* gout_host,
                             int64_t n, int64_t bucket, int levels, int mode, int device);
 
-/* ---- benchmark hook: override a path-selection threshold (tools/block_bench.py measures the
- * variants against each other with it); value -1 restores the built-in choice.
- *   key 0: longest row (floats) taken by the warp-per-row two-pass variant
- *   key 1: longest row (floats) that keeps two rows in flight per CTA in the staged path
- *   key 2: threads per CTA of the staged path (64 / 128 / 256 / 512 / 1024)
- *   key 3: warp-path min/max backward sums r_b per element in float64 (1) or in float32 groups of four (0);
- *          built-in choice: per element when q is written in the same pass, grouped for the backward alone
- *   key 4: longest row (floats) taken by the warp path (<= 1024)
- *   key 5 / 6 / 7: host entry points: pipeline slots (1..8) / chunk elements / staging path (0 = chunked copies,
- *          1 = one launch on pinned host pointers) */
-int qd_debug_set_tuning(int key, int64_t value);
-
 /* ---- self tests used by tests/ (device side arithmetic checks) ---------- */
 int qd_selftest_division(int64_t pairs, uint64_t seed, int64_t* mismatches, qd_stream_t stream);
 

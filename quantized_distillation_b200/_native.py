@@ -80,7 +80,6 @@ SIGNATURES = {
     "qd_multi_l2norm": (C.c_int, [_p, _p, _i32, _p, _p]),
     "qd_uniform_fwd_host": (C.c_int, [_p, _p, _i64, _i64, _i32, _i32]),
     "qd_uniform_fwd_bwd_host": (C.c_int, [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _i32]),
-    "qd_debug_set_tuning": (C.c_int, [_i32, _i64]),
     "qd_selftest_division": (C.c_int, [_i64, _u64, C.POINTER(_i64), _p]),
 }
 

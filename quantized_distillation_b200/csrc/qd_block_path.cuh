@@ -3,8 +3,8 @@
 //
 // Since round 2 the deterministic uniform op (forward, every backward mode) and the centroid op run on the
 // staged chunk ring; this kernel keeps the ops the ring does not implement -- per-row statistics, x_hat in the
-// padded layout, stochastic rounding -- in two variants (the benchmark hook can still force them for the
-// other ops, which is how tools/block_bench.py compares the variants):
+// padded layout, stochastic rounding -- in two variants, and the min/max backward on rows of 1025 ..
+// kWarp2MinmaxMaxRow floats in the first:
 //
 // WARP TWO-PASS (GROUP = 32, rows up to 2 * kWarpTwoPassMaxRow floats): a warp streams its row once for
 // min/max (tagged L2::evict_last) and again (L2 hit) for the element-wise pass; no block barrier anywhere,
@@ -91,7 +91,6 @@ __device__ __forceinline__ double cta_sum(double v, double* scratch) {
 
 // Round-1 measurement (tools/block_bench.py, 64 Mi floats): warp-per-row two-pass won up to 2048-4096 floats per
 // row, the whole-row staging above that, up to the 49152-float shared-memory limit.
-constexpr int kStagedMaxRow = QD_MAX_STAGED_BUCKET;  // floats; longer rows would use the L2 re-read variant
 constexpr int kWarpTwoPassMaxRow = 2048;  // floats; rows up to here: one WARP per row, two passes (second from L1/L2)
 constexpr int kWarp2MinmaxMaxRow = 2048;  // floats; the min/max backward takes the two-pass variant up to here (qd_quant.cu)
 
@@ -139,14 +138,12 @@ __device__ __forceinline__ void for_each_in_row(const float* s_row, const float*
 template <int OP, int BWD, bool STAGED, int GROUP>
 __global__ void __launch_bounds__(kBlockCtaThreads) block_rows_kernel(const __grid_constant__ Params P) {
     static_assert(!(STAGED && GROUP == 32), "staging is a CTA-wide operation");
+    static_assert(OP == OP_STATS || OP == OP_SCALE || (OP == OP_UNIFORM && (BWD == BWD_OFF || (BWD == BWD_MINMAX && GROUP == 32))),
+                  "block path: stats, scale, uniform forward (stochastic rounding), min/max backward warp two-pass");
     extern __shared__ __align__(128) float s_row[];
     __shared__ __align__(8) uint64_t s_bar[kMaxStageChunks];
-    __shared__ float s_k[OP == OP_NONUNIFORM ? 256 : 1];
-    __shared__ float s_t[OP == OP_NONUNIFORM ? 256 : 1];
     __shared__ double s_scratch[kBlockCtaThreads / 32];
 
-    Centroids cen{s_k, s_t, P.num_points};
-    if constexpr (OP == OP_NONUNIFORM) centroid_setup(s_k, s_t, P.points, P.num_points, P.rule);
     if (STAGED && threadIdx.x == 0) {
         for (int c = 0; c < kMaxStageChunks; ++c) mbar_init(&s_bar[c], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -159,7 +156,6 @@ __global__ void __launch_bounds__(kBlockCtaThreads) block_rows_kernel(const __gr
     const float max_el = P.max_element;
     uint32_t phase_bits = 0;  // bit c = parity the next wait on s_bar[c] must see
     const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
-    (void)pol_keep;
     constexpr int kGroups = kBlockCtaThreads / GROUP;  // rows in flight per CTA
 
     for (int64_t row = (int64_t)blockIdx.x * kGroups + (GROUP == 32 ? (threadIdx.x >> 5) : 0); row < P.geo.rows;
@@ -302,7 +298,6 @@ __global__ void __launch_bounds__(kBlockCtaThreads) block_rows_kernel(const __gr
             }
             // gout = g here; the two elements the min/max backward changes are patched after the sweep
             auto fix = [&](int e, float xv, float qv, float gv) -> float {
-                if constexpr (BWD == BWD_TRUNC) gv = (fabsf(xv) > 1.0f) ? 0.f : gv;
                 if constexpr (BWD == BWD_MINMAX) {
                     if (qv == qlo) imin2 = min(imin2, e);
                     if (qv == qhi) imax2 = min(imax2, e);
@@ -350,8 +345,7 @@ __global__ void __launch_bounds__(kBlockCtaThreads) block_rows_kernel(const __gr
                 imin2 = grp_min_int<GROUP>(imin2, reinterpret_cast<int*>(s_scratch));
                 imax2 = grp_min_int<GROUP>(imax2, reinterpret_cast<int*>(s_scratch));
                 rb = (float)grp_sum<GROUP>(acc, s_scratch);
-                if constexpr (GROUP == 32) __syncwarp();   // the row's gout stores are ordered before the patch
-                else __syncthreads();
+                __syncwarp();   // the row's gout stores are ordered before the patch
                 if (tid == 0 && imin2 != imax2) {  // +r at argmax', -r at argmin' (quant_functions.py:380-393)
                     float* pmax = P.gout + base + imax2;
                     float* pmin = P.gout + base + imin2;
@@ -359,63 +353,6 @@ __global__ void __launch_bounds__(kBlockCtaThreads) block_rows_kernel(const __gr
                     *pmin = __fadd_rn(__ldcg(pmin), -rb);
                 }
             }
-        } else if constexpr (OP == OP_NONUNIFORM) {
-            const RowDivider div(rs.alpha);
-            const float thr = div.thr();
-            auto one = [&](int e, float t, float& qv) -> int {
-                const float xh = div.exact(__fsub_rn(t, rs.beta));
-                float kval;
-                const int id = smem_index<256>(cen.k, cen.t, xh, kval);
-                qv = from_unit(kval, rs.alpha, rs.beta);
-                if (pre) qv = __fadd_rn(qv, mean);
-                return id;
-            };
-            for_each_in_row<STAGED, GROUP>(
-                s_row, src, len, gvec, pre, mean, max_el,
-                [&](int e, float4 t) {
-                    // exact x_hat for four elements with one slow-path branch, then the table search
-                    const float a[4] = {__fsub_rn(t.x, rs.beta), __fsub_rn(t.y, rs.beta), __fsub_rn(t.z, rs.beta), __fsub_rn(t.w, rs.beta)};
-                    float xh[4];
-                    bool unsafe = !div.ok;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        xh[j] = div.fast(a[j]);
-                        unsafe = unsafe || div.needs_exact(a[j], thr);
-                    }
-                    if (unsafe) {
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) xh[j] = RowDivider::slow_div(a[j], rs.alpha);
-                    }
-                    float qq[4];
-                    int ii[4];
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        float kval;
-                        if (cen.K <= 4) ii[j] = smem_index<4>(cen.k, cen.t, xh[j], kval);
-                        else if (cen.K <= 16) ii[j] = smem_index<16>(cen.k, cen.t, xh[j], kval);
-                        else ii[j] = smem_index<256>(cen.k, cen.t, xh[j], kval);
-                        qq[j] = from_unit(kval, rs.alpha, rs.beta);
-                        if (pre) qq[j] = __fadd_rn(qq[j], mean);
-                    }
-                    const float4 qo = make_float4(qq[0], qq[1], qq[2], qq[3]);
-                    const int i0 = ii[0], i1 = ii[1], i2 = ii[2], i3 = ii[3];
-                    if (P.q != nullptr) {
-                        if (ovec) st_hint4(P.q + base + e, qo, pol_stream);
-                        else { P.q[base + e] = qo.x; P.q[base + e + 1] = qo.y; P.q[base + e + 2] = qo.z; P.q[base + e + 3] = qo.w; }
-                    }
-                    if (P.idx8 != nullptr) {
-                        if (ovec) *reinterpret_cast<uint32_t*>(P.idx8 + base + e) = (uint32_t)i0 | ((uint32_t)i1 << 8) | ((uint32_t)i2 << 16) | ((uint32_t)i3 << 24);
-                        else { P.idx8[base + e] = (uint8_t)i0; P.idx8[base + e + 1] = (uint8_t)i1; P.idx8[base + e + 2] = (uint8_t)i2; P.idx8[base + e + 3] = (uint8_t)i3; }
-                    }
-                    if (P.idx64 != nullptr) { P.idx64[base + e] = i0; P.idx64[base + e + 1] = i1; P.idx64[base + e + 2] = i2; P.idx64[base + e + 3] = i3; }
-                },
-                [&](int e, float t) {
-                    float qv;
-                    const int id = one(e, t, qv);
-                    if (P.q != nullptr) P.q[base + e] = qv;
-                    if (P.idx8 != nullptr) P.idx8[base + e] = (uint8_t)id;
-                    if (P.idx64 != nullptr) P.idx64[base + e] = id;
-                });
         }
         if constexpr (GROUP != 32) __syncthreads();  // everyone is done with the row (and s_row) before the next one
     }

@@ -14,16 +14,13 @@
 #include "qd_launch.h"
 
 using qd::fail;
-using qd::tuning;
 
 namespace {
 
-// pipeline depth and chunk size: three slots of 8-16 MiB per buffer sit on the plateau of the tuning
-// sweeps (tools/e2e_variants.py: slots beyond 2 and chunks beyond 16 MiB changed nothing)
-constexpr int kMaxSlots = 8;
+// pipeline depth and chunk size: three slots of 8-16 MiB per buffer sit on the plateau of the sweeps (slots and chunk
+// sizes forced through a since-removed tuning hook: slots beyond 2 and chunks beyond 16 MiB changed nothing)
 constexpr int kSlots = 3;
 constexpr int64_t kChunkElems = 4 << 20;
-constexpr int64_t kMaxChunkElems = 32 << 20;
 constexpr int64_t kDirectMaxElems = 8 << 20;   // largest tensor run as ONE launch on pinned host pointers
 
 struct Slot {
@@ -36,7 +33,7 @@ struct Slot {
 struct HostCtx {
     int slots = 0;              // allocated slots
     int64_t chunk_cap = 0;      // their capacity in elements
-    Slot slot[kMaxSlots];
+    Slot slot[kSlots];
     float *big_x = nullptr, *big_g = nullptr, *big_q = nullptr, *big_gout = nullptr;  // bucket=None path
     int64_t big_cap = 0;
     void* big_ws = nullptr;
@@ -52,9 +49,9 @@ struct DeviceGuard {
     ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
-int ensure_ctx(int device, int slots, int64_t chunk_elems, HostCtx** out) {
+int ensure_ctx(int device, int64_t chunk_elems, HostCtx** out) {
     HostCtx& c = g_ctx[device];
-    if (c.slots < slots || c.chunk_cap < chunk_elems) {
+    if (c.slots < kSlots || c.chunk_cap < chunk_elems) {
         for (int i = 0; i < c.slots; ++i) {
             Slot& s = c.slot[i];
             cudaFree(s.x); cudaFree(s.g); cudaFree(s.q); cudaFree(s.gout); cudaFree(s.ws);
@@ -63,7 +60,7 @@ int ensure_ctx(int device, int slots, int64_t chunk_elems, HostCtx** out) {
         }
         c.slots = 0;
         c.chunk_cap = 0;
-        for (int i = 0; i < slots; ++i) {
+        for (int i = 0; i < kSlots; ++i) {
             Slot& s = c.slot[i];
             if (s.stream == nullptr) QD_CUDA(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
             const size_t bytes = (size_t)chunk_elems * sizeof(float);
@@ -74,7 +71,7 @@ int ensure_ctx(int device, int slots, int64_t chunk_elems, HostCtx** out) {
             s.ws_bytes = qd_workspace_bytes(chunk_elems, 0);
             QD_CUDA(cudaMalloc(&s.ws, s.ws_bytes));
         }
-        c.slots = slots;
+        c.slots = kSlots;
         c.chunk_cap = chunk_elems;
     }
     *out = &c;
@@ -92,21 +89,18 @@ int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t 
     QD_CUDA(cudaGetDevice(&guard.prev));
     QD_CUDA(cudaSetDevice(device));
     std::lock_guard<std::mutex> lk(g_mu[device]);
-    // tuning keys: 5 = slots, 6 = chunk elements, 7 = staging path (below)
-    const int64_t t_slots = tuning(5), t_chunk = tuning(6), t_path = tuning(7);
-    const int n_slots = (t_slots >= 1 && t_slots <= kMaxSlots) ? (int)t_slots : kSlots;
     // Pinned (cudaHostAlloc'd / registered) host buffers are device-addressable under UVA: the kernel can read its
     // inputs and write its outputs straight over PCIe.  Such a launch moves less per direction than the copy engines
     // but has no pipeline to fill and drain, so it wins on small tensors; the crossover is set at 8 Mi elements
-    // (tools/e2e_variants.py measures it; mixed forms -- DMA one way, the kernel the other -- lost at every size).
-    // key 7: 0 = staged pipeline, 1 = one launch on the host pointers, -1 = this rule.
+    // (measured with both paths forced through a since-removed tuning hook; mixed forms -- DMA one way, the kernel the
+    // other -- lost at every size).
     auto device_view = [](const void* p) -> void* {
         if (p == nullptr) return nullptr;
         cudaPointerAttributes at;
         if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return nullptr; }
         return at.type == cudaMemoryTypeHost ? at.devicePointer : nullptr;
     };
-    bool direct = t_path >= 0 ? t_path == 1 : n <= kDirectMaxElems;
+    bool direct = n <= kDirectMaxElems;
     const float *dev_x = nullptr, *dev_g = nullptr;
     float *dev_q = nullptr, *dev_gout = nullptr;
     if (direct) {
@@ -117,9 +111,9 @@ int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t 
         direct = dev_x != nullptr && dev_q != nullptr && (!bwd || (dev_g != nullptr && dev_gout != nullptr));
     }
     // staged pipeline: ~8 chunks per tensor, 8 MiB (below that per-copy overhead wins) to 16 MiB per buffer
-    const int64_t chunk_elems = (t_chunk >= 1024 && t_chunk <= kMaxChunkElems) ? t_chunk : (n >= (32ll << 20) ? kChunkElems : kChunkElems / 2);
+    const int64_t chunk_elems = n >= (32ll << 20) ? kChunkElems : kChunkElems / 2;
     HostCtx* c;
-    int rc = ensure_ctx(device, n_slots, chunk_elems, &c);
+    int rc = ensure_ctx(device, chunk_elems, &c);
     if (rc) return rc;
 
     int64_t rows, row_len, padded;
@@ -162,7 +156,8 @@ int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t 
     // same bucket size, which is exact because rows never straddle a chunk boundary and
     // only the last chunk holds the (short) tail row.
     // (A ramp of smaller chunks at the head and the tail to shorten the half-duplex fill / drain was measured and
-    // dropped: copies below 16 MiB lose more to per-copy overhead than the ramp saves, tools/e2e_variants.py.)
+    // dropped: copies below 16 MiB lose more to per-copy overhead than the ramp saves; chunk sizes were forced through a
+    // since-removed tuning hook.)
     // the register / staged-row kernels read and write every element once; the grid path (rows beyond
     // QD_MAX_STAGED_BUCKET floats) makes several passes and keeps its staging
     if (direct && row_len <= QD_MAX_STAGED_BUCKET) {
@@ -179,7 +174,7 @@ int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t 
     const int64_t chunk = rows_per_chunk * row_len;
     int k = 0;
     for (int64_t off = 0; off < n; off += chunk, ++k) {
-        Slot& s = c->slot[k % n_slots];
+        Slot& s = c->slot[k % kSlots];
         const int64_t len = (n - off < chunk) ? (n - off) : chunk;
         const size_t bytes = (size_t)len * sizeof(float);
         // a chunk shorter than the bucket must still be bucketed like the tail of the
@@ -194,7 +189,7 @@ int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t 
         QD_CUDA(cudaMemcpyAsync(hq + off, s.q, bytes, cudaMemcpyDeviceToHost, s.stream));
         if (bwd) QD_CUDA(cudaMemcpyAsync(hgout + off, s.gout, bytes, cudaMemcpyDeviceToHost, s.stream));
     }
-    for (int i = 0; i < n_slots; ++i) QD_CUDA(cudaStreamSynchronize(c->slot[i].stream));
+    for (int i = 0; i < kSlots; ++i) QD_CUDA(cudaStreamSynchronize(c->slot[i].stream));
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }

@@ -1,5 +1,5 @@
 // qd_launch.cu -- state of the shared host layer (qd_launch.h) and the entry points that read it: last error,
-// version, device info, tuning hook.
+// version, device info.
 #include "qd_launch.h"
 
 #include <cstdarg>
@@ -40,11 +40,6 @@ int dev_info(DevInfo** out) {
     *out = &g_dev[d];
     return QD_OK;
 }
-
-// ------------------------------------------------------------------ tuning hook
-static int64_t g_tune[8] = {-1, -1, -1, -1, -1, -1, -1, -1};
-
-int64_t tuning(int key) { return (key >= 0 && key < 8) ? g_tune[key] : -1; }
 
 // ------------------------------------------------------------------ grid sizing
 struct OccKey {
@@ -110,7 +105,7 @@ int opt_in_smem(const void* kernel, size_t smem, size_t* opted) {
 
 using namespace qd;
 
-extern "C" int qd_version(void) { return 100; }
+extern "C" int qd_version(void) { return 101; }
 extern "C" const char* qd_last_error(void) { return g_err; }
 
 extern "C" int qd_device_info(int* sm_count, int* cc_major, int* cc_minor) {
@@ -120,11 +115,5 @@ extern "C" int qd_device_info(int* sm_count, int* cc_major, int* cc_minor) {
     if (sm_count) *sm_count = di->sms;
     if (cc_major) *cc_major = di->major;
     if (cc_minor) *cc_minor = di->minor;
-    return QD_OK;
-}
-
-extern "C" int qd_debug_set_tuning(int key, int64_t value) {
-    if (key < 0 || key >= 8) return fail(QD_ERR_INVALID_ARG, "unknown tuning key %d", key);
-    g_tune[key] = value;
     return QD_OK;
 }

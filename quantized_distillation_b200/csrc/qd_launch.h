@@ -1,5 +1,5 @@
 // qd_launch.h -- host layer shared by every translation unit of libqd_b200.so (state in qd_launch.cu): the
-// per-thread error message, device properties, the tuning hook and grid sizing.  Host code only.
+// per-thread error message, device properties and grid sizing.  Host code only.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -37,9 +37,6 @@ int capped_grid(int64_t need, int64_t per_sm, int* grid);
 int resident_grid(const void* kernel, int threads, size_t smem, int64_t need, int* grid);
 // Opts `kernel` into `smem` bytes of dynamic shared memory; `opted` is the kernel's own per-device table (64 slots).
 int opt_in_smem(const void* kernel, size_t smem, size_t* opted);
-
-// tuning hook (qd_debug_set_tuning, benchmarks only): -1 = built-in choice; keys are listed where they are used
-int64_t tuning(int key);
 
 inline cudaStream_t as_stream(qd_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }

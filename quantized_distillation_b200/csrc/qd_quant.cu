@@ -5,7 +5,8 @@
 //     L <= 1024                  warp path    (registers, 1 HBM pass)
 //     L <= QD_MAX_STAGED_BUCKET  staged path  (TMA chunk ring in shared memory, 1 HBM pass; CTA size by L)
 //     otherwise                  grid path    (two streaming passes)
-// Thresholds inside these ranges come from tools/block_bench.py (every variant forced through the tuning hook).
+// Thresholds inside these ranges were measured with tools/block_bench.py, every variant forced through a tuning hook
+// that has since been removed.
 #include <cstring>
 
 #include "qd_abs_path.cuh"
@@ -52,11 +53,10 @@ static int launch_warp_inst(const Params& P, cudaStream_t s) {
         if (rc) return rc;
     }
     if constexpr (OP == OP_UNIFORM && BWD == (int)BWD_MINMAX) {
-        // r_b accumulation, chosen by A/B (tools/headline_ab.py, 64 Mi floats): the fused forward+backward is faster
-        // with one float64 add per element, the backward alone with the grouped lane sum.  So the variant follows the
-        // presence of the q output (key 3: 1 forces the per-element sum, 0 the grouped one).
-        const bool per_element = tuning(3) >= 0 ? (tuning(3) == 1) : (P.q != nullptr);
-        if (per_element) {
+        // r_b accumulation, chosen by A/B (64 Mi floats, both variants forced through a since-removed tuning hook):
+        // the fused forward+backward is faster with one float64 add per element, the backward alone with the grouped
+        // lane sum.  So the variant follows the presence of the q output.
+        if (P.q != nullptr) {
             auto kern_a = warp_rows_kernel<OP, BWD, R, VEC, true>;
             kern_a<<<grid, kWarpCtaThreads, 0, s>>>(P);
             QD_CUDA(cudaGetLastError());
@@ -97,12 +97,6 @@ static int launch_block_inst(const Params& P, cudaStream_t s) {
     return QD_OK;
 }
 
-// tuning keys of the block path:
-//   key 0: longest row (floats) handled by the warp-per-row two-pass variant of the block path
-//   key 1: longest row (floats) that keeps two rows in flight per CTA in the staged path
-//   key 2: CTA size of the staged path (64 / 128 / 256 / 512 / 1024), 0 or -1 = by row length
-//   key 3: 1 = headline kernel accumulates r_b with one float64 add per element (A/B measurement)
-
 // CTA per row, TMA chunk ring (qd_staged_path.cuh)
 template <int OP, int BWD, int STAGES, int T>
 static int launch_staged_inst(const Params& P, cudaStream_t s) {
@@ -122,47 +116,37 @@ static int launch_staged_inst(const Params& P, cudaStream_t s) {
     return QD_OK;
 }
 
-// CTA size and ring depth by row length (tools/block_bench.py, every variant forced through the tuning hook): 64
-// threads below 2048 floats (a 1280-float row is five full steps of a 64-thread CTA, three ragged ones of a 128-thread
-// CTA), 128 up to 3072, 256 up to 12288, 512 up to 24576, 1024 beyond; two rows in flight per CTA up to 3072 floats,
-// the chunk ring alone above (on H100 one row in flight is as fast or faster for every op at 4096 floats, and the
-// min/max backward gains most: fused 459 vs 526 us, alone 371 vs 429 us at 64 Mi floats).
-// Tuning key 1 = longest row with two rows in flight per CTA, key 2 = forced CTA size.
+// CTA size and ring depth by row length (tools/block_bench.py, every variant forced through a since-removed tuning
+// hook): 64 threads below 2048 floats (a 1280-float row is five full steps of a 64-thread CTA, three ragged ones of a
+// 128-thread CTA), 128 up to 3072, 256 up to 12288, 512 up to 24576, 1024 beyond; two rows in flight per CTA up to
+// 3072 floats, the chunk ring alone above (on H100 one row in flight is as fast or faster for every op at 4096 floats,
+// and the min/max backward gains most: fused 459 vs 526 us, alone 371 vs 429 us at 64 Mi floats).
 template <int OP, int BWD>
 static int launch_staged(const Params& P, cudaStream_t s) {
     const int64_t L = P.geo.row_len;
-    const int64_t two_max = tuning(1) >= 0 ? tuning(1) : kTwoStageMaxRow;
-    const bool two = L <= two_max && L <= 24576;
-    int T = L < 2048 ? 64 : L <= 3072 ? 128 : L <= 12288 ? 256 : L <= 24576 ? 512 : 1024;
-    if (tuning(2) > 0) T = (int)tuning(2);
-    if (two) {
-        if (T <= 64) return launch_staged_inst<OP, BWD, 2, 64>(P, s);
-        if (T <= 128) return launch_staged_inst<OP, BWD, 2, 128>(P, s);
-        if (T <= 256) return launch_staged_inst<OP, BWD, 2, 256>(P, s);
-        return launch_staged_inst<OP, BWD, 2, 512>(P, s);
-    }
-    if (T <= 256) return launch_staged_inst<OP, BWD, 1, 256>(P, s);
-    if (T <= 512) return launch_staged_inst<OP, BWD, 1, 512>(P, s);
+    if (L <= kTwoStageMaxRow) return L < 2048 ? launch_staged_inst<OP, BWD, 2, 64>(P, s) : launch_staged_inst<OP, BWD, 2, 128>(P, s);
+    if (L <= 12288) return launch_staged_inst<OP, BWD, 1, 256>(P, s);
+    if (L <= 24576) return launch_staged_inst<OP, BWD, 1, 512>(P, s);
     return launch_staged_inst<OP, BWD, 1, 1024>(P, s);
 }
 
+// Rows of 1025 .. QD_MAX_STAGED_BUCKET floats, and the ragged 513 .. 1023-float rows of the min/max backward.
 template <int OP, int BWD>
 static int launch_block(const Params& P, cudaStream_t s) {
-    // the staged ring wins or ties at every row length for the ops it implements (tools/block_bench.py);
-    // the ops it does not implement (stats / scale / stochastic) keep the round-1 warp two-pass / whole-row staging
-    constexpr bool kStagedOp = (OP == OP_UNIFORM || OP == OP_NONUNIFORM);
-    const bool staged_ok = kStagedOp && !P.stochastic;
-    // except the min/max backward on rows of 1025 .. 2048 floats, where the warp two-pass variant is faster on H100
-    // (64 Mi floats: fused 460 vs 527 us at 1280 floats, 464 vs 531 us at 2048; backward alone 373 vs 409, 380 vs 407)
-    constexpr bool kMinmax = OP == OP_UNIFORM && BWD == (int)BWD_MINMAX;
-    const bool minmax_warp2 = kMinmax && staged_ok && P.geo.row_len > 1024 && P.geo.row_len <= kWarp2MinmaxMaxRow;
-    const int64_t warp2_default = !staged_ok ? 2 * kWarpTwoPassMaxRow : minmax_warp2 ? kWarp2MinmaxMaxRow : 0;
-    const int64_t warp2_max = tuning(0) >= 0 ? tuning(0) : warp2_default;
-    if (P.geo.row_len <= warp2_max) return launch_block_inst<OP, BWD, false, 32>(P, s);               // warp per row, two passes
-    if constexpr (kStagedOp) {
-        if (staged_ok) return launch_staged<OP, BWD>(P, s);
+    if constexpr (OP == OP_UNIFORM || OP == OP_NONUNIFORM) {
+        // the staged ring wins or ties at every row length for the ops it implements (tools/block_bench.py), except
+        // the min/max backward on rows of 1025 .. 2048 floats, where the warp two-pass variant is faster on H100
+        // (64 Mi floats: fused 460 vs 527 us at 1280 floats, 464 vs 531 us at 2048; backward alone 373 vs 409, 380 vs 407)
+        if constexpr (OP == OP_UNIFORM && BWD == (int)BWD_MINMAX)
+            if (P.geo.row_len > 1024 && P.geo.row_len <= kWarp2MinmaxMaxRow) return launch_block_inst<OP, BWD, false, 32>(P, s);
+        return launch_staged<OP, BWD>(P, s);
+    } else {
+        // the ops the ring does not implement (stats / scale / stochastic) keep the round-1 kernels: warp per row, two
+        // passes, then CTA per row, whole-row staging (stochastic rounding is a run-time branch of OP_UNIFORM there)
+        constexpr int OP2 = (OP == OP_UNIFORM_STOCH) ? OP_UNIFORM : OP;
+        if (P.geo.row_len <= 2 * kWarpTwoPassMaxRow) return launch_block_inst<OP2, BWD, false, 32>(P, s);
+        return launch_block_inst<OP2, BWD, true, kBlockCtaThreads>(P, s);
     }
-    return launch_block_inst<OP, BWD, true, kBlockCtaThreads>(P, s);  // scale / stats / stochastic: CTA per row, whole-row staging
 }
 
 template <int OP, int BWD>
@@ -194,24 +178,19 @@ static bool rows_vectorizable(const Params& P) {
     return ptrs && (P.geo.rows == 1 || (P.geo.row_len % 4) == 0);
 }
 
-// longest row the register-resident warp path takes for (OP, BWD); set from tools/block_bench.py --small
-template <int OP, int BWD>
-static constexpr int64_t warp_path_max_row() { return 1024; }
-
 template <int OP, int BWD>
 static int run_rows(const Params& P, void* ws, size_t ws_bytes, cudaStream_t s) {
     if (P.geo.row_len >= (int64_t)1 << 31) return fail(QD_ERR_UNSUPPORTED, "rows of 2^31 elements or more are not supported");
-    // longest row of the register-resident warp path (key 4 of the tuning hook moves the border for measurements)
-    const int64_t warp_max = (tuning(4) >= 0 && tuning(4) <= 1024) ? tuning(4) : warp_path_max_row<OP, BWD>();
     // ragged rows of 513..1023 floats with the min/max backward: the R = 8 register kernel runs its predicated
-    // (non-FULL) variant at 128 registers there and loses to the staged ring (tools/block_bench.py --small);
-    // everything else up to 1024 floats is faster in registers
-    const bool ragged_minmax = OP == OP_UNIFORM && BWD == (int)BWD_MINMAX && P.geo.row_len > 512 && P.geo.row_len < 1024 && tuning(4) < 0;
-    if (P.geo.row_len <= warp_max && !ragged_minmax)
+    // (non-FULL) variant at 128 registers there and loses to the staged ring (measured with tools/block_bench.py
+    // --small, the ring forced down to these rows through a since-removed tuning hook); everything else up to 1024
+    // floats is faster in registers
+    const bool ragged_minmax = OP == OP_UNIFORM && BWD == (int)BWD_MINMAX && P.geo.row_len > 512 && P.geo.row_len < 1024;
+    if (P.geo.row_len <= 1024 && !ragged_minmax)
         return launch_warp<OP, (OP == OP_NONUNIFORM ? 256 : BWD)>(P, rows_vectorizable(P), s);
-    // the CTA / grid paths keep stochastic rounding as a run-time branch of OP_UNIFORM
+    if (P.geo.row_len <= QD_MAX_STAGED_BUCKET) return launch_block<OP, BWD>(P, s);
+    // the grid path keeps stochastic rounding as a run-time branch of OP_UNIFORM
     constexpr int OP2 = (OP == OP_UNIFORM_STOCH) ? OP_UNIFORM : OP;
-    if (P.geo.row_len <= QD_MAX_STAGED_BUCKET) return launch_block<OP2, BWD>(P, s);
     if (BWD == BWD_MINMAX)
         return fail(QD_ERR_UNSUPPORTED, "minmax backward needs bucket <= %d (reference: bucket_size None not supported, quant_functions.py:332-334)", QD_MAX_STAGED_BUCKET);
     return launch_grid<OP2, (BWD == BWD_MINMAX ? BWD_OFF : BWD)>(P, ws, ws_bytes, s);
@@ -442,8 +421,7 @@ extern "C" int qd_nonuniform_fwd(const float* x, const float* points, int num_po
     P.x = x; P.q = q; P.idx8 = idx_u8; P.idx64 = idx_i64; P.alpha = alpha; P.beta = beta;
     P.points = points; P.num_points = num_points; P.rule = rule; P.mean = mean; P.max_element = max_element;
     cudaStream_t s = as_stream(stream);
-    const int64_t warp_max = (tuning(4) >= 0 && tuning(4) <= 1024) ? tuning(4) : warp_path_max_row<OP_NONUNIFORM, BWD_OFF>();
-    if (P.geo.row_len <= warp_max) {  // warp path: centroid tables of up to 32 points live in the lanes (AUX = table size class)
+    if (P.geo.row_len <= 1024) {  // warp path: centroid tables of up to 32 points live in the lanes (AUX = table size class)
         const bool vec = rows_vectorizable(P);
         if (num_points <= 4) return launch_warp<OP_NONUNIFORM, 4>(P, vec, s);     // <= 32: table in the lanes (LaneSearch)
         if (num_points <= 8) return launch_warp<OP_NONUNIFORM, 8>(P, vec, s);

@@ -171,7 +171,7 @@ __device__ __forceinline__ void warp_load_row(const Params& P, int64_t row, int 
     if constexpr (BWD != BWD_OFF) load_row<R, VEC, FULL>(P.g + base, len, lane, gv);
 }
 
-// ACC_A: A/B switch of the r_b accumulation of the min/max backward (benchmarks only, qd_debug_set_tuning key 3):
+// ACC_A: r_b accumulation of the min/max backward, chosen by the launcher from whether q is written (qd_quant.cu):
 // false = minmax_lane_sum (division mode hoisted, float32 groups), true = one float64 add per element
 template <int OP, int AUX, int R, bool VEC, bool FULL, bool ACC_A = false, int PACK = 0>
 __device__ __forceinline__ void warp_compute_row(const Params& P, const Centroids& cen, const LaneTable<OP, AUX>& rt, int64_t row,
