@@ -227,6 +227,19 @@ int qd_packed_conv2d(const float* x, int64_t batch, int64_t in_channels, int64_t
                      int bits, const float* alpha, const float* beta, const float* points, int num_points, int levels,
                      int64_t bucket, const float* bias, float* y, qd_stream_t stream);
 
+/* Embedding lookup on packed weights: out[i, :] = row indices[i] of W, for W the tensor of num_embeddings*dim elements
+ * (flattened [num_embeddings, dim]) that qd_unpack_dequant_* writes from (packed, alpha, beta) at this bucket: every
+ * value is from_unit(unit[code], alpha, beta), bit for bit what the unpack writes for that row.  indices: `count`
+ * contiguous int32 (index_bytes 4) or int64 (index_bytes 8), repeats allowed; out: float32[count, dim], C order, any
+ * 4-byte alignment, not overlapping the indices.  levels, points and num_points as for qd_packed_linear.  An index
+ * outside [0, num_embeddings) is never dereferenced: its row of out is written NaN and *invalid (a device int32, may be
+ * NULL) is incremented once per such index; the kernel does not trap.  QD_ERR_INVALID_ARG: NULL pointers, index_bytes
+ * not 4 or 8, sizes < 1, sizes past 64-bit indexing, bits too narrow, out overlapping the indices.  QD_ERR_UNSUPPORTED:
+ * more rows than one launch holds.  Needs no workspace; only enqueues work on `stream` (graph-capturable). */
+int qd_packed_embedding(const void* indices, int index_bytes, int64_t count, int64_t num_embeddings, int64_t dim,
+                        const uint8_t* packed, int bits, const float* alpha, const float* beta, const float* points,
+                        int num_points, int levels, int64_t bucket, float* out, int32_t* invalid, qd_stream_t stream);
+
 /* ---- next row f2: Huffman-coded storage (the model helpers/functions.py:226-262 only sizes) ----------
  * Canonical code over uint8 symbols, codes of 1..QD_HUFFMAN_MAX_LENGTH bits (built on the host: codec.py).
  * Stream: a tensor's symbols are cut into chunks of QD_HUFFMAN_CHUNK; each chunk's codes are written MSB-first

@@ -54,6 +54,7 @@ SIGNATURES = {
     "qd_packed_linear": (C.c_int, [_p, _i64, _i64, _i64, _p, _i32, _p, _p, _p, _i32, _i32, _i64, _p, _p, _p]),
     "qd_packed_conv2d": (C.c_int, [_p, _i64, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _p, _i32, _p, _p, _p, _i32,
                                    _i32, _i64, _p, _p, _p]),
+    "qd_packed_embedding": (C.c_int, [_p, _i32, _i64, _i64, _i64, _p, _i32, _p, _p, _p, _i32, _i32, _i64, _p, _p, _p]),
     "qd_huffman_encode": (C.c_int, [_p, _i64, _p, _p, _i64, _p, _p, _p]),
     "qd_huffman_decode_dequant_uniform": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _i64, _i64, _i32, _p]),
     "qd_huffman_decode_dequant_nonuniform": (C.c_int, [_p, _i64, _p, _p, _p, _i32, _p, _p, _p, _i64, _i64, _p]),

@@ -1128,6 +1128,62 @@ class PackedConv2d(torch.nn.Module):
         return y if x.dim() == 4 else y[0]
 
 
+class PackedEmbedding(torch.nn.Module):
+    """Inference replacement of an ``nn.Embedding`` whose weight stays in its fixed-width stored form (one PackedEntry
+    of a PackedModel with a [num_embeddings, embedding_dim] shape) on the device.  Forward takes int32 or int64 CUDA
+    indices of any shape and returns ``input.shape + (embedding_dim,)`` float32 rows gathered by qd_packed_embedding,
+    which reads only the codes of those rows: every value is bit for bit what unpack_ writes for it.  The row of
+    ``padding_idx`` is returned as stored, as an unpack_-loaded nn.Embedding returns it.  Unlike torch, an index outside
+    [0, num_embeddings) does not raise a device-side assert: its output row is NaN and it is counted on the device,
+    which invalid_index_count() reads.  Forward never synchronises, so it can be captured in a CUDA graph."""
+
+    def __init__(self, entry: PackedEntry, kind: str, levels, bucket_size, padding_idx=None):
+        super().__init__()
+        if not entry.quantized or len(entry.shape) != 2:
+            raise ValueError(f"{entry.name}: a PackedEmbedding needs a quantized two-dimensional weight")
+        self.num_embeddings, self.embedding_dim = (int(d) for d in entry.shape)
+        if padding_idx is not None:
+            if not -self.num_embeddings <= padding_idx < self.num_embeddings:
+                raise ValueError(f"{entry.name}: padding_idx {padding_idx} outside the {self.num_embeddings} embeddings")
+            padding_idx = padding_idx % self.num_embeddings
+        self.padding_idx = padding_idx
+        _hold_sections(self, entry, kind, levels, bucket_size, None, 0)
+        self.register_buffer("invalid", torch.zeros(1, dtype=torch.int32, device=self.packed.device), persistent=False)
+
+    def extra_repr(self) -> str:
+        return (f"{self.num_embeddings}, {self.embedding_dim}, padding_idx={self.padding_idx}, {self.kind}, bits={self.bits}, "
+                f"bucket_size={self.bucket_size}")
+
+    def decoded_weight(self) -> torch.Tensor:
+        """The decoded float32 weight [num_embeddings, embedding_dim], bit for bit what unpack_ writes."""
+        return _decoded(self, (self.num_embeddings, self.embedding_dim))
+
+    def invalid_index_count(self) -> int:
+        """Number of out-of-range indices forward has met since the last call, read with one device synchronise, then
+        reset to 0."""
+        torch.cuda.synchronize(self.invalid.device)
+        n = int(self.invalid.item())
+        self.invalid.zero_()
+        return n
+
+    def forward(self, input: torch.Tensor) -> torch.Tensor:
+        if not torch.is_tensor(input) or not input.is_cuda or input.dtype not in (torch.int32, torch.int64):
+            raise ValueError("PackedEmbedding takes an int32 or int64 CUDA tensor of indices")
+        if input.device != self.packed.device:
+            raise ValueError(f"input on {input.device}, the packed weight on {self.packed.device}")
+        _check_state(self, input, "PackedEmbedding")
+        out = torch.empty(*input.shape, self.embedding_dim, dtype=torch.float32, device=input.device)
+        if input.numel():
+            idx = input.contiguous()
+            b = 0 if self.bucket_size is None else int(self.bucket_size)
+            with torch.cuda.device(input.device):
+                N.check(N.lib().qd_packed_embedding(N.ptr(idx), idx.element_size(), idx.numel(), self.num_embeddings,
+                                                    self.embedding_dim, N.ptr(self.packed), self.bits, N.ptr(self.alpha),
+                                                    N.ptr(self.beta), N.ptr(self.points), 0 if self.points is None else self.points.numel(),
+                                                    self.levels, b, N.ptr(out), N.ptr(self.invalid), N.stream_ptr(input.device)))
+        return out
+
+
 def _conv_padding(conv) -> tuple:
     """(pad_h, pad_w) of an nn.Conv2d's padding when it is symmetric: an int pair, "valid", or "same" whose total
     padding per side is even; None otherwise."""
@@ -1152,6 +1208,11 @@ def _conv_target(mod) -> bool:
             and _conv_padding(mod) is not None)
 
 
+def _embedding_target(mod) -> bool:
+    # type, not isinstance: a subclass may override forward; max_norm renormalises the weight in place during forward
+    return type(mod) is torch.nn.Embedding and mod.max_norm is None
+
+
 def _packed_linear(entry, pm, lin):
     return PackedLinear(entry, pm.kind, pm.levels, pm.bucket_size, None if lin.bias is None else lin.bias.data)
 
@@ -1161,22 +1222,34 @@ def _packed_conv(entry, pm, conv):
                         None if conv.bias is None else conv.bias.data)
 
 
-def _attach(pm: PackedModel, model, kinds) -> list:
+def _packed_embedding(entry, pm, emb):
+    return PackedEmbedding(entry, pm.kind, pm.levels, pm.bucket_size, emb.padding_idx)
+
+
+def _tied_pair(mods) -> bool:
+    """True when a weight's registrations are exactly one eligible nn.Embedding and one nn.Linear: a generator tied to
+    an embedding, whose [V, D] weight reads row v the same way in both."""
+    return len(mods) == 2 and mods[0] is not mods[1] and any(_embedding_target(m) for m in mods) \
+        and any(_linear_target(m) for m in mods)
+
+
+def _attach(pm: PackedModel, model, kinds, tied=False) -> list:
     """unpack_, except that every module accepted by the ``accept`` of one of ``kinds`` -- (accept, make, what) -- whose
     weight ``pm`` stores quantized and which is that weight's only holder is replaced in its parent by make(entry, pm,
-    module); the float32 weight is released.  Returns the names of the replaced modules."""
+    module); the float32 weight is released.  With ``tied``, so are both modules of a tied embedding / generator pair
+    (_tied_pair), and the two share one set of device sections.  Returns the names of the replaced modules."""
     named, bufs = _check_target(pm, model)
     index = {id(p): k for k, (_, p) in enumerate(named)}
-    holders = {}                                 # parameter -> registrations in the module tree, every path counted
+    holders = {}                                 # parameter -> its registrations in the module tree, every path counted
     for _, mod in model.named_modules(remove_duplicate=False):
         for p in mod._parameters.values():
             if p is not None:
-                holders[id(p)] = holders.get(id(p), 0) + 1
+                holders.setdefault(id(p), []).append(mod)
     targets = []                                 # (module name, parent, attribute, module, weight index, make)
     for mname, mod in model.named_modules():
         for accept, make, what in kinds:
             if accept(mod) and id(mod.weight) in index and pm.tensors[index[id(mod.weight)]].quantized \
-                    and holders[id(mod.weight)] == 1:
+                    and (len(holders[id(mod.weight)]) == 1 or tied and _tied_pair(holders[id(mod.weight)])):
                 if not mod.weight.is_cuda:
                     raise ValueError(f"{mname}: a Packed{what} runs on a CUDA device, the {what} is on {mod.weight.device}")
                 parent_name, _, attr = mname.rpartition(".")
@@ -1184,14 +1257,16 @@ def _attach(pm: PackedModel, model, kinds) -> list:
                 break
     _write_into(pm, named, bufs, skip={t[4] for t in targets})
     movers = {}
+    held = {}                                    # weight index -> the sections its first replacement holds
     for mname, parent, attr, mod, k, make in targets:
         dev = mod.weight.device
         t = pm.tensors[k]
         with torch.cuda.device(dev):
             move = movers.setdefault(dev, _mover(pm, dev))
-            entry = PackedEntry(t.name, t.shape, bits=t.bits, packed=move(t.packed), alpha=move(t.alpha), beta=move(t.beta),
-                                points=None if t.points is None else t.points.to(dev))
+            entry = held.get(k) or PackedEntry(t.name, t.shape, bits=t.bits, packed=move(t.packed), alpha=move(t.alpha),
+                                               beta=move(t.beta), points=None if t.points is None else t.points.to(dev))
             layer = make(entry, pm, mod)
+        held[k] = PackedEntry(t.name, t.shape, bits=t.bits, packed=layer.packed, alpha=layer.alpha, beta=layer.beta, points=layer.points)
         setattr(parent, attr, layer)
     return [t[0] for t in targets]
 
@@ -1208,15 +1283,22 @@ def attach_packed_linear_(pm: PackedModel, model) -> list:
     return _attach(pm, model, [(_linear_target, _packed_linear, "Linear")])
 
 
-def attach_packed_(pm: PackedModel, model) -> list:
+def attach_packed_(pm: PackedModel, model, *, embeddings=False) -> list:
     """attach_packed_linear_ for Linear and convolution layers: every nn.Linear it would replace becomes a
     PackedLinear, and every ``nn.Conv2d`` (the class itself, not a subclass) with groups 1, dilation 1, zero padding
     that is symmetric (int padding, "valid", or "same" that resolves to equal sides) and a weight ``pm`` stores
     quantized and it alone holds becomes a PackedConv2d with that weight's packed sections, its stride, padding and
-    bias.  The replaced float32 weights are released; every other parameter and layer, and the stored buffers, are
-    written exactly as unpack_ writes them, quantized tensors in one launch per device.  Everything is checked before
-    anything is written.  Returns the names of the replaced modules, in module order."""
-    return _attach(pm, model, [(_linear_target, _packed_linear, "Linear"), (_conv_target, _packed_conv, "Conv2d")])
+    bias.  With ``embeddings=True``, also every ``nn.Embedding`` (the class itself) without max_norm whose weight ``pm``
+    stores quantized and it alone holds becomes a PackedEmbedding; and a weight held by exactly one such embedding and
+    one nn.Linear -- a generator tied to an embedding -- replaces both, by a PackedEmbedding and a PackedLinear (with the
+    Linear's bias) that share one copy of the sections on the device.  Any other weight with several holders is
+    decoded as unpack_ decodes it.  The replaced float32 weights are released; every other parameter and layer, and the
+    stored buffers, are written exactly as unpack_ writes them, quantized tensors in one launch per device.  Everything
+    is checked before anything is written.  Returns the names of the replaced modules, in module order."""
+    kinds = [(_linear_target, _packed_linear, "Linear"), (_conv_target, _packed_conv, "Conv2d")]
+    if embeddings:
+        kinds.append((_embedding_target, _packed_embedding, "Embedding"))
+    return _attach(pm, model, kinds, tied=embeddings)
 
 
 def save_packed(pm: PackedModel, path) -> int:

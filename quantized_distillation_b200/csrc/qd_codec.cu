@@ -897,6 +897,170 @@ extern "C" int qd_packed_conv2d(const float* x, int64_t batch, int64_t in_channe
     return QD_OK;
 }
 
+// ------------------------------------------------------------------ f2: embedding lookup on packed weights
+// out[i, d] = q[idx_i*D + d] where q is the tensor qd_unpack_dequant_* writes: every value is
+// from_unit(unit[code], alpha[bucket], beta[bucket]) with the unit table of load_unit_table, and nothing else.
+//
+// A row of D outputs is served by lpr lanes, the power of two >= ceil(D/4) up to 32, so a warp serves 32/lpr rows at
+// once and the grid covers the count rows once, without a grid stride.  Lane l of a row takes the groups of four
+// columns 4*l, 4*(l + lpr), ...: so the lanes of a row read one contiguous span of codes per step.  A group's 4*bits
+// code bits are one or two aligned 32-bit words funnel-shifted (a row starts inside a byte whenever D*bits is not a
+// multiple of 8); a word that reaches past the last code byte is read byte by byte up to it.  A bucket cursor per
+// group (one division per row, then one compare per element) gives each element its (alpha, beta).  An index outside
+// [0, V) is never dereferenced: its row is written NaN and counted once in *invalid.
+constexpr int kPeThreads = 256;
+
+struct PackedEmbeddingArgs {
+    const void* indices;
+    const uint8_t* packed;
+    const float* alpha;
+    const float* beta;
+    const float* points;
+    float* out;
+    int32_t* invalid;           // may be NULL
+    int64_t count, V, D;
+    int64_t in_bytes;           // ceil(V*D*bits/8)
+    int64_t L, rows;            // bucket row length and bucket count (geometry_of)
+    int64_t step_q, step_r;     // (4*lpr) / L and (4*lpr) % L: a lane's bucket cursor from one of its groups to the next
+    int lpr_log2;               // log2 of the lanes per row
+    int index_bytes;            // 4 or 8
+    int num_points;
+    float S;
+    bool words_aligned;         // packed 4-byte aligned: a code word inside the tensor is one load
+};
+
+// 32-bit code word w (bytes 4w .. 4w+3 of packed); bytes at or past in_bytes read as 0 and are never loaded
+__device__ __forceinline__ uint32_t pe_word(const PackedEmbeddingArgs& a, int64_t w) {
+    const int64_t b0 = 4 * w;
+    if (a.words_aligned && b0 + 4 <= a.in_bytes) return __ldg(reinterpret_cast<const unsigned int*>(a.packed) + w);
+    uint32_t v = 0;
+    for (int i = 0; i < 4; ++i)
+        if (b0 + i < a.in_bytes) v |= (uint32_t)__ldg(a.packed + b0 + i) << (8 * i);
+    return v;
+}
+
+template <bool UNIFORM, int BITS>
+__global__ void __launch_bounds__(kPeThreads) packed_embedding_kernel(PackedEmbeddingArgs a) {
+    constexpr unsigned mask = (1u << BITS) - 1u;
+    __shared__ float s_unit[256];
+    const int lpr = 1 << a.lpr_log2, step = 4 << a.lpr_log2;
+    const int sub = (int)threadIdx.x & (lpr - 1);
+    const int64_t i = ((int64_t)blockIdx.x * kPeThreads + threadIdx.x) >> a.lpr_log2;
+    int64_t r = 0;
+    if (i < a.count)                                        // in flight while the unit table is built
+        r = a.index_bytes == 8 ? (int64_t)__ldg(static_cast<const long long*>(a.indices) + i)
+                               : (int64_t)__ldg(static_cast<const int*>(a.indices) + i);
+    load_unit_table<UNIFORM>(s_unit, a.points, a.num_points, a.S);
+    __syncthreads();
+    // lpr is a power of two, so D of 9-12, 17-28, ... leaves lanes with no group in the row: their first element would
+    // lie past the row, its bucket past the scale arrays at the tensor's end
+    if (i >= a.count || 4 * sub >= a.D) return;
+    float* dst = a.out + i * a.D;
+    const bool vec = (reinterpret_cast<uintptr_t>(dst) & 15) == 0;
+    auto store = [&](int64_t c, const float (&o)[4]) {
+        if (vec && c + 4 <= a.D) {
+            *reinterpret_cast<float4*>(dst + c) = make_float4(o[0], o[1], o[2], o[3]);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                if (c + j < a.D) dst[c + j] = o[j];
+        }
+    };
+    if (r < 0 || r >= a.V) {
+        const float nan = __int_as_float(0x7fc00000);
+        const float o[4] = {nan, nan, nan, nan};
+        for (int64_t c = 4 * sub; c < a.D; c += step) store(c, o);
+        if (sub == 0 && a.invalid != nullptr) atomicAdd(a.invalid, 1);
+        return;
+    }
+    // what a group reads -- its one or two code words and the (alpha, beta) of its first bucket -- is fetched one group
+    // ahead, so that the loads of the next group are in flight while this one is decoded and stored
+    struct Fetched { uint32_t lo, hi; float al, be; };
+    auto fetch = [&](int64_t e, int64_t b, Fetched& f) {
+        const int64_t bit = e * BITS;
+        f.lo = pe_word(a, bit >> 5);
+        f.hi = (int)(bit & 31) + 4 * BITS > 32 ? pe_word(a, (bit >> 5) + 1) : 0u;
+        f.al = __ldg(a.alpha + b);
+        f.be = __ldg(a.beta + b);
+    };
+    int64_t e = r * a.D + 4 * sub;                          // first element of the lane's group
+    int64_t bg = e / a.L, rg = e - bg * a.L;                // its bucket and offset in it
+    Fetched cur;
+    fetch(e, bg, cur);
+    for (int64_t c = 4 * sub; c < a.D; c += step, e += step) {
+        int64_t nb = bg + a.step_q, nr = rg + a.step_r;     // the cursor of the lane's next group
+        if (nr >= a.L) { nr -= a.L; ++nb; }
+        Fetched nxt = cur;
+        if (c + step < a.D) fetch(e + step, nb, nxt);
+        const uint32_t codes = __funnelshift_r(cur.lo, cur.hi, (unsigned)(e * BITS) & 31u);
+        int64_t b = bg, rr = rg;
+        float al = cur.al, be = cur.be;
+        float o[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            o[j] = from_unit(s_unit[(codes >> (j * BITS)) & mask], al, be);
+            if (j < 3 && ++rr == a.L) {                     // the next element starts bucket b + 1
+                rr = 0;
+                b = min(b + 1, a.rows - 1);                 // past the last bucket only beyond the tensor's end
+                al = __ldg(a.alpha + b);
+                be = __ldg(a.beta + b);
+            }
+        }
+        store(c, o);
+        bg = nb;
+        rg = nr;
+        cur = nxt;
+    }
+}
+
+extern "C" int qd_packed_embedding(const void* indices, int index_bytes, int64_t count, int64_t num_embeddings, int64_t dim,
+                                   const uint8_t* packed, int bits, const float* alpha, const float* beta, const float* points,
+                                   int num_points, int levels, int64_t bucket, float* out, int32_t* invalid, qd_stream_t stream) {
+    if (indices == nullptr || packed == nullptr || alpha == nullptr || beta == nullptr || out == nullptr)
+        return fail(QD_ERR_INVALID_ARG, "NULL argument");
+    if (index_bytes != 4 && index_bytes != 8) return fail(QD_ERR_INVALID_ARG, "index_bytes must be 4 (int32) or 8 (int64), got %d", index_bytes);
+    if (count < 1 || num_embeddings < 1 || dim < 1) return fail(QD_ERR_INVALID_ARG, "count, num_embeddings and dim must be >= 1");
+    if (num_embeddings > INT64_MAX / 8 / dim) return fail(QD_ERR_INVALID_ARG, "num_embeddings * dim is too large");
+    if (count > INT64_MAX / 4 / dim) return fail(QD_ERR_INVALID_ARG, "count * dim overflows 64-bit indexing");
+    if (!bits_ok(bits)) return fail(QD_ERR_INVALID_ARG, "bits must be 1, 2, 4 or 8");
+    const bool uniform = levels != 0;
+    if (uniform) {
+        if (points != nullptr || num_points != 0) return fail(QD_ERR_INVALID_ARG, "uniform weights have no points (points NULL, num_points 0)");
+        if (levels < 2 || levels > (1 << bits)) return fail(QD_ERR_INVALID_ARG, "levels must be in [2, 2^bits]");
+    } else if (points == nullptr || num_points < 1 || num_points > (1 << bits)) {
+        return fail(QD_ERR_INVALID_ARG, "num_points must be in [1, 2^bits]");
+    }
+    Geometry geo;
+    const int64_t n = num_embeddings * dim;
+    if (geometry_of(n, bucket, &geo)) return fail(QD_ERR_INVALID_ARG, "bucket must be >= 0");
+    int lpr_log2 = 0;
+    while (lpr_log2 < 5 && (int64_t)4 << lpr_log2 < dim) ++lpr_log2;
+    const int64_t rows_per_cta = kPeThreads >> lpr_log2;
+    const int64_t ctas = (count + rows_per_cta - 1) / rows_per_cta;
+    if (ctas > INT32_MAX) return fail(QD_ERR_UNSUPPORTED, "%lld indices: more rows than one launch holds", (long long)count);
+    const uintptr_t ib = reinterpret_cast<uintptr_t>(indices), ie = ib + (uintptr_t)count * index_bytes;
+    const uintptr_t ob = reinterpret_cast<uintptr_t>(out), oe = ob + (uintptr_t)(count * dim) * sizeof(float);
+    if (ib < oe && ob < ie) return fail(QD_ERR_INVALID_ARG, "out must not overlap the indices");
+    PackedEmbeddingArgs a{};
+    a.indices = indices, a.packed = packed, a.alpha = alpha, a.beta = beta, a.points = points, a.out = out, a.invalid = invalid;
+    a.count = count, a.V = num_embeddings, a.D = dim;
+    a.in_bytes = (n * bits + 7) / 8;
+    a.L = geo.row_len, a.rows = geo.rows;
+    a.step_q = ((int64_t)4 << lpr_log2) / a.L, a.step_r = ((int64_t)4 << lpr_log2) % a.L;
+    a.lpr_log2 = lpr_log2;
+    a.index_bytes = index_bytes;
+    a.num_points = num_points;
+    a.S = uniform ? (float)(levels - 1) : 0.f;
+    a.words_aligned = (reinterpret_cast<uintptr_t>(packed) & 3) == 0;
+    cudaStream_t st = as_stream(stream);
+    with_bits(bits, [&](auto b) {
+        if (uniform) packed_embedding_kernel<true, b><<<(unsigned)ctas, kPeThreads, 0, st>>>(a);
+        else packed_embedding_kernel<false, b><<<(unsigned)ctas, kPeThreads, 0, st>>>(a);
+    });
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
 // ------------------------------------------------------------------ f2: Huffman-coded storage (qd_huffman.cuh)
 extern "C" int qd_huffman_encode(const uint8_t* idx_u8, int64_t n, const qd_huffman_table* table, uint32_t* words_out,
                                  int64_t words_capacity, uint32_t* chunk_offsets, uint64_t* total_words, qd_stream_t stream) {

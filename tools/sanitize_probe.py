@@ -2,8 +2,12 @@
 import os
 import sys
 
-import numpy as np
-import torch
+# every tensor in its own cudaMalloc, so that memcheck sees its exact bounds: the caching allocator would place small
+# tensors inside larger segments, where a read past one tensor's end lands in memory the process owns
+os.environ.setdefault("PYTORCH_NO_CUDA_MEMORY_CACHING", "1")
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -83,5 +87,24 @@ for pinned in (True, False):
         hx, hg, hq, hgo = hx.pin_memory(), hg.pin_memory(), hq.pin_memory(), hgo.pin_memory()
     N.check(N.lib().qd_uniform_fwd_bwd_host(N.ptr(hx), N.ptr(hg), N.ptr(hq), N.ptr(hgo), m, 256, 16, N.BWD_MINMAX, 0))
     assert torch.equal(hq, Q.uniformQuantization(hx.cuda(), 16, bucket_size=256)[0].cpu())
+# packed embedding lookup: odd rows starting inside a byte at 1 / 2 / 4 bits, the tensor's last code byte, an output
+# 4 bytes off a 16-byte boundary, codes 1 byte off a word, out-of-range indices; widths 9 and 48 leave lanes of a row
+# without a group, on tables that end exactly at a bucket's end (9 x 100 at bucket 100, 25 x 48 at bucket 100, 11 x 9
+# at bucket None); bucket 3 is shorter than a lane's group
+for bits, V, D, bucket in ((1, 37, 7, 100), (2, 50, 3, 100), (4, 9, 31, 100), (8, 5, 257, 100), (2, 100, 9, 100),
+                           (4, 25, 48, 100), (2, 11, 9, None), (4, 40, 5, 3)):
+    s_levels = 1 << bits
+    pe = codec.pack_model(torch.nn.Embedding(V, D).cuda(), bits, bucket).tensors[0]   # numBits = bits: 2^bits levels
+    emb = codec.PackedEmbedding(pe, "uniform", s_levels, bucket)
+    idx = torch.tensor([V - 1, 0, -1, V, V - 1, 3 % V], device="cuda")
+    want = emb.decoded_weight()[idx.clamp(0, V - 1)]
+    ok = (idx >= 0) & (idx < V)
+    assert torch.equal(emb(idx)[ok], want[ok]) and emb.invalid_index_count() == 2
+    buf = torch.empty(idx.numel() * D + 1, device="cuda")
+    shifted = torch.zeros(emb.packed.numel() + 1, dtype=torch.uint8, device="cuda")
+    shifted[1:] = emb.packed
+    N.check(N.lib().qd_packed_embedding(N.ptr(idx), 8, idx.numel(), V, D, N.ptr(shifted) + 1, bits, N.ptr(emb.alpha), N.ptr(emb.beta),
+                                        None, 0, s_levels, bucket or 0, N.ptr(buf) + 4, None, N.stream_ptr()))
+    assert torch.equal(buf[1:].view(-1, D)[ok], want[ok])
 torch.cuda.synchronize()
 print("sanitize probe ok")
