@@ -240,6 +240,40 @@ int qd_packed_embedding(const void* indices, int index_bytes, int64_t count, int
                         const uint8_t* packed, int bits, const float* alpha, const float* beta, const float* points,
                         int num_points, int levels, int64_t bucket, float* out, int32_t* invalid, qd_stream_t stream);
 
+/* One LSTM step on packed weights for m rows (1 <= m <= QD_PACKED_LSTM_MAX_ROWS; larger m is QD_ERR_UNSUPPORTED):
+ * x float32[m, I] (row stride ldx >= I), h float32[m, H] (stride ldh >= H), c float32[m, H] (C order); w_ih and w_hh
+ * describe the packed [4H, I] and [4H, H] weights (HOST structs holding device pointers; n must be 4*H*I and 4*H*H,
+ * each its own bits and, non-uniform, its own points; q is not read), decoded as qd_unpack_dequant_* decodes them at
+ * the model's levels and bucket; b_ih and b_hh float32[4H] may be NULL.  Gate order is torch's: i, f, g, o (rows j,
+ * H+j, 2H+j, 3H+j of each weight for hidden unit j).  Writes h_out[m, H] (stride ldo >= H) and c_out[m, H].
+ * Numerical contract: with S_ih and S_hh the sums qd_packed_linear forms (so S_ih + b_ih is bit for bit
+ * qd_packed_linear(x, W_ih, b_ih) and S_hh is qd_packed_linear(h, W_hh, NULL)), each gate's preactivation is
+ * ((S_ih + b_ih) + S_hh) + b_hh in float32 (a NULL bias is not added); then c' = (sig(f)*c) + (sig(i)*tanh(g)) and
+ * h' = sig(o)*tanh(c'), sig(z) = 1/(1 + expf(-z)), every op rounded to float32 in that order (IEEE expf / tanhf, no
+ * contraction).  The order depends on (I, H, bits) alone: a row gives the same bits alone or in any batch, on any
+ * stream, in any replay.  c_out may be exactly c (each element is read and written by one thread) but must not overlap
+ * it otherwise; h_out must not overlap x, h, c or c_out, nor c_out x or h.  QD_ERR_INVALID_ARG: NULL pointers, sizes
+ * below 1, strides below the rows, bits too narrow for levels or points, the overlaps above.  No workspace; only
+ * enqueues work on `stream` (graph-capturable). */
+#define QD_PACKED_LSTM_MAX_ROWS 64
+int qd_packed_lstm_cell(const float* x, int64_t ldx, const float* h, int64_t ldh, const float* c, int64_t m, int64_t input_size,
+                        int64_t hidden_size, const qd_packed_tensor* w_ih, const qd_packed_tensor* w_hh, int levels, int64_t bucket,
+                        const float* b_ih, const float* b_hh, float* h_out, int64_t ldo, float* c_out, qd_stream_t stream);
+/* One LSTM layer in one direction over `steps` steps, one qd_packed_lstm_cell launch per step enqueued from a C loop
+ * (no host synchronisation: graph-capturable).  batch_sizes: HOST int64[steps], non-increasing, >= 1, the first at
+ * most QD_PACKED_LSTM_MAX_ROWS (PackedSequence layout; a padded batch passes `steps` equal entries).  Step t reads x
+ * rows and writes out rows at its offset sum(batch_sizes[0..t-1]) in the packed data (strides ldx >= I, ldo >= H: a
+ * bidirectional layer writes its half of a [., 2H] output).  reverse != 0 runs the steps T-1 .. 0.  h0, c0, h_n, c_n:
+ * float32[batch_sizes[0], H], C order.  A row's previous h is the previous step's out row when the row was active
+ * there, else its h0 row; c_n is first set from c0 (a stream-ordered copy, none when c_n == c0), then updated in place
+ * (rows inactive at a step are left untouched); a row's h_n is written by its last step.  Arithmetic as
+ * qd_packed_lstm_cell.  QD_ERR_INVALID_ARG as there, plus batch sizes that increase or are below 1, and out, h_n or
+ * c_n overlapping x, h0 or each other (c_n may be c0). */
+int qd_packed_lstm_layer(const float* x, int64_t ldx, const int64_t* batch_sizes, int64_t steps, int reverse, int64_t input_size,
+                         int64_t hidden_size, const qd_packed_tensor* w_ih, const qd_packed_tensor* w_hh, int levels, int64_t bucket,
+                         const float* b_ih, const float* b_hh, const float* h0, const float* c0, float* out, int64_t ldo,
+                         float* h_n, float* c_n, qd_stream_t stream);
+
 /* ---- next row f2: Huffman-coded storage (the model helpers/functions.py:226-262 only sizes) ----------
  * Canonical code over uint8 symbols, codes of 1..QD_HUFFMAN_MAX_LENGTH bits (built on the host: codec.py).
  * Stream: a tensor's symbols are cut into chunks of QD_HUFFMAN_CHUNK; each chunk's codes are written MSB-first

@@ -1184,6 +1184,246 @@ class PackedEmbedding(torch.nn.Module):
         return out
 
 
+class _PackedWeight(torch.nn.Module):
+    """One packed [rows, cols] weight matrix of a recurrent module and the bias that goes with it, held as the sections
+    _hold_sections registers (packed, alpha, beta, points, bias)."""
+
+    def __init__(self, entry: PackedEntry, kind: str, levels, bucket_size, bias, rows: int, cols: int):
+        super().__init__()
+        if not entry.quantized or tuple(entry.shape) != (rows, cols):
+            raise ValueError(f"{entry.name}: expected a quantized [{rows}, {cols}] weight, got {tuple(entry.shape)}"
+                             f"{'' if entry.quantized else ' kept float32'}")
+        self.shape = (rows, cols)
+        _hold_sections(self, entry, kind, levels, bucket_size, bias, rows)
+
+    def decoded(self) -> torch.Tensor:
+        return _decoded(self, self.shape)
+
+    def descriptor(self) -> np.ndarray:
+        """The host qd_packed_tensor of the weight (q NULL: the LSTM entry points do not write one)."""
+        d = np.zeros(1, _PACKED_TENSOR)
+        d[0] = (N.ptr(self.packed), N.ptr(self.alpha), N.ptr(self.beta), 0 if self.points is None else N.ptr(self.points), 0,
+                self.shape[0] * self.shape[1], self.bits, 0 if self.points is None else self.points.numel())
+        return d
+
+
+def _check_weights(weights, x, what: str) -> None:
+    for w in weights:
+        _check_input(w, x, what)
+        _check_state(w, x, what)
+
+
+def _lstm_pair(entry_ih, entry_hh, kind, levels, bucket_size, bias_ih, bias_hh, hidden_size, input_size) -> torch.nn.ModuleList:
+    return torch.nn.ModuleList([_PackedWeight(entry_ih, kind, levels, bucket_size, bias_ih, 4 * hidden_size, input_size),
+                                _PackedWeight(entry_hh, kind, levels, bucket_size, bias_hh, 4 * hidden_size, hidden_size)])
+
+
+class PackedLSTMCell(torch.nn.Module):
+    """Inference replacement of an ``nn.LSTMCell`` whose two weight matrices stay in their fixed-width stored form (two
+    PackedEntry of a PackedModel, [4H, I] and [4H, H]) on the device.  Takes input [B, I] or [I] and ``hx`` = (h, c) or
+    None (zeros), returns (h', c') in nn.LSTMCell's shapes.  Up to CROSSOVER_ROWS rows (none by default), forward runs
+    qd_packed_lstm_cell: one launch that reads the codes of both weights and applies the cell update in registers,
+    every weight bit for bit the decoded one, each gate's sum in qd_packed_linear's fixed float32 order (include/qd_b200.h
+    states the contract).  Larger batches decode both weights into scratch tensors and call torch's LSTM cell: exactly
+    what an unpack_-loaded nn.LSTMCell computes.  Forward only, no host synchronisation (graph-capturable)."""
+    # largest batch that runs on the packed kernel (at most N.PACKED_LSTM_MAX_ROWS).  Measured (DESIGN.md section
+    # 3.7.6): on the NMT decoder cells the kernel loses to decode + torch at batch 1, 5, 30 and 64 (35.7 against
+    # 21.7 us per step at batch 1, 1000 -> 500), so by default every batch decodes.
+    CROSSOVER_ROWS = 0
+
+    def __init__(self, entry_ih: PackedEntry, entry_hh: PackedEntry, kind: str, levels, bucket_size, bias_ih: torch.Tensor = None,
+                 bias_hh: torch.Tensor = None):
+        super().__init__()
+        if len(entry_ih.shape) != 2 or entry_ih.shape[0] % 4 or entry_ih.shape[0] < 4:
+            raise ValueError(f"{entry_ih.name}: an LSTM input weight is [4 * hidden_size, input_size], got {tuple(entry_ih.shape)}")
+        self.hidden_size, self.input_size = int(entry_ih.shape[0]) // 4, int(entry_ih.shape[1])
+        self.bias = bias_ih is not None or bias_hh is not None
+        self.weights = _lstm_pair(entry_ih, entry_hh, kind, levels, bucket_size, bias_ih, bias_hh, self.hidden_size, self.input_size)
+
+    def extra_repr(self) -> str:
+        ih = self.weights[0]
+        return f"{self.input_size}, {self.hidden_size}, bias={self.bias}, {ih.kind}, bits={ih.bits}/{self.weights[1].bits}, bucket_size={ih.bucket_size}"
+
+    def decoded_weights(self) -> tuple:
+        """(weight_ih, weight_hh) decoded to float32, bit for bit what unpack_ writes."""
+        return self.weights[0].decoded(), self.weights[1].decoded()
+
+    def forward(self, input: torch.Tensor, hx=None) -> tuple:
+        _check_weights(self.weights, input, "PackedLSTMCell")
+        if input.dim() not in (1, 2) or input.shape[-1] != self.input_size:
+            raise ValueError(f"input of shape {tuple(input.shape)}, expected (B, {self.input_size}) or ({self.input_size},)")
+        batched = input.dim() == 2
+        x = input if batched else input.unsqueeze(0)
+        B, H = x.shape[0], self.hidden_size
+        if hx is None:
+            h = c = torch.zeros(B, H, dtype=torch.float32, device=x.device)
+        else:
+            h, c = hx
+            for t in (h, c):
+                _check_weights(self.weights, t, "PackedLSTMCell")
+                if tuple(t.shape) != ((B, H) if batched else (H,)):
+                    raise ValueError(f"hidden state of shape {tuple(t.shape)}, expected {(B, H) if batched else (H,)}")
+            h, c = (h, c) if batched else (h.unsqueeze(0), c.unsqueeze(0))
+        ih, hh = self.weights
+        with torch.cuda.device(x.device):
+            if B == 0 or B > self.CROSSOVER_ROWS:
+                w_ih, w_hh = self.decoded_weights()
+                h1, c1 = torch._VF.lstm_cell(x, (h, c), w_ih, w_hh, ih.bias, hh.bias)
+            else:
+                x, h = (t if t.stride(-1) == 1 and t.stride(0) >= t.shape[1] else t.contiguous() for t in (x, h))
+                c = c.contiguous()
+                h1 = torch.empty(B, H, dtype=torch.float32, device=x.device)
+                c1 = torch.empty(B, H, dtype=torch.float32, device=x.device)
+                d_ih, d_hh = ih.descriptor(), hh.descriptor()
+                N.check(N.lib().qd_packed_lstm_cell(N.ptr(x), x.stride(0), N.ptr(h), h.stride(0), N.ptr(c), B, self.input_size, H,
+                                                    d_ih.ctypes.data, d_hh.ctypes.data, ih.levels,
+                                                    _bucket(ih.bucket_size), N.ptr(ih.bias), N.ptr(hh.bias), N.ptr(h1), H, N.ptr(c1),
+                                                    N.stream_ptr(x.device)))
+        return (h1, c1) if batched else (h1[0], c1[0])
+
+
+class PackedLSTM(torch.nn.Module):
+    """Inference replacement of an ``nn.LSTM`` (no projection) whose weight matrices stay in their fixed-width stored
+    form on the device: ``weights`` is one (entry_ih, entry_hh) pair per layer and direction in nn.LSTM's order (l0,
+    l0_reverse, l1, ...), ``biases`` the matching (bias_ih, bias_hh) pairs or None.  Takes what nn.LSTM takes -- padded
+    3-D input (batch_first or not), unbatched 2-D input, or a PackedSequence (sorted or not), with ``hx`` = (h_0, c_0)
+    or None -- and returns (output, (h_n, c_n)) in nn.LSTM's shapes.  For batches of up to CROSSOVER_ROWS rows (none by
+    default), every
+    layer and direction is one qd_packed_lstm_layer call (one fused cell launch per step, no host synchronisation, so
+    the forward can be captured in a CUDA graph); the arithmetic is qd_packed_lstm_cell's, so a sequence gives the same
+    bits alone, inside any batch and at any position of a PackedSequence.  Larger batches decode every weight and call
+    torch's LSTM: exactly what an unpack_-loaded nn.LSTM computes.  Inter-layer dropout is not applied: in training
+    mode with dropout > 0 and several layers forward raises, since the result would differ from nn.LSTM's."""
+    # largest batch that runs on qd_packed_lstm_layer (at most N.PACKED_LSTM_MAX_ROWS).  Measured (DESIGN.md section
+    # 3.7.6): on the NMT encoder layer the kernel loses to decode + torch at batch 1, 5, 30 and 64, so by default every
+    # batch decodes.
+    CROSSOVER_ROWS = 0
+
+    def __init__(self, weights, kind: str, levels, bucket_size, *, num_layers=1, batch_first=False, dropout=0.0, bidirectional=False,
+                 biases=None):
+        super().__init__()
+        dirs = 2 if bidirectional else 1
+        if num_layers < 1 or len(weights) != num_layers * dirs:
+            raise ValueError(f"{len(weights)} weight pairs for {num_layers} layers x {dirs} directions")
+        if biases is not None and len(biases) != len(weights):
+            raise ValueError(f"{len(biases)} bias pairs for {len(weights)} weight pairs")
+        first = weights[0][0]
+        if len(first.shape) != 2 or first.shape[0] % 4 or first.shape[0] < 4:
+            raise ValueError(f"{first.name}: an LSTM input weight is [4 * hidden_size, input_size], got {tuple(first.shape)}")
+        self.hidden_size, self.input_size = int(first.shape[0]) // 4, int(first.shape[1])
+        self.num_layers, self.batch_first, self.dropout, self.bidirectional = num_layers, batch_first, float(dropout), bidirectional
+        self.bias = biases is not None
+        self.cells = torch.nn.ModuleList()
+        for k, (e_ih, e_hh) in enumerate(weights):
+            b_ih, b_hh = biases[k] if biases is not None else (None, None)
+            in_size = self.input_size if k < dirs else dirs * self.hidden_size
+            self.cells.append(_lstm_pair(e_ih, e_hh, kind, levels, bucket_size, b_ih, b_hh, self.hidden_size, in_size))
+
+    def extra_repr(self) -> str:
+        ih = self.cells[0][0]
+        return (f"{self.input_size}, {self.hidden_size}, num_layers={self.num_layers}, bias={self.bias}, batch_first={self.batch_first}, "
+                f"dropout={self.dropout}, bidirectional={self.bidirectional}, {ih.kind}, bucket_size={ih.bucket_size}")
+
+    def decoded_weights(self) -> list:
+        """nn.LSTM's flat weight list (w_ih, w_hh[, b_ih, b_hh] per layer and direction), the matrices decoded to float32 bit
+        for bit as unpack_ writes them."""
+        flat = []
+        for ih, hh in self.cells:
+            flat += [ih.decoded(), hh.decoded()] + ([ih.bias, hh.bias] if self.bias else [])
+        return flat
+
+    def forward(self, input, hx=None):
+        packed_in = isinstance(input, torch.nn.utils.rnn.PackedSequence)
+        weights = [w for pair in self.cells for w in pair]
+        x = input.data if packed_in else input
+        _check_weights(weights, x, "PackedLSTM")
+        if self.training and self.dropout > 0 and self.num_layers > 1:
+            raise RuntimeError("PackedLSTM does not apply inter-layer dropout: call eval(), or set dropout to 0")
+        dirs, H, L = 2 if self.bidirectional else 1, self.hidden_size, self.num_layers
+        if packed_in:
+            if x.dim() != 2 or x.shape[1] != self.input_size:
+                raise ValueError(f"PackedSequence data of shape {tuple(x.shape)}, expected (N, {self.input_size})")
+            batch_sizes = input.batch_sizes
+            B, batched = int(batch_sizes[0]), True
+        else:
+            if x.dim() not in (2, 3) or x.shape[-1] != self.input_size:
+                raise ValueError(f"input of shape {tuple(x.shape)}, expected 3-D or 2-D with {self.input_size} features")
+            batched = x.dim() == 3
+            batch_dim = 0 if self.batch_first else 1
+            if not batched:
+                x = x.unsqueeze(batch_dim)
+            B = x.shape[batch_dim]
+        if hx is None:
+            h0 = torch.zeros(L * dirs, B, H, dtype=torch.float32, device=x.device)
+            c0 = torch.zeros_like(h0)
+        else:
+            h0, c0 = hx
+            for t in (h0, c0):
+                _check_weights(weights, t, "PackedLSTM")
+                if tuple(t.shape) != ((L * dirs, B, H) if batched else (L * dirs, H)):
+                    raise ValueError(f"hidden state of shape {tuple(t.shape)}, expected {(L * dirs, B, H) if batched else (L * dirs, H)}")
+            if not batched:
+                h0, c0 = h0.unsqueeze(1), c0.unsqueeze(1)
+            if packed_in and input.sorted_indices is not None:         # nn.LSTM's permute_hidden
+                h0, c0 = h0.index_select(1, input.sorted_indices), c0.index_select(1, input.sorted_indices)
+        with torch.cuda.device(x.device):
+            if B == 0 or x.numel() == 0 or B > self.CROSSOVER_ROWS:
+                out, h_n, c_n = self._decoded_forward(x, batch_sizes if packed_in else None, h0, c0)
+            else:
+                out, h_n, c_n = self._packed_forward(x, batch_sizes if packed_in else None, h0, c0)
+        if packed_in:
+            if input.unsorted_indices is not None:
+                h_n, c_n = h_n.index_select(1, input.unsorted_indices), c_n.index_select(1, input.unsorted_indices)
+            return torch.nn.utils.rnn.PackedSequence(out, batch_sizes, input.sorted_indices, input.unsorted_indices), (h_n, c_n)
+        if not batched:
+            out, h_n, c_n = out.squeeze(batch_dim), h_n.squeeze(1), c_n.squeeze(1)
+        return out, (h_n, c_n)
+
+    def _decoded_forward(self, x, batch_sizes, h0, c0):
+        import warnings
+        flat = self.decoded_weights()
+        with warnings.catch_warnings():       # the decoded weights are not one flattened buffer; cuDNN copies them into one
+            warnings.filterwarnings("ignore", message="RNN module weights are not part of single contiguous chunk")
+            if batch_sizes is not None:
+                out, h_n, c_n = torch._VF.lstm(x, batch_sizes, (h0, c0), flat, self.bias, self.num_layers, self.dropout, self.training,
+                                               self.bidirectional)
+            else:
+                out, h_n, c_n = torch._VF.lstm(x, (h0, c0), flat, self.bias, self.num_layers, self.dropout, self.training,
+                                               self.bidirectional, self.batch_first)
+        return out, h_n, c_n
+
+    def _packed_forward(self, x, batch_sizes, h0, c0):
+        dirs, H = 2 if self.bidirectional else 1, self.hidden_size
+        if batch_sizes is not None:
+            bs = np.ascontiguousarray(batch_sizes.cpu().numpy(), dtype=np.int64)
+            data = x
+        else:
+            seq = x.transpose(0, 1) if self.batch_first else x               # (T, B, I)
+            bs = np.full(seq.shape[0], seq.shape[1], dtype=np.int64)
+            data = seq.reshape(-1, self.input_size)
+        if data.stride(-1) != 1:
+            data = data.contiguous()
+        h0, c0 = h0.contiguous(), c0.contiguous()
+        h_n, c_n = torch.empty_like(h0), torch.empty_like(c0)
+        rows, sp = data.shape[0], N.stream_ptr(data.device)
+        for layer in range(self.num_layers):
+            out = torch.empty(rows, dirs * H, dtype=torch.float32, device=data.device)
+            for d in range(dirs):
+                k = layer * dirs + d
+                ih, hh = self.cells[k]
+                d_ih, d_hh = ih.descriptor(), hh.descriptor()
+                N.check(N.lib().qd_packed_lstm_layer(N.ptr(data), data.stride(0), bs.ctypes.data, len(bs), d, ih.shape[1], H,
+                                                     d_ih.ctypes.data, d_hh.ctypes.data, ih.levels,
+                                                     _bucket(ih.bucket_size), N.ptr(ih.bias), N.ptr(hh.bias), N.ptr(h0[k]), N.ptr(c0[k]),
+                                                     N.ptr(out) + 4 * d * H, dirs * H, N.ptr(h_n[k]), N.ptr(c_n[k]), sp))
+            data = out
+        if batch_sizes is None:
+            data = data.view(len(bs), -1, dirs * H)
+            if self.batch_first:
+                data = data.transpose(0, 1).contiguous()
+        return data, h_n, c_n
+
+
 def _conv_padding(conv) -> tuple:
     """(pad_h, pad_w) of an nn.Conv2d's padding when it is symmetric: an int pair, "valid", or "same" whose total
     padding per side is even; None otherwise."""
@@ -1213,17 +1453,53 @@ def _embedding_target(mod) -> bool:
     return type(mod) is torch.nn.Embedding and mod.max_norm is None
 
 
-def _packed_linear(entry, pm, lin):
-    return PackedLinear(entry, pm.kind, pm.levels, pm.bucket_size, None if lin.bias is None else lin.bias.data)
+def _packed_linear(entries, pm, lin):
+    return PackedLinear(entries[0], pm.kind, pm.levels, pm.bucket_size, None if lin.bias is None else lin.bias.data)
 
 
-def _packed_conv(entry, pm, conv):
-    return PackedConv2d(entry, pm.kind, pm.levels, pm.bucket_size, conv.stride, _conv_padding(conv),
+def _packed_conv(entries, pm, conv):
+    return PackedConv2d(entries[0], pm.kind, pm.levels, pm.bucket_size, conv.stride, _conv_padding(conv),
                         None if conv.bias is None else conv.bias.data)
 
 
-def _packed_embedding(entry, pm, emb):
-    return PackedEmbedding(entry, pm.kind, pm.levels, pm.bucket_size, emb.padding_idx)
+def _packed_embedding(entries, pm, emb):
+    return PackedEmbedding(entries[0], pm.kind, pm.levels, pm.bucket_size, emb.padding_idx)
+
+
+def _lstm_target(mod) -> bool:
+    return type(mod) is torch.nn.LSTM and mod.proj_size == 0
+
+
+def _lstm_cell_target(mod) -> bool:
+    return type(mod) is torch.nn.LSTMCell
+
+
+def _own_bias(b):
+    # a copy: on CUDA an nn.LSTM's parameters are views into one flattened buffer, which must not outlive the module
+    return None if b is None else b.data.clone()
+
+
+def _packed_lstm(entries, pm, lstm):
+    biases = None
+    if lstm.bias:
+        names = [n for n in lstm._flat_weights_names if n.startswith("bias")]
+        biases = [(_own_bias(getattr(lstm, a)), _own_bias(getattr(lstm, b))) for a, b in zip(names[0::2], names[1::2])]
+    return PackedLSTM(list(zip(entries[0::2], entries[1::2])), pm.kind, pm.levels, pm.bucket_size, num_layers=lstm.num_layers,
+                      batch_first=lstm.batch_first, dropout=lstm.dropout, bidirectional=lstm.bidirectional, biases=biases)
+
+
+def _packed_lstm_cell(entries, pm, cell):
+    return PackedLSTMCell(entries[0], entries[1], pm.kind, pm.levels, pm.bucket_size, _own_bias(cell.bias_ih), _own_bias(cell.bias_hh))
+
+
+def _weight_matrices(mod) -> list:
+    """The weights a packed replacement of ``mod`` holds: an LSTM's (ih, hh) per layer and direction in nn.LSTM's order,
+    an LSTMCell's (ih, hh), else the module's one weight."""
+    if isinstance(mod, torch.nn.LSTM):
+        return [getattr(mod, n) for n in mod._flat_weights_names if n.startswith("weight")]
+    if isinstance(mod, torch.nn.LSTMCell):
+        return [mod.weight_ih, mod.weight_hh]
+    return [mod.weight]
 
 
 def _tied_pair(mods) -> bool:
@@ -1235,9 +1511,10 @@ def _tied_pair(mods) -> bool:
 
 def _attach(pm: PackedModel, model, kinds, tied=False) -> list:
     """unpack_, except that every module accepted by the ``accept`` of one of ``kinds`` -- (accept, make, what) -- whose
-    weight ``pm`` stores quantized and which is that weight's only holder is replaced in its parent by make(entry, pm,
-    module); the float32 weight is released.  With ``tied``, so are both modules of a tied embedding / generator pair
-    (_tied_pair), and the two share one set of device sections.  Returns the names of the replaced modules."""
+    weight matrices (_weight_matrices) ``pm`` all stores quantized and which is each one's only holder is replaced in
+    its parent by make(entries, pm, module), one entry per matrix; the float32 matrices are released.  With ``tied``,
+    so are both modules of a tied embedding / generator pair (_tied_pair), and the two share one set of device sections.
+    Returns the names of the replaced modules."""
     named, bufs = _check_target(pm, model)
     index = {id(p): k for k, (_, p) in enumerate(named)}
     holders = {}                                 # parameter -> its registrations in the module tree, every path counted
@@ -1245,28 +1522,35 @@ def _attach(pm: PackedModel, model, kinds, tied=False) -> list:
         for p in mod._parameters.values():
             if p is not None:
                 holders.setdefault(id(p), []).append(mod)
-    targets = []                                 # (module name, parent, attribute, module, weight index, make)
+
+    def eligible(ws):
+        return all(id(w) in index and pm.tensors[index[id(w)]].quantized for w in ws) and \
+            (all(len(holders[id(w)]) == 1 for w in ws) or tied and len(ws) == 1 and _tied_pair(holders[id(ws[0])]))
+    targets = []                                 # (module name, parent, attribute, module, weight indices, make)
     for mname, mod in model.named_modules():
         for accept, make, what in kinds:
-            if accept(mod) and id(mod.weight) in index and pm.tensors[index[id(mod.weight)]].quantized \
-                    and (len(holders[id(mod.weight)]) == 1 or tied and _tied_pair(holders[id(mod.weight)])):
-                if not mod.weight.is_cuda:
-                    raise ValueError(f"{mname}: a Packed{what} runs on a CUDA device, the {what} is on {mod.weight.device}")
+            if accept(mod) and eligible(ws := _weight_matrices(mod)):
+                if not ws[0].is_cuda:
+                    raise ValueError(f"{mname}: a Packed{what} runs on a CUDA device, the {what} is on {ws[0].device}")
                 parent_name, _, attr = mname.rpartition(".")
-                targets.append((mname, model.get_submodule(parent_name) if parent_name else model, attr, mod, index[id(mod.weight)], make))
+                targets.append((mname, model.get_submodule(parent_name) if parent_name else model, attr, mod,
+                                [index[id(w)] for w in ws], make))
                 break
-    _write_into(pm, named, bufs, skip={t[4] for t in targets})
+    _write_into(pm, named, bufs, skip={k for t in targets for k in t[4]})
     movers = {}
     held = {}                                    # weight index -> the sections its first replacement holds
-    for mname, parent, attr, mod, k, make in targets:
-        dev = mod.weight.device
-        t = pm.tensors[k]
+    for mname, parent, attr, mod, ks, make in targets:
+        dev = _weight_matrices(mod)[0].device
         with torch.cuda.device(dev):
             move = movers.setdefault(dev, _mover(pm, dev))
-            entry = held.get(k) or PackedEntry(t.name, t.shape, bits=t.bits, packed=move(t.packed), alpha=move(t.alpha),
-                                               beta=move(t.beta), points=None if t.points is None else t.points.to(dev))
-            layer = make(entry, pm, mod)
-        held[k] = PackedEntry(t.name, t.shape, bits=t.bits, packed=layer.packed, alpha=layer.alpha, beta=layer.beta, points=layer.points)
+            entries = [held.get(k) or PackedEntry(t.name, t.shape, bits=t.bits, packed=move(t.packed), alpha=move(t.alpha),
+                                                  beta=move(t.beta), points=None if t.points is None else t.points.to(dev))
+                       for k, t in ((k, pm.tensors[k]) for k in ks)]
+            layer = make(entries, pm, mod)
+        if len(ks) == 1:
+            t = pm.tensors[ks[0]]
+            held[ks[0]] = PackedEntry(t.name, t.shape, bits=t.bits, packed=layer.packed, alpha=layer.alpha, beta=layer.beta,
+                                      points=layer.points)
         setattr(parent, attr, layer)
     return [t[0] for t in targets]
 
@@ -1283,7 +1567,7 @@ def attach_packed_linear_(pm: PackedModel, model) -> list:
     return _attach(pm, model, [(_linear_target, _packed_linear, "Linear")])
 
 
-def attach_packed_(pm: PackedModel, model, *, embeddings=False) -> list:
+def attach_packed_(pm: PackedModel, model, *, embeddings=False, recurrent=False) -> list:
     """attach_packed_linear_ for Linear and convolution layers: every nn.Linear it would replace becomes a
     PackedLinear, and every ``nn.Conv2d`` (the class itself, not a subclass) with groups 1, dilation 1, zero padding
     that is symmetric (int padding, "valid", or "same" that resolves to equal sides) and a weight ``pm`` stores
@@ -1294,10 +1578,17 @@ def attach_packed_(pm: PackedModel, model, *, embeddings=False) -> list:
     Linear's bias) that share one copy of the sections on the device.  Any other weight with several holders is
     decoded as unpack_ decodes it.  The replaced float32 weights are released; every other parameter and layer, and the
     stored buffers, are written exactly as unpack_ writes them, quantized tensors in one launch per device.  Everything
-    is checked before anything is written.  Returns the names of the replaced modules, in module order."""
+    is checked before anything is written.  With ``recurrent=True``, also every ``nn.LSTM`` (the class itself) without
+    projection becomes a PackedLSTM, and every ``nn.LSTMCell`` a PackedLSTMCell, when ``pm`` stores all of its weight
+    matrices quantized and it alone holds each of them; its biases are written as unpack_ writes them and handed to the
+    packed module (as copies: nothing keeps an LSTM's flattened weight buffer alive).  Every other recurrent module -- a
+    GRU, a subclass, one with a shared or float32 matrix -- is decoded as unpack_ decodes it.  Returns the names of the
+    replaced modules, in module order."""
     kinds = [(_linear_target, _packed_linear, "Linear"), (_conv_target, _packed_conv, "Conv2d")]
     if embeddings:
         kinds.append((_embedding_target, _packed_embedding, "Embedding"))
+    if recurrent:
+        kinds += [(_lstm_target, _packed_lstm, "LSTM"), (_lstm_cell_target, _packed_lstm_cell, "LSTMCell")]
     return _attach(pm, model, kinds, tied=embeddings)
 
 

@@ -6,6 +6,7 @@
 
 #include "qd_huffman.cuh"
 #include "qd_launch.h"
+#include "qd_packed_walk.cuh"
 
 using namespace qd;
 
@@ -180,14 +181,6 @@ extern "C" int qd_unpack_indices(const uint8_t* packed, int bits, uint8_t* idx_u
     with_bits(bits, [&](auto b) { unpack_indices_kernel<b><<<grid, 256, 0, as_stream(stream)>>>(packed, idx_u8, n); });
     QD_CUDA(cudaGetLastError());
     return QD_OK;
-}
-
-template <bool UNIFORM>
-__device__ __forceinline__ void load_unit_table(float* s_unit, const float* __restrict__ points, int K, float S) {
-    for (int i = threadIdx.x; i < 256; i += blockDim.x) {
-        if (UNIFORM) s_unit[i] = ((float)i <= S) ? level_to_unit((float)i, S) : 0.f;
-        else s_unit[i] = (i < K) ? points[i] : 0.f;
-    }
 }
 
 // The element loop of one tensor's unpack, as CTA `block` of the `nblocks` CTAs that serve the tensor: the per-tensor
@@ -418,22 +411,14 @@ extern "C" int qd_unpack_dequant_model(const qd_packed_tensor* tensors, int coun
 // y[i, o] = sum_k x[i, k] * q[o*K + k] (+ bias[o]) where q is the tensor qd_unpack_dequant_* writes: every weight is
 // from_unit(unit[code], alpha[bucket], beta[bucket]) with the unit table of load_unit_table.
 //
-// A warp owns four consecutive output features and walks their rows together, so that one shared-memory read of x
-// feeds four weight rows.  A row is cut into quads of 4*E codes (E = 32/BITS per 32-bit word; quad d holds columns
-// 4*E*d .. 4*E*d+4*E-1, one 128-bit load when rows start on 16-byte boundaries); lane L takes quads L, L+32, ... in
-// increasing order and sums its elements in column order, one fmaf per element and x row, then the warp folds its
-// 32 partial sums with a fixed xor butterfly.  The order is therefore fixed by K and BITS alone: neither the grid,
-// the chunking of x nor the batch size m changes a single bit of y[i, o].
+// A warp owns four consecutive output features and walks their rows with the quad walk of qd_packed_walk.cuh, then
+// folds its 32 partial sums with warp_sum's fixed xor butterfly: the order is fixed by K and BITS alone, so neither the
+// grid, the chunking of x nor the batch size m changes a single bit of y[i, o].
 //
 // x rows m0 .. m0+MT-1 (MT = 1, 2, 4, 8 accumulators per lane and row, blockIdx.y = row tile) are staged in shared
 // memory, in chunks of kc columns when MT*K floats exceed kPlSmemBytes.  With one chunk the tile is staged once and
-// the CTA walks its slabs of output features; with several, each slab restages them.  The float4 groups of the tile
-// are XOR-swizzled within blocks of eight so that the 32 lanes' reads (stride 4*E floats) hit distinct banks.
-constexpr int kPlWarps = 8;
-constexpr int kPlThreads = kPlWarps * 32;
-constexpr int kPlRowsPerWarp = 4;
+// the CTA walks its slabs of output features; with several, each slab restages them.
 constexpr int kPlSlab = kPlWarps * kPlRowsPerWarp;   // output features per CTA iteration
-constexpr size_t kPlSmemBytes = 96 * 1024;           // x tile, unless one warp-wide step of MT rows needs more
 
 struct PackedLinearArgs {
     const float* x;
@@ -454,35 +439,9 @@ struct PackedLinearArgs {
     bool x_vec;                 // x 16-byte aligned and K a multiple of 4
 };
 
-// position of float4 group g of a tile row: bits 0-2 XOR-ed with the quad index (E float4 groups per quad)
-template <int BITS>
-__device__ __forceinline__ int pl_slot(int g) {
-    constexpr int shift = BITS == 8 ? 2 : BITS == 4 ? 3 : BITS == 2 ? 4 : 5;   // log2(E)
-    return g ^ ((g >> shift) & 7);
-}
-
-// the 32 code bits of elements e0 .. e0+E-1 (e0*BITS need not be a multiple of 32); bytes past the tensor read as 0
-template <int BITS>
-__device__ __forceinline__ uint32_t pl_word(const PackedLinearArgs& a, int64_t e0) {
-    const int64_t bit = e0 * BITS;
-    const int64_t b0 = bit >> 3;
-    unsigned long long v = 0;
-    for (int i = 0; i < 5; ++i)
-        if (b0 + i < a.in_bytes) v |= (unsigned long long)a.packed[b0 + i] << (8 * i);
-    return (uint32_t)(v >> (unsigned)(bit & 7));
-}
-
-template <int BITS>
-__device__ __forceinline__ uint4 pl_quad(const PackedLinearArgs& a, int64_t e0) {
-    if (a.quad_aligned) return __ldcs(reinterpret_cast<const uint4*>(a.packed + ((e0 * BITS) >> 3)));
-    constexpr int E = 32 / BITS;
-    return make_uint4(pl_word<BITS>(a, e0), pl_word<BITS>(a, e0 + E), pl_word<BITS>(a, e0 + 2 * E), pl_word<BITS>(a, e0 + 3 * E));
-}
-
 template <bool UNIFORM, int BITS, int MT>
 __global__ void __launch_bounds__(kPlThreads, 1) packed_linear_kernel(PackedLinearArgs a) {
-    constexpr int E = 32 / BITS, E4 = E / 4;
-    constexpr unsigned mask = (1u << BITS) - 1u;
+    constexpr int E = 32 / BITS;
     extern __shared__ float4 s_x[];
     __shared__ float s_unit[256];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -492,28 +451,9 @@ __global__ void __launch_bounds__(kPlThreads, 1) packed_linear_kernel(PackedLine
     const int64_t qpr = (a.K + 4 * E - 1) / (4 * E);      // quads per weight row
     const int64_t chunks = (a.K + a.kc - 1) / a.kc;
     const int64_t slabs = (a.O + kPlSlab - 1) / kPlSlab;
-    auto stage = [&](int64_t c) {
-        const int64_t c0 = c * a.kc;
-        for (int t = threadIdx.x; t < MT * kc4; t += kPlThreads) {
-            const int i = t / kc4, g = t - i * kc4;
-            const int64_t k = c0 + 4 * (int64_t)g;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (m0 + i < a.m && k < a.K) {
-                const float* xr = a.x + (m0 + i) * a.K;
-                if (a.x_vec) {
-                    v = __ldg(reinterpret_cast<const float4*>(xr + k));
-                } else {
-                    v.x = xr[k];
-                    if (k + 1 < a.K) v.y = xr[k + 1];
-                    if (k + 2 < a.K) v.z = xr[k + 2];
-                    if (k + 3 < a.K) v.w = xr[k + 3];
-                }
-            }
-            s_x[i * kc4 + pl_slot<BITS>(g)] = v;
-        }
-    };
+    auto x_row = [&](int64_t i) { return a.x + i * a.K; };
     load_unit_table<UNIFORM>(s_unit, a.points, a.num_points, a.S);
-    if (chunks == 1) stage(0);
+    if (chunks == 1) pl_stage<BITS, MT>(s_x, x_row, m0, a.m, a.K, a.kc, kc4, a.x_vec, 0);
     __syncthreads();
     for (int64_t slab = blockIdx.x; slab < slabs; slab += gridDim.x) {
         // rows past O repeat row O-1: computed, never written
@@ -531,78 +471,10 @@ __global__ void __launch_bounds__(kPlThreads, 1) packed_linear_kernel(PackedLine
         for (int64_t c = 0; c < chunks; ++c) {
             if (chunks > 1) {
                 __syncthreads();
-                stage(c);
+                pl_stage<BITS, MT>(s_x, x_row, m0, a.m, a.K, a.kc, kc4, a.x_vec, c);
                 __syncthreads();
             }
-            const int64_t d_first = c * kq + lane, d_end = min(qpr, (c + 1) * kq);
-            if (d_first >= d_end) continue;
-            int64_t bk[kPlRowsPerWarp], rk[kPlRowsPerWarp];   // bucket of the quad's first element, offset in it
-#pragma unroll
-            for (int r = 0; r < kPlRowsPerWarp; ++r) {
-                const int64_t e0 = orow[r] * a.K + d_first * 4 * E;
-                bk[r] = e0 / a.L;
-                rk[r] = e0 - bk[r] * a.L;
-            }
-            for (int64_t d = d_first; d < d_end; d += 32) {
-                uint4 cq[kPlRowsPerWarp];
-#pragma unroll
-                for (int r = 0; r < kPlRowsPerWarp; ++r) cq[r] = pl_quad<BITS>(a, orow[r] * a.K + d * 4 * E);
-                // per row, a cursor (bucket bc, offset rc) that walks the quad's elements in order: alpha / beta are
-                // fetched once per bucket, and a bucket ending inside the quad costs one compare per element
-                float al[kPlRowsPerWarp], be[kPlRowsPerWarp];
-                int64_t bc[kPlRowsPerWarp], rc[kPlRowsPerWarp];
-#pragma unroll
-                for (int r = 0; r < kPlRowsPerWarp; ++r) {
-                    bc[r] = bk[r];
-                    rc[r] = rk[r];
-                    al[r] = __ldg(a.alpha + bc[r]);
-                    be[r] = __ldg(a.beta + bc[r]);
-                }
-                // columns of the quad inside the row: < 4*E only in its last quad
-                const int valid = (int)min((int64_t)(4 * E), a.K - d * 4 * E);
-                const int gbase = (int)(d - c * kq) * E;
-                // loops over the quad's words and float4 groups stay rolled: the kernel body must fit the instruction
-                // cache, since a lane runs it only a few times per launch
-#pragma unroll 1
-                for (int u = 0; u < 4; ++u) {
-#pragma unroll 1
-                    for (int t = 0; t < E4; ++t) {
-                        float q[kPlRowsPerWarp][4];
-#pragma unroll
-                        for (int r = 0; r < kPlRowsPerWarp; ++r) {
-                            const uint32_t cw = u == 0 ? cq[r].x : u == 1 ? cq[r].y : u == 2 ? cq[r].z : cq[r].w;
-#pragma unroll
-                            for (int jj = 0; jj < 4; ++jj) {
-                                const int jw = 4 * t + jj, j = u * E + jw;
-                                q[r][jj] = j < valid ? from_unit(s_unit[(cw >> (jw * BITS)) & mask], al[r], be[r]) : 0.f;
-                                if (++rc[r] == a.L) {                  // next element starts bucket bc + 1
-                                    rc[r] = 0;
-                                    const int64_t b = min(++bc[r], a.rows - 1);
-                                    al[r] = __ldg(a.alpha + b);
-                                    be[r] = __ldg(a.beta + b);
-                                }
-                            }
-                        }
-#pragma unroll
-                        for (int i = 0; i < MT; ++i) {
-                            const float4 xv = s_x[i * kc4 + pl_slot<BITS>(gbase + u * E4 + t)];
-#pragma unroll
-                            for (int r = 0; r < kPlRowsPerWarp; ++r) {
-                                acc[r][i] = __fmaf_rn(xv.x, q[r][0], acc[r][i]);
-                                acc[r][i] = __fmaf_rn(xv.y, q[r][1], acc[r][i]);
-                                acc[r][i] = __fmaf_rn(xv.z, q[r][2], acc[r][i]);
-                                acc[r][i] = __fmaf_rn(xv.w, q[r][3], acc[r][i]);
-                            }
-                        }
-                    }
-                }
-#pragma unroll
-                for (int r = 0; r < kPlRowsPerWarp; ++r) {
-                    bk[r] += a.step_q;
-                    rk[r] += a.step_r;
-                    if (rk[r] >= a.L) { rk[r] -= a.L; ++bk[r]; }
-                }
-            }
+            pl_walk<BITS, MT>(a, s_unit, s_x, kc4, kq, qpr, c, lane, orow, acc);
         }
 #pragma unroll
         for (int r = 0; r < kPlRowsPerWarp; ++r) {
@@ -621,8 +493,7 @@ __global__ void __launch_bounds__(kPlThreads, 1) packed_linear_kernel(PackedLine
 template <int MT, bool UNIFORM, int BITS>
 static int launch_packed_linear(PackedLinearArgs a, cudaStream_t st) {
     constexpr int64_t step_cols = 32 * 4 * (32 / BITS);   // columns of one warp-wide step
-    const int64_t room = std::max<int64_t>(1, (int64_t)(kPlSmemBytes / (MT * sizeof(float))) / step_cols) * step_cols;
-    a.kc = std::min(room, (a.K + step_cols - 1) / step_cols * step_cols);
+    a.kc = pl_chunk_cols<MT, BITS>(a.K);
     a.step_q = step_cols / a.L;
     a.step_r = step_cols % a.L;
     const size_t smem = (size_t)MT * a.kc * sizeof(float);

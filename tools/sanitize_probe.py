@@ -106,5 +106,20 @@ for bits, V, D, bucket in ((1, 37, 7, 100), (2, 50, 3, 100), (4, 9, 31, 100), (8
     N.check(N.lib().qd_packed_embedding(N.ptr(idx), 8, idx.numel(), V, D, N.ptr(shifted) + 1, bits, N.ptr(emb.alpha), N.ptr(emb.beta),
                                         None, 0, s_levels, bucket or 0, N.ptr(buf) + 4, None, N.stream_ptr()))
     assert torch.equal(buf[1:].view(-1, D)[ok], want[ok])
+# packed LSTM cell and layer: odd sizes whose rows start inside a byte, buckets straddling gate rows, 1 / 4 / 8 rows
+# (row tiles of 1, 4 and 8), a bidirectional two-layer LSTM over an unsorted PackedSequence
+for bits, I, Hd, bucket in ((1, 7, 5, 100), (2, 33, 17, 3), (4, 129, 250, 256), (8, 10, 9, None)):
+    lstm_pm = codec.pack_model(torch.nn.LSTM(I, Hd, num_layers=2, bidirectional=True).cuda(), bits, bucket)
+    net = torch.nn.Sequential(torch.nn.LSTM(I, Hd, num_layers=2, bidirectional=True)).cuda()
+    assert codec.attach_packed_(lstm_pm, net, recurrent=True) == ["0"]
+    xs = torch.nn.utils.rnn.pack_padded_sequence(torch.randn(6, 8, I).cuda(), torch.tensor([6, 1, 3, 6, 2, 5, 4, 1]), enforce_sorted=False)
+    net[0].CROSSOVER_ROWS = N.PACKED_LSTM_MAX_ROWS                  # the kernel path, not decode + torch
+    with torch.no_grad():
+        net[0](xs)
+        cell_pm = codec.pack_model(torch.nn.LSTMCell(I, Hd).cuda(), bits, bucket)
+        cell = codec.PackedLSTMCell(cell_pm.tensors[0], cell_pm.tensors[1], "uniform", 1 << bits, bucket)
+        cell.CROSSOVER_ROWS = N.PACKED_LSTM_MAX_ROWS
+        for m_rows in (1, 4, 8):
+            cell(torch.randn(m_rows, I).cuda())
 torch.cuda.synchronize()
 print("sanitize probe ok")
