@@ -274,6 +274,35 @@ int qd_packed_lstm_layer(const float* x, int64_t ldx, const int64_t* batch_sizes
                          const float* b_ih, const float* b_hh, const float* h0, const float* c0, float* out, int64_t ldo,
                          float* h_n, float* c_n, qd_stream_t stream);
 
+/* One GRU step on packed weights for m rows (1 <= m <= QD_PACKED_GRU_MAX_ROWS; larger m is QD_ERR_UNSUPPORTED):
+ * x float32[m, I] (row stride ldx >= I), h float32[m, H] (stride ldh >= H); w_ih and w_hh describe the packed [3H, I]
+ * and [3H, H] weights (HOST structs holding device pointers; n must be 3*H*I and 3*H*H, each its own bits and,
+ * non-uniform, its own points; q is not read), decoded as qd_unpack_dequant_* decodes them at the model's levels and
+ * bucket; b_ih and b_hh float32[3H] may be NULL.  Gate order is torch's: r, z, n (rows j, H+j, 2H+j of each weight for
+ * hidden unit j).  Writes h_out[m, H] (stride ldo >= H).
+ * Numerical contract: with gi = qd_packed_linear(x, W_ih, b_ih) and gh = qd_packed_linear(h, W_hh, b_hh), bit for bit
+ * (a NULL bias is not added), r = sig(gi_r + gh_r), z = sig(gi_z + gh_z), n = tanh(gi_n + r*gh_n) and
+ * h' = n + z*(h - n): torch's GRU cell, b_hn inside r*(...).  sig(v) = 1/(1 + expf(-v)); every op is rounded to float32
+ * in that order (IEEE expf / tanhf, no contraction).  Unlike the LSTM cell's ((S_ih + b_ih) + S_hh) + b_hh, gi and gh
+ * are each complete before they meet, for r and z too, since n needs gh_n on its own.  The order depends on (I, H,
+ * bits) alone: a row gives the same bits alone or in any batch, on any stream, in any replay.  h_out must not overlap x
+ * or h (every warp reads all of h).  QD_ERR_INVALID_ARG: NULL pointers, sizes below 1, strides below the rows, bits too
+ * narrow for levels or points, the overlaps above.  No workspace; only enqueues work on `stream` (graph-capturable). */
+#define QD_PACKED_GRU_MAX_ROWS 64
+int qd_packed_gru_cell(const float* x, int64_t ldx, const float* h, int64_t ldh, int64_t m, int64_t input_size, int64_t hidden_size,
+                       const qd_packed_tensor* w_ih, const qd_packed_tensor* w_hh, int levels, int64_t bucket, const float* b_ih,
+                       const float* b_hh, float* h_out, int64_t ldo, qd_stream_t stream);
+/* One GRU layer in one direction over `steps` steps, one qd_packed_gru_cell launch per step enqueued from a C loop (no
+ * host synchronisation: graph-capturable), with qd_packed_lstm_layer's protocol: batch_sizes is HOST int64[steps],
+ * non-increasing, >= 1, the first at most QD_PACKED_GRU_MAX_ROWS; step t reads x rows and writes out rows at its
+ * offset sum(batch_sizes[0..t-1]) (strides ldx >= I, ldo >= H); reverse != 0 runs the steps T-1 .. 0; a row's
+ * previous h is the previous step's out row when the row was active there, else its h0 row; a row's h_n is written by
+ * its last step.  h0, h_n: float32[batch_sizes[0], H], C order.  Arithmetic as qd_packed_gru_cell.  QD_ERR_INVALID_ARG
+ * as there, plus batch sizes that increase or are below 1, and out or h_n overlapping x, h0 or each other. */
+int qd_packed_gru_layer(const float* x, int64_t ldx, const int64_t* batch_sizes, int64_t steps, int reverse, int64_t input_size,
+                        int64_t hidden_size, const qd_packed_tensor* w_ih, const qd_packed_tensor* w_hh, int levels, int64_t bucket,
+                        const float* b_ih, const float* b_hh, const float* h0, float* out, int64_t ldo, float* h_n, qd_stream_t stream);
+
 /* ---- next row f2: Huffman-coded storage (the model helpers/functions.py:226-262 only sizes) ----------
  * Canonical code over uint8 symbols, codes of 1..QD_HUFFMAN_MAX_LENGTH bits (built on the host: codec.py).
  * Stream: a tensor's symbols are cut into chunks of QD_HUFFMAN_CHUNK; each chunk's codes are written MSB-first

@@ -21,6 +21,7 @@ SCALE_ABSMAX, SCALE_ABSNORM = 1, 2
 MAX_STAGED_BUCKET = 49152
 PACKED_LINEAR_MAX_ROWS = 64     # QD_PACKED_LINEAR_MAX_ROWS
 PACKED_LSTM_MAX_ROWS = 64       # QD_PACKED_LSTM_MAX_ROWS
+PACKED_GRU_MAX_ROWS = 64        # QD_PACKED_GRU_MAX_ROWS
 
 _p, _i64, _i32, _u64, _f32, _sz = C.c_void_p, C.c_int64, C.c_int, C.c_uint64, C.c_float, C.c_size_t
 
@@ -58,6 +59,8 @@ SIGNATURES = {
     "qd_packed_embedding": (C.c_int, [_p, _i32, _i64, _i64, _i64, _p, _i32, _p, _p, _p, _i32, _i32, _i64, _p, _p, _p]),
     "qd_packed_lstm_cell": (C.c_int, [_p, _i64, _p, _i64, _p, _i64, _i64, _i64, _p, _p, _i32, _i64, _p, _p, _p, _i64, _p, _p]),
     "qd_packed_lstm_layer": (C.c_int, [_p, _i64, _p, _i64, _i32, _i64, _i64, _p, _p, _i32, _i64, _p, _p, _p, _p, _p, _i64, _p, _p, _p]),
+    "qd_packed_gru_cell": (C.c_int, [_p, _i64, _p, _i64, _i64, _i64, _i64, _p, _p, _i32, _i64, _p, _p, _p, _i64, _p]),
+    "qd_packed_gru_layer": (C.c_int, [_p, _i64, _p, _i64, _i32, _i64, _i64, _p, _p, _i32, _i64, _p, _p, _p, _p, _i64, _p, _p]),
     "qd_huffman_encode":(C.c_int, [_p, _i64, _p, _p, _i64, _p, _p, _p]),
     "qd_huffman_decode_dequant_uniform": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _i64, _i64, _i32, _p]),
     "qd_huffman_decode_dequant_nonuniform": (C.c_int, [_p, _i64, _p, _p, _p, _i32, _p, _p, _p, _i64, _i64, _p]),

@@ -1213,9 +1213,17 @@ def _check_weights(weights, x, what: str) -> None:
         _check_state(w, x, what)
 
 
-def _lstm_pair(entry_ih, entry_hh, kind, levels, bucket_size, bias_ih, bias_hh, hidden_size, input_size) -> torch.nn.ModuleList:
-    return torch.nn.ModuleList([_PackedWeight(entry_ih, kind, levels, bucket_size, bias_ih, 4 * hidden_size, input_size),
-                                _PackedWeight(entry_hh, kind, levels, bucket_size, bias_hh, 4 * hidden_size, hidden_size)])
+def _gate_sizes(entry, gates: int, what: str) -> tuple:
+    """(hidden_size, input_size) of a recurrent input weight [gates * hidden_size, input_size]; ``what`` names the layer
+    with its article ("an LSTM")."""
+    if len(entry.shape) != 2 or entry.shape[0] % gates or entry.shape[0] < gates:
+        raise ValueError(f"{entry.name}: {what} input weight is [{gates} * hidden_size, input_size], got {tuple(entry.shape)}")
+    return int(entry.shape[0]) // gates, int(entry.shape[1])
+
+
+def _cell_pair(entry_ih, entry_hh, kind, levels, bucket_size, bias_ih, bias_hh, gates, hidden_size, input_size) -> torch.nn.ModuleList:
+    return torch.nn.ModuleList([_PackedWeight(entry_ih, kind, levels, bucket_size, bias_ih, gates * hidden_size, input_size),
+                                _PackedWeight(entry_hh, kind, levels, bucket_size, bias_hh, gates * hidden_size, hidden_size)])
 
 
 class PackedLSTMCell(torch.nn.Module):
@@ -1234,11 +1242,9 @@ class PackedLSTMCell(torch.nn.Module):
     def __init__(self, entry_ih: PackedEntry, entry_hh: PackedEntry, kind: str, levels, bucket_size, bias_ih: torch.Tensor = None,
                  bias_hh: torch.Tensor = None):
         super().__init__()
-        if len(entry_ih.shape) != 2 or entry_ih.shape[0] % 4 or entry_ih.shape[0] < 4:
-            raise ValueError(f"{entry_ih.name}: an LSTM input weight is [4 * hidden_size, input_size], got {tuple(entry_ih.shape)}")
-        self.hidden_size, self.input_size = int(entry_ih.shape[0]) // 4, int(entry_ih.shape[1])
+        self.hidden_size, self.input_size = _gate_sizes(entry_ih, 4, "an LSTM")
         self.bias = bias_ih is not None or bias_hh is not None
-        self.weights = _lstm_pair(entry_ih, entry_hh, kind, levels, bucket_size, bias_ih, bias_hh, self.hidden_size, self.input_size)
+        self.weights = _cell_pair(entry_ih, entry_hh, kind, levels, bucket_size, bias_ih, bias_hh, 4, self.hidden_size, self.input_size)
 
     def extra_repr(self) -> str:
         ih = self.weights[0]
@@ -1282,22 +1288,13 @@ class PackedLSTMCell(torch.nn.Module):
         return (h1, c1) if batched else (h1[0], c1[0])
 
 
-class PackedLSTM(torch.nn.Module):
-    """Inference replacement of an ``nn.LSTM`` (no projection) whose weight matrices stay in their fixed-width stored
-    form on the device: ``weights`` is one (entry_ih, entry_hh) pair per layer and direction in nn.LSTM's order (l0,
-    l0_reverse, l1, ...), ``biases`` the matching (bias_ih, bias_hh) pairs or None.  Takes what nn.LSTM takes -- padded
-    3-D input (batch_first or not), unbatched 2-D input, or a PackedSequence (sorted or not), with ``hx`` = (h_0, c_0)
-    or None -- and returns (output, (h_n, c_n)) in nn.LSTM's shapes.  For batches of up to CROSSOVER_ROWS rows (none by
-    default), every
-    layer and direction is one qd_packed_lstm_layer call (one fused cell launch per step, no host synchronisation, so
-    the forward can be captured in a CUDA graph); the arithmetic is qd_packed_lstm_cell's, so a sequence gives the same
-    bits alone, inside any batch and at any position of a PackedSequence.  Larger batches decode every weight and call
-    torch's LSTM: exactly what an unpack_-loaded nn.LSTM computes.  Inter-layer dropout is not applied: in training
-    mode with dropout > 0 and several layers forward raises, since the result would differ from nn.LSTM's."""
-    # largest batch that runs on qd_packed_lstm_layer (at most N.PACKED_LSTM_MAX_ROWS).  Measured (DESIGN.md section
-    # 3.7.6): on the NMT encoder layer the kernel loses to decode + torch at batch 1, 5, 30 and 64, so by default every
-    # batch decodes.
-    CROSSOVER_ROWS = 0
+class _PackedRNN(torch.nn.Module):
+    """The sequence plumbing PackedLSTM and PackedGRU share: the weight pairs per layer and direction, the input layouts
+    (padded 3-D, batch_first or not, unbatched 2-D, PackedSequence sorted or not), the state checks and the
+    PackedSequence permutation, and the choice between the packed layer kernel and decode + torch.  A subclass names
+    its gates per hidden unit, its state tensors, its layer entry point and its torch function."""
+    _gates = _states = None                      # weight rows per hidden unit; state tensors per layer (h or h, c)
+    _what = _article = _layer_fn = _vf = None    # module name, "an LSTM" / "a GRU", qd_packed_*_layer, torch._VF function
 
     def __init__(self, weights, kind: str, levels, bucket_size, *, num_layers=1, batch_first=False, dropout=0.0, bidirectional=False,
                  biases=None):
@@ -1307,17 +1304,14 @@ class PackedLSTM(torch.nn.Module):
             raise ValueError(f"{len(weights)} weight pairs for {num_layers} layers x {dirs} directions")
         if biases is not None and len(biases) != len(weights):
             raise ValueError(f"{len(biases)} bias pairs for {len(weights)} weight pairs")
-        first = weights[0][0]
-        if len(first.shape) != 2 or first.shape[0] % 4 or first.shape[0] < 4:
-            raise ValueError(f"{first.name}: an LSTM input weight is [4 * hidden_size, input_size], got {tuple(first.shape)}")
-        self.hidden_size, self.input_size = int(first.shape[0]) // 4, int(first.shape[1])
+        self.hidden_size, self.input_size = _gate_sizes(weights[0][0], self._gates, self._article)
         self.num_layers, self.batch_first, self.dropout, self.bidirectional = num_layers, batch_first, float(dropout), bidirectional
         self.bias = biases is not None
         self.cells = torch.nn.ModuleList()
         for k, (e_ih, e_hh) in enumerate(weights):
             b_ih, b_hh = biases[k] if biases is not None else (None, None)
             in_size = self.input_size if k < dirs else dirs * self.hidden_size
-            self.cells.append(_lstm_pair(e_ih, e_hh, kind, levels, bucket_size, b_ih, b_hh, self.hidden_size, in_size))
+            self.cells.append(_cell_pair(e_ih, e_hh, kind, levels, bucket_size, b_ih, b_hh, self._gates, self.hidden_size, in_size))
 
     def extra_repr(self) -> str:
         ih = self.cells[0][0]
@@ -1325,20 +1319,22 @@ class PackedLSTM(torch.nn.Module):
                 f"dropout={self.dropout}, bidirectional={self.bidirectional}, {ih.kind}, bucket_size={ih.bucket_size}")
 
     def decoded_weights(self) -> list:
-        """nn.LSTM's flat weight list (w_ih, w_hh[, b_ih, b_hh] per layer and direction), the matrices decoded to float32 bit
-        for bit as unpack_ writes them."""
+        """torch's flat weight list (w_ih, w_hh[, b_ih, b_hh] per layer and direction), the matrices decoded to float32
+        bit for bit as unpack_ writes them."""
         flat = []
         for ih, hh in self.cells:
             flat += [ih.decoded(), hh.decoded()] + ([ih.bias, hh.bias] if self.bias else [])
         return flat
 
-    def forward(self, input, hx=None):
+    def _run(self, input, hx) -> tuple:
+        """(output, final states) for ``hx`` = the initial state tensors (a tuple of _states) or None (zeros), in the
+        input's layout."""
         packed_in = isinstance(input, torch.nn.utils.rnn.PackedSequence)
         weights = [w for pair in self.cells for w in pair]
         x = input.data if packed_in else input
-        _check_weights(weights, x, "PackedLSTM")
+        _check_weights(weights, x, self._what)
         if self.training and self.dropout > 0 and self.num_layers > 1:
-            raise RuntimeError("PackedLSTM does not apply inter-layer dropout: call eval(), or set dropout to 0")
+            raise RuntimeError(f"{self._what} does not apply inter-layer dropout: call eval(), or set dropout to 0")
         dirs, H, L = 2 if self.bidirectional else 1, self.hidden_size, self.num_layers
         if packed_in:
             if x.dim() != 2 or x.shape[1] != self.input_size:
@@ -1354,45 +1350,46 @@ class PackedLSTM(torch.nn.Module):
                 x = x.unsqueeze(batch_dim)
             B = x.shape[batch_dim]
         if hx is None:
-            h0 = torch.zeros(L * dirs, B, H, dtype=torch.float32, device=x.device)
-            c0 = torch.zeros_like(h0)
+            states = [torch.zeros(L * dirs, B, H, dtype=torch.float32, device=x.device) for _ in range(self._states)]
         else:
-            h0, c0 = hx
-            for t in (h0, c0):
-                _check_weights(weights, t, "PackedLSTM")
+            states = list(hx)
+            if len(states) != self._states:
+                raise ValueError(f"{len(states)} state tensors, expected {self._states}")
+            for t in states:
+                _check_weights(weights, t, self._what)
                 if tuple(t.shape) != ((L * dirs, B, H) if batched else (L * dirs, H)):
                     raise ValueError(f"hidden state of shape {tuple(t.shape)}, expected {(L * dirs, B, H) if batched else (L * dirs, H)}")
             if not batched:
-                h0, c0 = h0.unsqueeze(1), c0.unsqueeze(1)
-            if packed_in and input.sorted_indices is not None:         # nn.LSTM's permute_hidden
-                h0, c0 = h0.index_select(1, input.sorted_indices), c0.index_select(1, input.sorted_indices)
+                states = [t.unsqueeze(1) for t in states]
+            if packed_in and input.sorted_indices is not None:         # torch's permute_hidden
+                states = [t.index_select(1, input.sorted_indices) for t in states]
         with torch.cuda.device(x.device):
             if B == 0 or x.numel() == 0 or B > self.CROSSOVER_ROWS:
-                out, h_n, c_n = self._decoded_forward(x, batch_sizes if packed_in else None, h0, c0)
+                out, finals = self._decoded_forward(x, batch_sizes if packed_in else None, states)
             else:
-                out, h_n, c_n = self._packed_forward(x, batch_sizes if packed_in else None, h0, c0)
+                out, finals = self._packed_forward(x, batch_sizes if packed_in else None, states)
         if packed_in:
             if input.unsorted_indices is not None:
-                h_n, c_n = h_n.index_select(1, input.unsorted_indices), c_n.index_select(1, input.unsorted_indices)
-            return torch.nn.utils.rnn.PackedSequence(out, batch_sizes, input.sorted_indices, input.unsorted_indices), (h_n, c_n)
+                finals = [t.index_select(1, input.unsorted_indices) for t in finals]
+            return torch.nn.utils.rnn.PackedSequence(out, batch_sizes, input.sorted_indices, input.unsorted_indices), tuple(finals)
         if not batched:
-            out, h_n, c_n = out.squeeze(batch_dim), h_n.squeeze(1), c_n.squeeze(1)
-        return out, (h_n, c_n)
+            out, finals = out.squeeze(batch_dim), [t.squeeze(1) for t in finals]
+        return out, tuple(finals)
 
-    def _decoded_forward(self, x, batch_sizes, h0, c0):
+    def _decoded_forward(self, x, batch_sizes, states):
         import warnings
         flat = self.decoded_weights()
+        hx = tuple(states) if len(states) > 1 else states[0]
+        rnn = getattr(torch._VF, self._vf)
         with warnings.catch_warnings():       # the decoded weights are not one flattened buffer; cuDNN copies them into one
             warnings.filterwarnings("ignore", message="RNN module weights are not part of single contiguous chunk")
             if batch_sizes is not None:
-                out, h_n, c_n = torch._VF.lstm(x, batch_sizes, (h0, c0), flat, self.bias, self.num_layers, self.dropout, self.training,
-                                               self.bidirectional)
+                res = rnn(x, batch_sizes, hx, flat, self.bias, self.num_layers, self.dropout, self.training, self.bidirectional)
             else:
-                out, h_n, c_n = torch._VF.lstm(x, (h0, c0), flat, self.bias, self.num_layers, self.dropout, self.training,
-                                               self.bidirectional, self.batch_first)
-        return out, h_n, c_n
+                res = rnn(x, hx, flat, self.bias, self.num_layers, self.dropout, self.training, self.bidirectional, self.batch_first)
+        return res[0], list(res[1:])
 
-    def _packed_forward(self, x, batch_sizes, h0, c0):
+    def _packed_forward(self, x, batch_sizes, states):
         dirs, H = 2 if self.bidirectional else 1, self.hidden_size
         if batch_sizes is not None:
             bs = np.ascontiguousarray(batch_sizes.cpu().numpy(), dtype=np.int64)
@@ -1403,25 +1400,130 @@ class PackedLSTM(torch.nn.Module):
             data = seq.reshape(-1, self.input_size)
         if data.stride(-1) != 1:
             data = data.contiguous()
-        h0, c0 = h0.contiguous(), c0.contiguous()
-        h_n, c_n = torch.empty_like(h0), torch.empty_like(c0)
+        states = [t.contiguous() for t in states]
+        finals = [torch.empty_like(t) for t in states]
         rows, sp = data.shape[0], N.stream_ptr(data.device)
+        layer_fn = getattr(N.lib(), self._layer_fn)
         for layer in range(self.num_layers):
             out = torch.empty(rows, dirs * H, dtype=torch.float32, device=data.device)
             for d in range(dirs):
                 k = layer * dirs + d
                 ih, hh = self.cells[k]
                 d_ih, d_hh = ih.descriptor(), hh.descriptor()
-                N.check(N.lib().qd_packed_lstm_layer(N.ptr(data), data.stride(0), bs.ctypes.data, len(bs), d, ih.shape[1], H,
-                                                     d_ih.ctypes.data, d_hh.ctypes.data, ih.levels,
-                                                     _bucket(ih.bucket_size), N.ptr(ih.bias), N.ptr(hh.bias), N.ptr(h0[k]), N.ptr(c0[k]),
-                                                     N.ptr(out) + 4 * d * H, dirs * H, N.ptr(h_n[k]), N.ptr(c_n[k]), sp))
+                # (x, ldx, batch_sizes, steps, reverse, I, H, w_ih, w_hh, levels, bucket, b_ih, b_hh, initial states, out,
+                # ldo, final states, stream)
+                N.check(layer_fn(N.ptr(data), data.stride(0), bs.ctypes.data, len(bs), d, ih.shape[1], H, d_ih.ctypes.data, d_hh.ctypes.data,
+                                 ih.levels, _bucket(ih.bucket_size), N.ptr(ih.bias), N.ptr(hh.bias), *(N.ptr(t[k]) for t in states),
+                                 N.ptr(out) + 4 * d * H, dirs * H, *(N.ptr(t[k]) for t in finals), sp))
             data = out
         if batch_sizes is None:
             data = data.view(len(bs), -1, dirs * H)
             if self.batch_first:
                 data = data.transpose(0, 1).contiguous()
-        return data, h_n, c_n
+        return data, finals
+
+
+class PackedLSTM(_PackedRNN):
+    """Inference replacement of an ``nn.LSTM`` (no projection) whose weight matrices stay in their fixed-width stored
+    form on the device: ``weights`` is one (entry_ih, entry_hh) pair per layer and direction in nn.LSTM's order (l0,
+    l0_reverse, l1, ...), ``biases`` the matching (bias_ih, bias_hh) pairs or None.  Takes what nn.LSTM takes -- padded
+    3-D input (batch_first or not), unbatched 2-D input, or a PackedSequence (sorted or not), with ``hx`` = (h_0, c_0)
+    or None -- and returns (output, (h_n, c_n)) in nn.LSTM's shapes.  For batches of up to CROSSOVER_ROWS rows (none by
+    default), every
+    layer and direction is one qd_packed_lstm_layer call (one fused cell launch per step, no host synchronisation, so
+    the forward can be captured in a CUDA graph); the arithmetic is qd_packed_lstm_cell's, so a sequence gives the same
+    bits alone, inside any batch and at any position of a PackedSequence.  Larger batches decode every weight and call
+    torch's LSTM: exactly what an unpack_-loaded nn.LSTM computes.  Inter-layer dropout is not applied: in training
+    mode with dropout > 0 and several layers forward raises, since the result would differ from nn.LSTM's."""
+    # largest batch that runs on qd_packed_lstm_layer (at most N.PACKED_LSTM_MAX_ROWS).  Measured (DESIGN.md section
+    # 3.7.6): on the NMT encoder layer the kernel loses to decode + torch at batch 1, 5, 30 and 64, so by default every
+    # batch decodes.
+    CROSSOVER_ROWS = 0
+    _gates, _states, _what, _article, _layer_fn, _vf = 4, 2, "PackedLSTM", "an LSTM", "qd_packed_lstm_layer", "lstm"
+
+    def forward(self, input, hx=None):
+        out, (h_n, c_n) = self._run(input, hx)
+        return out, (h_n, c_n)
+
+
+class PackedGRU(_PackedRNN):
+    """Inference replacement of an ``nn.GRU`` whose weight matrices stay in their fixed-width stored form on the device:
+    ``weights`` is one (entry_ih, entry_hh) pair per layer and direction in nn.GRU's order (l0, l0_reverse, l1, ...),
+    ``biases`` the matching (bias_ih, bias_hh) pairs or None.  Takes what nn.GRU takes -- padded 3-D input
+    (batch_first or not), unbatched 2-D input, or a PackedSequence (sorted or not), with ``hx`` = h_0 or None -- and
+    returns (output, h_n) in nn.GRU's shapes.  For batches of up to CROSSOVER_ROWS rows (none by default), every layer
+    and direction is one qd_packed_gru_layer call (one fused cell launch per step, no host synchronisation, so the
+    forward can be captured in a CUDA graph); the arithmetic is qd_packed_gru_cell's, so a sequence gives the same bits
+    alone, inside any batch and at any position of a PackedSequence.  Larger batches decode every weight and call
+    torch's GRU: exactly what an unpack_-loaded nn.GRU computes.  Inter-layer dropout is not applied: in training mode
+    with dropout > 0 and several layers forward raises, since the result would differ from nn.GRU's."""
+    # largest batch that runs on qd_packed_gru_layer (at most N.PACKED_GRU_MAX_ROWS).  Measured (DESIGN.md section
+    # 3.7.7): on the NMT encoder layer the kernel loses to decode + torch at batch 1, 5, 30 and 64 (28.6 against 8.7 us
+    # per step at batch 1), so by default every batch decodes.
+    CROSSOVER_ROWS = 0
+    _gates, _states, _what, _article, _layer_fn, _vf = 3, 1, "PackedGRU", "a GRU", "qd_packed_gru_layer", "gru"
+
+    def forward(self, input, hx=None):
+        out, (h_n,) = self._run(input, None if hx is None else (hx,))
+        return out, h_n
+
+
+class PackedGRUCell(torch.nn.Module):
+    """Inference replacement of an ``nn.GRUCell`` whose two weight matrices stay in their fixed-width stored form (two
+    PackedEntry of a PackedModel, [3H, I] and [3H, H]) on the device.  Takes input [B, I] or [I] and ``hx`` = h or None
+    (zeros), returns h' in nn.GRUCell's shape.  Up to CROSSOVER_ROWS rows (none by default), forward runs
+    qd_packed_gru_cell: one launch that reads the codes of both weights and applies the cell update in registers, every
+    weight bit for bit the decoded one, each gate's linear output in qd_packed_linear's fixed float32 order
+    (include/qd_b200.h states the contract).  Larger batches decode both weights into scratch tensors and call torch's
+    GRU cell: exactly what an unpack_-loaded nn.GRUCell computes.  Forward only, no host synchronisation
+    (graph-capturable)."""
+    # largest batch that runs on the packed kernel (at most N.PACKED_GRU_MAX_ROWS).  Measured (DESIGN.md section
+    # 3.7.7): on the NMT decoder cells the kernel loses to decode + torch at batch 1, 5, 30 and 64 (28.9 against
+    # 19.7 us per step at batch 1, 1000 -> 500), so by default every batch decodes.
+    CROSSOVER_ROWS = 0
+
+    def __init__(self, entry_ih: PackedEntry, entry_hh: PackedEntry, kind: str, levels, bucket_size, bias_ih: torch.Tensor = None,
+                 bias_hh: torch.Tensor = None):
+        super().__init__()
+        self.hidden_size, self.input_size = _gate_sizes(entry_ih, 3, "a GRU")
+        self.bias = bias_ih is not None or bias_hh is not None
+        self.weights = _cell_pair(entry_ih, entry_hh, kind, levels, bucket_size, bias_ih, bias_hh, 3, self.hidden_size, self.input_size)
+
+    def extra_repr(self) -> str:
+        ih = self.weights[0]
+        return f"{self.input_size}, {self.hidden_size}, bias={self.bias}, {ih.kind}, bits={ih.bits}/{self.weights[1].bits}, bucket_size={ih.bucket_size}"
+
+    def decoded_weights(self) -> tuple:
+        """(weight_ih, weight_hh) decoded to float32, bit for bit what unpack_ writes."""
+        return self.weights[0].decoded(), self.weights[1].decoded()
+
+    def forward(self, input: torch.Tensor, hx=None) -> torch.Tensor:
+        _check_weights(self.weights, input, "PackedGRUCell")
+        if input.dim() not in (1, 2) or input.shape[-1] != self.input_size:
+            raise ValueError(f"input of shape {tuple(input.shape)}, expected (B, {self.input_size}) or ({self.input_size},)")
+        batched = input.dim() == 2
+        x = input if batched else input.unsqueeze(0)
+        B, H = x.shape[0], self.hidden_size
+        if hx is None:
+            h = torch.zeros(B, H, dtype=torch.float32, device=x.device)
+        else:
+            _check_weights(self.weights, hx, "PackedGRUCell")
+            if tuple(hx.shape) != ((B, H) if batched else (H,)):
+                raise ValueError(f"hidden state of shape {tuple(hx.shape)}, expected {(B, H) if batched else (H,)}")
+            h = hx if batched else hx.unsqueeze(0)
+        ih, hh = self.weights
+        with torch.cuda.device(x.device):
+            if B == 0 or B > self.CROSSOVER_ROWS:
+                w_ih, w_hh = self.decoded_weights()
+                h1 = torch._VF.gru_cell(x, h, w_ih, w_hh, ih.bias, hh.bias)
+            else:
+                x, h = (t if t.stride(-1) == 1 and t.stride(0) >= t.shape[1] else t.contiguous() for t in (x, h))
+                h1 = torch.empty(B, H, dtype=torch.float32, device=x.device)
+                d_ih, d_hh = ih.descriptor(), hh.descriptor()
+                N.check(N.lib().qd_packed_gru_cell(N.ptr(x), x.stride(0), N.ptr(h), h.stride(0), B, self.input_size, H, d_ih.ctypes.data,
+                                                   d_hh.ctypes.data, ih.levels, _bucket(ih.bucket_size), N.ptr(ih.bias), N.ptr(hh.bias),
+                                                   N.ptr(h1), H, N.stream_ptr(x.device)))
+        return h1 if batched else h1[0]
 
 
 def _conv_padding(conv) -> tuple:
@@ -1474,30 +1576,51 @@ def _lstm_cell_target(mod) -> bool:
     return type(mod) is torch.nn.LSTMCell
 
 
+def _gru_target(mod) -> bool:
+    return type(mod) is torch.nn.GRU
+
+
+def _gru_cell_target(mod) -> bool:
+    return type(mod) is torch.nn.GRUCell
+
+
 def _own_bias(b):
-    # a copy: on CUDA an nn.LSTM's parameters are views into one flattened buffer, which must not outlive the module
+    # a copy: on CUDA an nn.LSTM's or nn.GRU's parameters are views into one flattened buffer, which must not outlive
+    # the module
     return None if b is None else b.data.clone()
 
 
-def _packed_lstm(entries, pm, lstm):
+def _packed_rnn(cls, entries, pm, rnn):
     biases = None
-    if lstm.bias:
-        names = [n for n in lstm._flat_weights_names if n.startswith("bias")]
-        biases = [(_own_bias(getattr(lstm, a)), _own_bias(getattr(lstm, b))) for a, b in zip(names[0::2], names[1::2])]
-    return PackedLSTM(list(zip(entries[0::2], entries[1::2])), pm.kind, pm.levels, pm.bucket_size, num_layers=lstm.num_layers,
-                      batch_first=lstm.batch_first, dropout=lstm.dropout, bidirectional=lstm.bidirectional, biases=biases)
+    if rnn.bias:
+        names = [n for n in rnn._flat_weights_names if n.startswith("bias")]
+        biases = [(_own_bias(getattr(rnn, a)), _own_bias(getattr(rnn, b))) for a, b in zip(names[0::2], names[1::2])]
+    return cls(list(zip(entries[0::2], entries[1::2])), pm.kind, pm.levels, pm.bucket_size, num_layers=rnn.num_layers,
+               batch_first=rnn.batch_first, dropout=rnn.dropout, bidirectional=rnn.bidirectional, biases=biases)
+
+
+def _packed_lstm(entries, pm, lstm):
+    return _packed_rnn(PackedLSTM, entries, pm, lstm)
+
+
+def _packed_gru(entries, pm, gru):
+    return _packed_rnn(PackedGRU, entries, pm, gru)
 
 
 def _packed_lstm_cell(entries, pm, cell):
     return PackedLSTMCell(entries[0], entries[1], pm.kind, pm.levels, pm.bucket_size, _own_bias(cell.bias_ih), _own_bias(cell.bias_hh))
 
 
+def _packed_gru_cell(entries, pm, cell):
+    return PackedGRUCell(entries[0], entries[1], pm.kind, pm.levels, pm.bucket_size, _own_bias(cell.bias_ih), _own_bias(cell.bias_hh))
+
+
 def _weight_matrices(mod) -> list:
-    """The weights a packed replacement of ``mod`` holds: an LSTM's (ih, hh) per layer and direction in nn.LSTM's order,
-    an LSTMCell's (ih, hh), else the module's one weight."""
-    if isinstance(mod, torch.nn.LSTM):
+    """The weights a packed replacement of ``mod`` holds: an LSTM's or GRU's (ih, hh) per layer and direction in torch's
+    order, an LSTMCell's or GRUCell's (ih, hh), else the module's one weight."""
+    if isinstance(mod, (torch.nn.LSTM, torch.nn.GRU)):
         return [getattr(mod, n) for n in mod._flat_weights_names if n.startswith("weight")]
-    if isinstance(mod, torch.nn.LSTMCell):
+    if isinstance(mod, (torch.nn.LSTMCell, torch.nn.GRUCell)):
         return [mod.weight_ih, mod.weight_hh]
     return [mod.weight]
 
@@ -1567,7 +1690,7 @@ def attach_packed_linear_(pm: PackedModel, model) -> list:
     return _attach(pm, model, [(_linear_target, _packed_linear, "Linear")])
 
 
-def attach_packed_(pm: PackedModel, model, *, embeddings=False, recurrent=False) -> list:
+def attach_packed_(pm: PackedModel, model, *, embeddings=False, recurrent=False, gru=False) -> list:
     """attach_packed_linear_ for Linear and convolution layers: every nn.Linear it would replace becomes a
     PackedLinear, and every ``nn.Conv2d`` (the class itself, not a subclass) with groups 1, dilation 1, zero padding
     that is symmetric (int padding, "valid", or "same" that resolves to equal sides) and a weight ``pm`` stores
@@ -1581,14 +1704,17 @@ def attach_packed_(pm: PackedModel, model, *, embeddings=False, recurrent=False)
     is checked before anything is written.  With ``recurrent=True``, also every ``nn.LSTM`` (the class itself) without
     projection becomes a PackedLSTM, and every ``nn.LSTMCell`` a PackedLSTMCell, when ``pm`` stores all of its weight
     matrices quantized and it alone holds each of them; its biases are written as unpack_ writes them and handed to the
-    packed module (as copies: nothing keeps an LSTM's flattened weight buffer alive).  Every other recurrent module -- a
-    GRU, a subclass, one with a shared or float32 matrix -- is decoded as unpack_ decodes it.  Returns the names of the
-    replaced modules, in module order."""
+    packed module (as copies: nothing keeps an LSTM's flattened weight buffer alive).  With ``gru=True``, likewise
+    every ``nn.GRU`` becomes a PackedGRU and every ``nn.GRUCell`` a PackedGRUCell.  Every other recurrent module -- a
+    GRU without ``gru=True``, an LSTM without ``recurrent=True``, a subclass, one with a projection or a shared or
+    float32 matrix -- is decoded as unpack_ decodes it.  Returns the names of the replaced modules, in module order."""
     kinds = [(_linear_target, _packed_linear, "Linear"), (_conv_target, _packed_conv, "Conv2d")]
     if embeddings:
         kinds.append((_embedding_target, _packed_embedding, "Embedding"))
     if recurrent:
         kinds += [(_lstm_target, _packed_lstm, "LSTM"), (_lstm_cell_target, _packed_lstm_cell, "LSTMCell")]
+    if gru:
+        kinds += [(_gru_target, _packed_gru, "GRU"), (_gru_cell_target, _packed_gru_cell, "GRUCell")]
     return _attach(pm, model, kinds, tied=embeddings)
 
 

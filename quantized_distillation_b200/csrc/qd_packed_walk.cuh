@@ -1,6 +1,6 @@
 // qd_packed_walk.cuh -- the device half of the layers that run from fixed-width packed codes: the unit table, and
-// the quad walk of qd_packed_linear (staging of the activation tile, one warp's four weight rows summed against it)
-// that the packed LSTM cell (qd_recurrent.cu) runs twice, once per weight.  Everything here is __forceinline__, so
+// the quad walk of qd_packed_linear (staging of the activation tile, one warp's weight rows summed against it) that
+// the packed LSTM and GRU cells (qd_recurrent.cu) run twice, once per weight.  Everything here is __forceinline__, so
 // each kernel compiles it as if written in place.
 #pragma once
 #include <algorithm>
@@ -20,9 +20,10 @@ __device__ __forceinline__ void load_unit_table(float* s_unit, const float* __re
 }
 
 // ------------------------------------------------------------------ the quad walk
-// A warp owns four weight rows and walks them together, so that one shared-memory read of x feeds four rows.  A row
-// is cut into quads of 4*E codes (E = 32/BITS per 32-bit word; quad d holds columns 4*E*d .. 4*E*d+4*E-1, one 128-bit
-// load when rows start on 16-byte boundaries); lane L takes quads L, L+32, ... in increasing order and sums its
+// A warp owns R weight rows (four; three in the GRU cell) and walks them together, so that one shared-memory read of x
+// feeds R rows.  A row is cut into quads of 4*E codes (E = 32/BITS per 32-bit word; quad d holds columns
+// 4*E*d .. 4*E*d+4*E-1, one 128-bit load when rows start on 16-byte boundaries); lane L takes quads L, L+32, ... in
+// increasing order and sums its
 // elements in column order, one fmaf per element and x row; the caller then folds the 32 partial sums with warp_sum's
 // fixed xor butterfly.  The order is therefore fixed by K and BITS alone: neither the grid, the chunking of x nor the
 // row count m changes a single bit of a sum.
@@ -36,7 +37,7 @@ __device__ __forceinline__ void load_unit_table(float* s_unit, const float* __re
 // from one of its quads to the next) and quad_aligned (packed 16-byte aligned and K*bits a multiple of 128).
 constexpr int kPlWarps = 8;
 constexpr int kPlThreads = kPlWarps * 32;
-constexpr int kPlRowsPerWarp = 4;
+constexpr int kPlRowsPerWarp = 4;                    // rows per warp of qd_packed_linear and the LSTM cell
 constexpr size_t kPlSmemBytes = 96 * 1024;           // x tile, unless one warp-wide step of MT rows needs more
 
 // position of float4 group g of a tile row: bits 0-2 XOR-ed with the quad index (E float4 groups per quad)
@@ -90,33 +91,34 @@ __device__ __forceinline__ void pl_stage(float4* s_x, Row row, int64_t m0, int64
     }
 }
 
-// Adds this lane's share of chunk c of the four weight rows orow[] times the staged x rows to acc[row][x row]: quads
+// Adds this lane's share of chunk c of the R weight rows orow[] times the staged x rows to acc[row][x row]: quads
 // d = c*kq + lane, +32, ... below min(qpr, (c+1)*kq), where kq = kc / (4*E) is the quads per chunk and qpr the quads
-// per weight row.
-template <int BITS, int MT, class A>
+// per weight row.  Each row's sum is walked on its own (its codes, its bucket cursor, its accumulators), so a row's
+// bits do not depend on R: qd_packed_linear and the LSTM cell walk four rows per warp, the GRU cell three.
+template <int BITS, int MT, int R, class A>
 __device__ __forceinline__ void pl_walk(const A& a, const float* s_unit, const float4* s_x, int kc4, int64_t kq, int64_t qpr, int64_t c,
-                                        int lane, const int64_t (&orow)[kPlRowsPerWarp], float (&acc)[kPlRowsPerWarp][MT]) {
+                                        int lane, const int64_t (&orow)[R], float (&acc)[R][MT]) {
     constexpr int E = 32 / BITS, E4 = E / 4;
     constexpr unsigned mask = (1u << BITS) - 1u;
     const int64_t d_first = c * kq + lane, d_end = min(qpr, (c + 1) * kq);
     if (d_first >= d_end) return;
-    int64_t bk[kPlRowsPerWarp], rk[kPlRowsPerWarp];   // bucket of the quad's first element, offset in it
+    int64_t bk[R], rk[R];                           // bucket of the quad's first element, offset in it
 #pragma unroll
-    for (int r = 0; r < kPlRowsPerWarp; ++r) {
+    for (int r = 0; r < R; ++r) {
         const int64_t e0 = orow[r] * a.K + d_first * 4 * E;
         bk[r] = e0 / a.L;
         rk[r] = e0 - bk[r] * a.L;
     }
     for (int64_t d = d_first; d < d_end; d += 32) {
-        uint4 cq[kPlRowsPerWarp];
+        uint4 cq[R];
 #pragma unroll
-        for (int r = 0; r < kPlRowsPerWarp; ++r) cq[r] = pl_quad<BITS>(a, orow[r] * a.K + d * 4 * E);
+        for (int r = 0; r < R; ++r) cq[r] = pl_quad<BITS>(a, orow[r] * a.K + d * 4 * E);
         // per row, a cursor (bucket bc, offset rc) that walks the quad's elements in order: alpha / beta are
         // fetched once per bucket, and a bucket ending inside the quad costs one compare per element
-        float al[kPlRowsPerWarp], be[kPlRowsPerWarp];
-        int64_t bc[kPlRowsPerWarp], rc[kPlRowsPerWarp];
+        float al[R], be[R];
+        int64_t bc[R], rc[R];
 #pragma unroll
-        for (int r = 0; r < kPlRowsPerWarp; ++r) {
+        for (int r = 0; r < R; ++r) {
             bc[r] = bk[r];
             rc[r] = rk[r];
             al[r] = __ldg(a.alpha + bc[r]);
@@ -131,9 +133,9 @@ __device__ __forceinline__ void pl_walk(const A& a, const float* s_unit, const f
         for (int u = 0; u < 4; ++u) {
 #pragma unroll 1
             for (int t = 0; t < E4; ++t) {
-                float q[kPlRowsPerWarp][4];
+                float q[R][4];
 #pragma unroll
-                for (int r = 0; r < kPlRowsPerWarp; ++r) {
+                for (int r = 0; r < R; ++r) {
                     const uint32_t cw = u == 0 ? cq[r].x : u == 1 ? cq[r].y : u == 2 ? cq[r].z : cq[r].w;
 #pragma unroll
                     for (int jj = 0; jj < 4; ++jj) {
@@ -151,7 +153,7 @@ __device__ __forceinline__ void pl_walk(const A& a, const float* s_unit, const f
                 for (int i = 0; i < MT; ++i) {
                     const float4 xv = s_x[i * kc4 + pl_slot<BITS>(gbase + u * E4 + t)];
 #pragma unroll
-                    for (int r = 0; r < kPlRowsPerWarp; ++r) {
+                    for (int r = 0; r < R; ++r) {
                         acc[r][i] = __fmaf_rn(xv.x, q[r][0], acc[r][i]);
                         acc[r][i] = __fmaf_rn(xv.y, q[r][1], acc[r][i]);
                         acc[r][i] = __fmaf_rn(xv.z, q[r][2], acc[r][i]);
@@ -161,7 +163,7 @@ __device__ __forceinline__ void pl_walk(const A& a, const float* s_unit, const f
             }
         }
 #pragma unroll
-        for (int r = 0; r < kPlRowsPerWarp; ++r) {
+        for (int r = 0; r < R; ++r) {
             bk[r] += a.step_q;
             rk[r] += a.step_r;
             if (rk[r] >= a.L) { rk[r] -= a.L; ++bk[r]; }

@@ -121,5 +121,20 @@ for bits, I, Hd, bucket in ((1, 7, 5, 100), (2, 33, 17, 3), (4, 129, 250, 256), 
         cell.CROSSOVER_ROWS = N.PACKED_LSTM_MAX_ROWS
         for m_rows in (1, 4, 8):
             cell(torch.randn(m_rows, I).cuda())
+# packed GRU cell and layer: the same sizes, buckets and row tiles, a bidirectional two-layer GRU over an unsorted
+# PackedSequence
+for bits, I, Hd, bucket in ((1, 7, 5, 100), (2, 33, 17, 3), (4, 129, 250, 256), (8, 10, 9, None)):
+    gru_pm = codec.pack_model(torch.nn.GRU(I, Hd, num_layers=2, bidirectional=True).cuda(), bits, bucket)
+    net = torch.nn.Sequential(torch.nn.GRU(I, Hd, num_layers=2, bidirectional=True)).cuda()
+    assert codec.attach_packed_(gru_pm, net, gru=True) == ["0"]
+    xs = torch.nn.utils.rnn.pack_padded_sequence(torch.randn(6, 8, I).cuda(), torch.tensor([6, 1, 3, 6, 2, 5, 4, 1]), enforce_sorted=False)
+    net[0].CROSSOVER_ROWS = N.PACKED_GRU_MAX_ROWS                   # the kernel path, not decode + torch
+    with torch.no_grad():
+        net[0](xs)
+        cell_pm = codec.pack_model(torch.nn.GRUCell(I, Hd).cuda(), bits, bucket)
+        cell = codec.PackedGRUCell(cell_pm.tensors[0], cell_pm.tensors[1], "uniform", 1 << bits, bucket)
+        cell.CROSSOVER_ROWS = N.PACKED_GRU_MAX_ROWS
+        for m_rows in (1, 4, 8):
+            cell(torch.randn(m_rows, I).cuda())
 torch.cuda.synchronize()
 print("sanitize probe ok")
