@@ -123,7 +123,10 @@ int qd_uniform_fwd(const float* x, float* q, uint8_t* idx_u8, float* alpha, floa
 int qd_uniform_bwd(const float* x, const float* g, float* gout, int64_t n, int64_t bucket, int levels, int mode,
                    void* workspace, size_t workspace_bytes, qd_stream_t stream);
 
-/* forward + backward in one pass over (x, g): 16 bytes per element. */
+/* forward + backward in one pass over (x, g): 16 bytes per element.  q may alias x and gout may alias g, one or both
+ * (the same pointer, as an in-place training step passes them); the results are the bits of the call without aliasing.
+ * No other overlap of the four arrays is allowed.  q is qd_uniform_fwd's q; gout is qd_uniform_bwd's in the same mode,
+ * refused where that one is (for QD_BWD_MINMAX the two may add the terms of r_b in another order). */
 int qd_uniform_fwd_bwd(const float* x, const float* g, float* q, float* gout, int64_t n, int64_t bucket,
                        int levels, int mode, void* workspace, size_t workspace_bytes, qd_stream_t stream);
 

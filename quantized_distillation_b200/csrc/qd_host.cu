@@ -119,6 +119,13 @@ int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t 
     int64_t rows, row_len, padded;
     rc = qd_bucket_geometry(n, bucket, &rows, &row_len, &padded);
     if (rc) return rc;
+    // what the fused op refuses, refused before any copy is enqueued: an error return leaves no transfer in flight on
+    // the caller's buffers and nothing written to the outputs
+    if (bwd && mode != QD_BWD_STE && mode != QD_BWD_TRUNCATED && mode != QD_BWD_MINMAX)
+        return fail(QD_ERR_INVALID_ARG, "unknown backward mode %d", mode);
+    if (bwd && mode == QD_BWD_MINMAX && (bucket == 0 || row_len > QD_MAX_STAGED_BUCKET))
+        return fail(QD_ERR_UNSUPPORTED, "minmax backward needs a bucket of at most %d floats (quant_functions.py:332-334)",
+                    QD_MAX_STAGED_BUCKET);
 
     if (row_len > chunk_elems) {
         // one row spans more than a chunk (bucket None on a large tensor): no row-aligned
@@ -145,7 +152,10 @@ int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t 
                                       c->big_ws_bytes, s)
                  : qd_uniform_fwd(c->big_x, c->big_q, nullptr, nullptr, nullptr, nullptr, nullptr, n, bucket, levels,
                                   nullptr, 0.f, 0, 0, 0, c->big_ws, c->big_ws_bytes, s);
-        if (rc) return rc;
+        if (rc) {
+            cudaStreamSynchronize(s);  // the copies above still read the caller's buffers
+            return rc;
+        }
         QD_CUDA(cudaMemcpyAsync(hq, c->big_q, bytes, cudaMemcpyDeviceToHost, s));
         if (bwd) QD_CUDA(cudaMemcpyAsync(hgout, c->big_gout, bytes, cudaMemcpyDeviceToHost, s));
         QD_CUDA(cudaStreamSynchronize(s));
@@ -185,7 +195,10 @@ int run_host(const float* hx, const float* hg, float* hq, float* hgout, int64_t 
         rc = bwd ? qd_uniform_fwd_bwd(s.x, s.g, s.q, s.gout, len, bucket, levels, mode, s.ws, s.ws_bytes, s.stream)
                  : qd_uniform_fwd(s.x, s.q, nullptr, nullptr, nullptr, nullptr, nullptr, len, bucket, levels, nullptr,
                                   0.f, 0, 0, 0, s.ws, s.ws_bytes, s.stream);
-        if (rc) return rc;
+        if (rc) {
+            for (int i = 0; i < kSlots; ++i) cudaStreamSynchronize(c->slot[i].stream);  // copies of earlier chunks in flight
+            return rc;
+        }
         QD_CUDA(cudaMemcpyAsync(hq + off, s.q, bytes, cudaMemcpyDeviceToHost, s.stream));
         if (bwd) QD_CUDA(cudaMemcpyAsync(hgout + off, s.gout, bytes, cudaMemcpyDeviceToHost, s.stream));
     }

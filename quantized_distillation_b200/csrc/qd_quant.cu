@@ -32,15 +32,20 @@ extern "C" int qd_bucket_geometry(int64_t n, int64_t bucket, int64_t* rows, int6
 static constexpr size_t kPointsGradMaxCtas = 132 * 8;  // 8 CTAs per SM of a 132-SM H100 SXM; bigger parts are capped here
 static size_t points_grad_ws_bytes() { return kPointsGradMaxCtas * 256 * sizeof(double); }
 
-extern "C" size_t qd_workspace_bytes(int64_t n, int64_t bucket) {
-    Geometry g;
-    if (geometry_of(n, bucket, &g)) return 0;
+// the workspace a geometry needs: what qd_workspace_bytes states, and what the grid path checks it has
+static size_t workspace_bytes_of(const Geometry& g) {
     size_t bytes = points_grad_ws_bytes();
     if (g.row_len > QD_MAX_STAGED_BUCKET) {
         size_t grid = (size_t)(g.rows * grid_chunks_per_row(g)) * sizeof(ChunkPartial) + (size_t)g.rows * sizeof(RowStat) + 256;
         if (grid > bytes) bytes = grid;
     }
     return bytes + 256;
+}
+
+extern "C" size_t qd_workspace_bytes(int64_t n, int64_t bucket) {
+    Geometry g;
+    if (geometry_of(n, bucket, &g)) return 0;
+    return workspace_bytes_of(g);
 }
 
 // ------------------------------------------------------------------ launchers
@@ -153,7 +158,8 @@ template <int OP, int BWD>
 static int launch_grid(const Params& P, void* ws, size_t ws_bytes, cudaStream_t s) {
     const int64_t cpr = grid_chunks_per_row(P.geo);
     const int64_t items = P.geo.rows * cpr;
-    const size_t need = (size_t)items * sizeof(ChunkPartial) + (size_t)P.geo.rows * sizeof(RowStat);
+    // the stated size, not just the bytes used below: a caller that passes less is refused on every geometry alike
+    const size_t need = workspace_bytes_of(P.geo);
     if (ws == nullptr || ws_bytes < need) return fail(QD_ERR_WORKSPACE, "workspace of %zu bytes needed, %zu given", need, ws_bytes);
     ChunkPartial* partial = reinterpret_cast<ChunkPartial*>(ws);
     RowStat* rowstat = reinterpret_cast<RowStat*>(partial + items);
