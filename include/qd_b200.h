@@ -306,6 +306,37 @@ int qd_packed_gru_layer(const float* x, int64_t ldx, const int64_t* batch_sizes,
                         int64_t hidden_size, const qd_packed_tensor* w_ih, const qd_packed_tensor* w_hh, int levels, int64_t bucket,
                         const float* b_ih, const float* b_hh, const float* h0, float* out, int64_t ldo, float* h_n, qd_stream_t stream);
 
+/* ---- the NMT loss over the target vocabulary (onmt/Loss.py:97-120, NMTLossCompute.compute_loss) ----------
+ * logits, teacher_logits: float32[rows, V], C order, any 4-byte alignment (16-byte aligned rows load 128 bits at a
+ * time; the results do not depend on alignment).  teacher_logits may be NULL (no distillation term).  target: int64[rows].
+ * padding_idx: -1 (none) or in [0, V).  w (weight_teacher_loss) in [0, 1]; ignored without a teacher.  Per row with
+ * target y, lse_s = log sum_c exp(z_s), lse_t likewise over z_t, S_t = sum_c exp(z_t - m_t) for the row maximum m_t,
+ * A = sum_c exp(z_t - m_t) (z_t - z_s), where a column with z_t = -inf adds 0 and a column with z_t finite and
+ * z_s = -inf makes A (and the loss) +inf, however small its teacher probability:
+ *   y == padding_idx: loss_i = 0, counted nowhere, gradient row 0;
+ *   y outside [0, V) otherwise: never dereferenced; loss_i and the gradient row are NaN, counted in n_invalid;
+ *   else without a teacher: loss_i = lse_s - z_s[y]; with one: (1-w)(lse_s - z_s[y]) + w (A/S_t - lse_t + lse_s);
+ *        counted in n_words, and in n_correct when y is the first-occurrence argmax of z_s.
+ * The sums run in float64 over IEEE expf terms, in an order fixed by V alone: a row gives the same bits alone or at any
+ * position of any batch, and two calls give the same bits.  A row whose student logits are all -inf has lse_s = -inf
+ * and a NaN loss and gradient, as the log-softmax has; the argmax of a row holding NaN is unspecified.
+ * Neither call synchronises or allocates (graph-capturable). */
+size_t qd_nmt_loss_workspace_bytes(int64_t rows);
+/* row_lse: float32[rows][2] = (lse_s, lse_t; 0 without a teacher), read by the backward.  loss: one device float32,
+ * sum_i loss_i rounded once.  counts: device int64[3] = n_words, n_correct, n_invalid.  workspace: device, 16-byte
+ * aligned, >= qd_nmt_loss_workspace_bytes(rows) bytes (may be NULL when that is 0), else QD_ERR_WORKSPACE.  rows may be
+ * 0 (loss 0, counts 0).  QD_ERR_INVALID_ARG: NULL or misaligned pointers, rows < 0, V < 1, rows*V past 64-bit
+ * indexing, padding_idx or w out of range, outputs overlapping the inputs or each other. */
+int qd_nmt_loss_fwd(const float* logits, const float* teacher_logits, const int64_t* target, int64_t rows, int64_t V,
+                    int64_t padding_idx, float w, float* row_lse, float* loss, int64_t* counts, void* workspace,
+                    size_t workspace_bytes, qd_stream_t stream);
+/* grad_logits[i, c] = g (exp(z_s - lse_s) - w exp(z_t - lse_t) - (1-w)[c = y]), g = *grad_loss (a device float32
+ * read by the kernel), float32 ops in that order; row_lse from qd_nmt_loss_fwd on the same inputs.  Padding rows get 0,
+ * invalid targets NaN.  grad_logits: float32[rows, V], must not overlap the inputs.  Same checks as the forward. */
+int qd_nmt_loss_bwd(const float* logits, const float* teacher_logits, const int64_t* target, const float* row_lse,
+                    const float* grad_loss, int64_t rows, int64_t V, int64_t padding_idx, float w, float* grad_logits,
+                    qd_stream_t stream);
+
 /* ---- next row f2: Huffman-coded storage (the model helpers/functions.py:226-262 only sizes) ----------
  * Canonical code over uint8 symbols, codes of 1..QD_HUFFMAN_MAX_LENGTH bits (built on the host: codec.py).
  * Stream: a tensor's symbols are cut into chunks of QD_HUFFMAN_CHUNK; each chunk's codes are written MSB-first

@@ -61,6 +61,9 @@ SIGNATURES = {
     "qd_packed_lstm_layer": (C.c_int, [_p, _i64, _p, _i64, _i32, _i64, _i64, _p, _p, _i32, _i64, _p, _p, _p, _p, _p, _i64, _p, _p, _p]),
     "qd_packed_gru_cell": (C.c_int, [_p, _i64, _p, _i64, _i64, _i64, _i64, _p, _p, _i32, _i64, _p, _p, _p, _i64, _p]),
     "qd_packed_gru_layer": (C.c_int, [_p, _i64, _p, _i64, _i32, _i64, _i64, _p, _p, _i32, _i64, _p, _p, _p, _p, _i64, _p, _p]),
+    "qd_nmt_loss_workspace_bytes": (_sz, [_i64]),
+    "qd_nmt_loss_fwd": (C.c_int, [_p, _p, _p, _i64, _i64, _i64, _f32, _p, _p, _p, _p, _sz, _p]),
+    "qd_nmt_loss_bwd": (C.c_int, [_p, _p, _p, _p, _p, _i64, _i64, _i64, _f32, _p, _p]),
     "qd_huffman_encode":(C.c_int, [_p, _i64, _p, _p, _i64, _p, _p, _p]),
     "qd_huffman_decode_dequant_uniform": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _i64, _i64, _i32, _p]),
     "qd_huffman_decode_dequant_nonuniform": (C.c_int, [_p, _i64, _p, _p, _p, _i32, _p, _p, _p, _i64, _i64, _p]),

@@ -136,5 +136,18 @@ for bits, I, Hd, bucket in ((1, 7, 5, 100), (2, 33, 17, 3), (4, 129, 250, 256), 
         cell.CROSSOVER_ROWS = N.PACKED_GRU_MAX_ROWS
         for m_rows in (1, 4, 8):
             cell(torch.randn(m_rows, I).cuda())
+# fused NMT loss, forward and backward: rows shorter than a group of four, odd rows (every 16-byte phase), rows of
+# several groups per thread, with and without a teacher, padding and out-of-range targets, and an offset view
+from quantized_distillation_b200.nmt_loss import nmt_loss  # noqa: E402
+for R, V in ((3, 1), (5, 3), (7, 1025), (4, 10_004)):
+    for teacher in (False, True):
+        buf = torch.randn(R * V + 1, device="cuda")
+        zs = (buf[1:] if V > 4 else buf[:R * V]).view(R, V).detach().requires_grad_(True)
+        zt = torch.randn(R, V, device="cuda") if teacher else None
+        tg = torch.randint(0, V, (R,), device="cuda")
+        tg[0] = 0
+        tg[-1] = V + 2
+        loss, stats = nmt_loss(zs, tg, 0, zt)
+        loss.backward()
 torch.cuda.synchronize()
 print("sanitize probe ok")
