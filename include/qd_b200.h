@@ -337,6 +337,29 @@ int qd_nmt_loss_bwd(const float* logits, const float* teacher_logits, const int6
                     const float* grad_loss, int64_t rows, int64_t V, int64_t padding_idx, float w, float* grad_logits,
                     qd_stream_t stream);
 
+/* ---- one beam search step of B sentences (onmt/Beam.py:55-106, Beam.advance; Translator.translateBatch) ----------
+ * Rows follow onmt's beam-major decoder batch: row r = k*B + b is beam k of sentence b (K = beam).  out: float32
+ * [K*B, V], C order, any 4-byte alignment.  With normalize = 0 it holds log-probabilities lp; with normalize = 1 the
+ * generator Linear's logits x, and lp = fl(x - lse) with lse bit-identical to qd_nmt_loss_fwd's lse_s of the same row.
+ * scores, last_tokens, origin, flat_origin, tokens: [K*B]; n_finished, eos_top: [B].  Per sentence b, the key of row k,
+ * column j is lp[0, j] on the first step (rows k > 0 take no part and last_tokens is not read); otherwise -1e20f in
+ * every column when last_tokens[r] == eos (such a row is never read), else fl(lp[k, j] + scores[k]).  The K selected
+ * entries are the top K of the K*V keys, keys descending, a tie to the lower flat index k*V + j, NaN above every number
+ * (as torch.topk) and -0 equal to +0.  Selected entry i of sentence b goes to row i*B + b: scores = its key,
+ * origin = flat / V, tokens = flat mod V, flat_origin = origin*B + b (the index that reorders the decoder state);
+ * n_finished[b] += the selected tokens equal to eos; eos_top[b] = 1 when beam 0's token is eos (else unchanged).
+ * scores, n_finished and eos_top are updated in place; nothing else may overlap.  workspace: device, 16-byte aligned,
+ * >= qd_beam_workspace_bytes(batch, beam).  No atomics, no synchronisation, no allocation: deterministic and
+ * graph-capturable.  QD_ERR_INVALID_ARG: NULL or misaligned pointers (float arrays 4 bytes, int64 arrays 8,
+ * n_finished 4), beam outside [1, QD_BEAM_MAX], batch < 0, normalize not 0 or 1, V < beam or V >= 2^32, eos outside
+ * [0, V), batch*beam*V past 64-bit indexing, overlapping arrays; QD_ERR_WORKSPACE: a short workspace.  batch 0 does
+ * nothing. */
+#define QD_BEAM_MAX 16
+size_t qd_beam_workspace_bytes(int64_t batch, int beam);
+int qd_beam_step(const float* out, int normalize, int64_t batch, int beam, int64_t V, int64_t eos, int first_step,
+                 float* scores, const int64_t* last_tokens, int64_t* origin, int64_t* flat_origin, int64_t* tokens,
+                 int32_t* n_finished, uint8_t* eos_top, void* workspace, size_t workspace_bytes, qd_stream_t stream);
+
 /* ---- next row f2: Huffman-coded storage (the model helpers/functions.py:226-262 only sizes) ----------
  * Canonical code over uint8 symbols, codes of 1..QD_HUFFMAN_MAX_LENGTH bits (built on the host: codec.py).
  * Stream: a tensor's symbols are cut into chunks of QD_HUFFMAN_CHUNK; each chunk's codes are written MSB-first

@@ -22,6 +22,7 @@ MAX_STAGED_BUCKET = 49152
 PACKED_LINEAR_MAX_ROWS = 64     # QD_PACKED_LINEAR_MAX_ROWS
 PACKED_LSTM_MAX_ROWS = 64       # QD_PACKED_LSTM_MAX_ROWS
 PACKED_GRU_MAX_ROWS = 64        # QD_PACKED_GRU_MAX_ROWS
+BEAM_MAX = 16                   # QD_BEAM_MAX
 
 _p, _i64, _i32, _u64, _f32, _sz = C.c_void_p, C.c_int64, C.c_int, C.c_uint64, C.c_float, C.c_size_t
 
@@ -64,6 +65,8 @@ SIGNATURES = {
     "qd_nmt_loss_workspace_bytes": (_sz, [_i64]),
     "qd_nmt_loss_fwd": (C.c_int, [_p, _p, _p, _i64, _i64, _i64, _f32, _p, _p, _p, _p, _sz, _p]),
     "qd_nmt_loss_bwd": (C.c_int, [_p, _p, _p, _p, _p, _i64, _i64, _i64, _f32, _p, _p]),
+    "qd_beam_workspace_bytes": (_sz, [_i64, _i32]),
+    "qd_beam_step": (C.c_int, [_p, _i32, _i64, _i32, _i64, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
     "qd_huffman_encode":(C.c_int, [_p, _i64, _p, _p, _i64, _p, _p, _p]),
     "qd_huffman_decode_dequant_uniform": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _i64, _i64, _i32, _p]),
     "qd_huffman_decode_dequant_nonuniform": (C.c_int, [_p, _i64, _p, _p, _p, _i32, _p, _p, _p, _i64, _i64, _p]),

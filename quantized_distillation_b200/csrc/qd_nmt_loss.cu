@@ -15,12 +15,13 @@
 #include <cmath>
 
 #include "qd_launch.h"
+#include "qd_lse.cuh"
 
 using namespace qd;
 
 namespace {
 
-constexpr int kNlThreads = 256;      // per row, forward and backward
+constexpr int kNlThreads = kLseThreads;   // per row, forward and backward; the lse walk of qd_lse.cuh
 constexpr int kNlReduceThreads = 512;
 
 enum RowKind : int { kRowPad = 0, kRowWord = 1, kRowCorrect = 2, kRowInvalid = 3 };
@@ -41,44 +42,23 @@ struct NlArgs {
     double w;
 };
 
-__device__ __forceinline__ bool aligned16_dev(const float* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
-// group k (columns 4k .. 4k+3) of a row; columns at or past V read as -inf and are never loaded
-__device__ __forceinline__ void load_group(const float* row, bool vec, int64_t c, int64_t V, float (&v)[4]) {
-    if (vec && c + 4 <= V) {
-        const float4 q = __ldg(reinterpret_cast<const float4*>(row + c));
-        v[0] = q.x, v[1] = q.y, v[2] = q.z, v[3] = q.w;
-    } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) v[j] = c + j < V ? __ldg(row + c + j) : -INFINITY;
-    }
-}
-
-// (m, s) <- the pair rescaled to max m_new >= m; s is 0 while m is -inf
-__device__ __forceinline__ double rescale(float m, float m_new) {
-    return m == -INFINITY ? 0.0 : exp((double)m - (double)m_new);
-}
-
 // a * f for a rescale factor f in [0, 1]; an infinite cross term stays infinite (inf * 0 would be NaN)
 __device__ __forceinline__ double scale_a(double a, double f) { return isinf(a) ? a : a * f; }
 
 struct Online {                      // one thread's state over its columns
-    float ms = -INFINITY, mt = -INFINITY, best = -INFINITY;
-    double ss = 0.0, st = 0.0, a = 0.0;
+    LseAcc s;                        // the student's (max, sum)
+    float mt = -INFINITY, best = -INFINITY;
+    double st = 0.0, a = 0.0;
     int64_t arg = -1;
 };
 
 template <bool TEACHER>
 __device__ __forceinline__ void absorb(Online& o, const float (&s)[4], const float (&t)[4], int64_t c) {
-    float gm = fmaxf(fmaxf(s[0], s[1]), fmaxf(s[2], s[3]));
-    if (gm > o.ms) {
-        o.ss *= rescale(o.ms, gm);
-        o.ms = gm;
-    }
+    lse_absorb(o.s, s);
     if (TEACHER) {
         float gt = fmaxf(fmaxf(t[0], t[1]), fmaxf(t[2], t[3]));
         if (gt > o.mt) {
-            const double f = rescale(o.mt, gt);
+            const double f = lse_rescale(o.mt, gt);
             o.st *= f;
             o.a = scale_a(o.a, f);
             o.mt = gt;
@@ -86,8 +66,6 @@ __device__ __forceinline__ void absorb(Online& o, const float (&s)[4], const flo
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-        // -inf (and the columns past V) add exactly 0; NaN propagates into the sums
-        if (s[j] != -INFINITY) o.ss += (double)expf(__fsub_rn(s[j], o.ms));
         if (o.arg < 0 || s[j] > o.best) {
             o.best = s[j];
             o.arg = c + j;
@@ -106,12 +84,10 @@ __device__ __forceinline__ void absorb(Online& o, const float (&s)[4], const flo
 // o <- o combined with p; an argmax tie keeps the lower column
 template <bool TEACHER>
 __device__ __forceinline__ void combine(Online& o, const Online& p) {
-    const float ms = fmaxf(o.ms, p.ms);
-    o.ss = o.ss * rescale(o.ms, ms) + p.ss * rescale(p.ms, ms);
-    o.ms = ms;
+    lse_combine(o.s, p.s);
     if (TEACHER) {
         const float mt = fmaxf(o.mt, p.mt);
-        const double fo = rescale(o.mt, mt), fp = rescale(p.mt, mt);
+        const double fo = lse_rescale(o.mt, mt), fp = lse_rescale(p.mt, mt);
         o.st = o.st * fo + p.st * fp;
         o.a = scale_a(o.a, fo) + scale_a(p.a, fp);
         o.mt = mt;
@@ -162,7 +138,7 @@ __global__ void __launch_bounds__(kNlThreads) nmt_loss_fwd_kernel(NlArgs a) {
         }
         if (threadIdx.x == 0) {
             const Online f = s_o[0];
-            const double lse_s = (double)f.ms + log(f.ss);
+            const double lse_s = lse_value(f.s);
             const double lse_t = TEACHER ? (double)f.mt + log(f.st) : 0.0;
             a.row_lse[2 * r] = (float)lse_s;
             a.row_lse[2 * r + 1] = (float)lse_t;

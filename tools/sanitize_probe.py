@@ -149,5 +149,15 @@ for R, V in ((3, 1), (5, 3), (7, 1025), (4, 10_004)):
         tg[-1] = V + 2
         loss, stats = nmt_loss(zs, tg, 0, zt)
         loss.backward()
+# beam search step: every row-list width, V = K (one group) to several groups per thread, an offset (unaligned) view,
+# the first step and a later one with a row that ended on EOS, on logits and on log-probabilities
+from quantized_distillation_b200.beam import BatchBeam  # noqa: E402
+for K, B, V in ((1, 3, 1), (2, 1, 5), (5, 7, 1025), (16, 2, 10_004)):
+    bb = BatchBeam(B, K, 2, 0, V - 1, 0, 3, "cuda")
+    for t, normalized in enumerate((False, True, False)):
+        buf = torch.randn(K * B * V + 1, device="cuda")
+        bb.advance(buf[1:].view(K * B, V), torch.rand(K * B, 4, device="cuda"), normalized)
+        bb.tokens[t + 1, 0, 0] = V - 1
+    bb.done()
 torch.cuda.synchronize()
 print("sanitize probe ok")
