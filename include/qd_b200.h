@@ -131,15 +131,23 @@ int qd_uniform_fwd_bwd(const float* x, const float* g, float* q, float* gout, in
                        int levels, int mode, void* workspace, size_t workspace_bytes, qd_stream_t stream);
 
 /* ---- a6/a7: nonUniformQuantization (quant_functions.py:196-290, 509-573) -
- * points[K] device, sorted ascending; idx_u8 (K <= 256) and/or idx_i64 optional. */
+ * points[K] device, sorted ascending; idx_u8 (K <= 256) and/or idx_i64 optional.
+ * q may alias x (modify_in_place); no other overlap of x with an output is allowed.
+ * Index of a NaN x_hat is K-1 under both rules, as in the reference, and every
+ * index is < K (x_hat = +inf gets K-1 whatever the table size).  A NaN x_hat
+ * arises from finite input too: a row whose max - min overflows has alpha = +inf
+ * and x_hat = inf/inf at its maximum.  The same rule holds in qd_centroid_index,
+ * qd_nonuniform_fwd_packed and the centroid plans. */
 int qd_nonuniform_fwd(const float* x, const float* points, int num_points, int rule, float* q, uint8_t* idx_u8,
                       int64_t* idx_i64, float* alpha, float* beta, int64_t n, int64_t bucket, const float* mean,
                       float max_element, void* workspace, size_t workspace_bytes, qd_stream_t stream);
 
 /* ---- a8: nonUniformQuantization_variable.backward (quant_functions.py:471-506)
  * grad_points[K] = sum_{i: idx_i = k} fl32(g_i * alpha_row(i)); exactly one of
- * idx_u8 / idx_i64 non-NULL.  Deterministic (fixed reduction tree, float64
- * accumulation), so data-parallel replicas stay bit-identical. */
+ * idx_u8 / idx_i64 non-NULL.  Indices outside [0, num_points) add nothing.
+ * Deterministic (fixed reduction tree, float64 accumulation), so data-parallel
+ * replicas stay bit-identical.  The workspace must hold qd_workspace_bytes(n,
+ * bucket) bytes; less, or NULL, is QD_ERR_WORKSPACE with nothing written. */
 int qd_nonuniform_bwd(const float* g, const uint8_t* idx_u8, const int64_t* idx_i64, const float* alpha,
                       int num_points, float* grad_points, int64_t n, int64_t bucket,
                       void* workspace, size_t workspace_bytes, qd_stream_t stream);

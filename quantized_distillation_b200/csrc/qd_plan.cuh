@@ -145,7 +145,8 @@ __device__ __forceinline__ void nu_load_tables(LaneSearch<KP>& ls, const float* 
     const float k0 = (lane < K) ? __ldg(points + lane) : inf;
     const float k1 = (lane + 1 < K) ? __ldg(points + lane + 1) : inf;
     ls.k_lane = k0;
-    ls.t_lane = (lane + 1 < K) ? __fadd_rn(k0, __fmul_rn(__fsub_rn(k1, k0), 0.5f)) : inf;
+    // NaN beyond K-2, as in centroid_setup: the search never counts it, even for NaN / +inf x_hat
+    ls.t_lane = (lane + 1 < K) ? __fadd_rn(k0, __fmul_rn(__fsub_rn(k1, k0), 0.5f)) : __int_as_float(0x7fffffff);
     ls.t1 = (KP >= 2) ? __shfl_sync(kFullMask, ls.t_lane, KP / 2 - 1) : 0.f;
     ls.t2lo = (KP >= 4) ? __shfl_sync(kFullMask, ls.t_lane, KP / 4 - 1) : 0.f;
     ls.t2hi = (KP >= 4) ? __shfl_sync(kFullMask, ls.t_lane, 3 * KP / 4 - 1) : 0.f;

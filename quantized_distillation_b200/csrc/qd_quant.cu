@@ -459,6 +459,8 @@ __global__ void __launch_bounds__(kPgThreads) points_grad_partial(const float* _
     const int64_t tiles_per_row = (geo.row_len + kPgTile - 1) / kPgTile;
     const int64_t items = tile_mode ? (geo.n + kPgTile - 1) / kPgTile : geo.rows * tiles_per_row;
     const int64_t stride = (int64_t)gridDim.x * kPgWarps;
+    // index minus sweep base, unsigned: negative indices and indices >= K fall outside [0, kcount) (int64: all 64 bits)
+    using IdU = typename std::conditional<sizeof(IdxT) == 8, uint64_t, unsigned>::type;
     const bool vec_ok = sizeof(IdxT) == 1 && ((reinterpret_cast<uintptr_t>(g) & 15) == 0) &&
                         ((reinterpret_cast<uintptr_t>(idx) & 3) == 0);
 
@@ -501,8 +503,8 @@ __global__ void __launch_bounds__(kPgThreads) points_grad_partial(const float* _
                     for (int e = lane; e < len; e += 32) {
                         const int64_t ge = start + e;
                         const float a = (geo.rows == 1) ? alpha[0] : alpha[ge / geo.row_len];
-                        const unsigned id = (unsigned)idx[ge] - (unsigned)kg;
-                        if (id < (unsigned)kcount) col[id][lane] += __fmul_rn(g[ge], a);
+                        const IdU id = (IdU)idx[ge] - (IdU)kg;
+                        if (id < (IdU)kcount) col[id][lane] += __fmul_rn(g[ge], a);
                     }
                 }
             } else {
@@ -512,8 +514,8 @@ __global__ void __launch_bounds__(kPgThreads) points_grad_partial(const float* _
                 const int len = (int)min((int64_t)kPgTile, row_end - start);
                 const float a = alpha[row];
                 for (int e = lane; e < len; e += 32) {
-                    const unsigned id = (unsigned)idx[start + e] - (unsigned)kg;
-                    if (id < (unsigned)kcount) col[id][lane] += __fmul_rn(g[start + e], a);
+                    const IdU id = (IdU)idx[start + e] - (IdU)kg;
+                    if (id < (IdU)kcount) col[id][lane] += __fmul_rn(g[start + e], a);
                 }
             }
             if (++since_flush == kPgFlushEvery) {
@@ -571,7 +573,9 @@ extern "C" int qd_nonuniform_bwd(const float* g, const uint8_t* idx_u8, const in
     int rc = capped_grid((items + kPgWarps - 1) / kPgWarps, 8, &grid);
     if (rc) return rc;
     if (grid > (int)kPointsGradMaxCtas) grid = (int)kPointsGradMaxCtas;
-    const size_t need = (size_t)grid * num_points * sizeof(double);
+    // the stated size, qd_workspace_bytes(n, bucket), not just the grid * K partials this launch uses: a caller
+    // that sizes its buffer by some other rule is told so on every geometry, not only on the large ones
+    const size_t need = workspace_bytes_of(geo);
     if (workspace == nullptr || workspace_bytes < need) return fail(QD_ERR_WORKSPACE, "workspace of %zu bytes needed, %zu given", need, workspace_bytes);
     double* partial = reinterpret_cast<double*>(workspace);
     cudaStream_t s = as_stream(stream);
