@@ -368,6 +368,50 @@ int qd_beam_step(const float* out, int normalize, int64_t batch, int beam, int64
                  float* scores, const int64_t* last_tokens, int64_t* origin, int64_t* flat_origin, int64_t* tokens,
                  int32_t* n_finished, uint8_t* eos_top, void* workspace, size_t workspace_bytes, qd_stream_t stream);
 
+/* ---- the n_best hypotheses of B finished beam searches (onmt/Beam.py:108-133, sortFinished(minimum=n_best) and
+ * getHyp; Translator.translateBatch) from the histories of steps = T calls of qd_beam_step ------------------------------
+ * tokens: int64 [T+1, K, B] (tokens[t] the input of step t, tokens[t+1] its selected tokens); origins: int64 [T, K, B];
+ * step_scores: float32 [T, K, B] (the scores after step t); attn: float32 [T, K, B, S], S = src_len (the attention of
+ * step t gathered by origin).  All C order; only the first T (+1) steps of larger buffers are read.  Per sentence b
+ * the finished list holds (step_scores[t-1][k], t, k) for t = 1 .. T, k = 0 .. K-1 with tokens[t][k] == eos, in that
+ * order; while it holds fewer than n_best entries, (step_scores[T-1][0], T, 0) is appended (0.0 when T = 0), as the
+ * reference's minimum loop does.  The list is stable-sorted on -score (-0 equal to +0; NaN scores rank above every
+ * number, a rule of this kernel: the reference's sort has no defined order for them) and its n_best first entries
+ * are walked back through origins.  Hypothesis h = b*n_best + j: hyp_scores[h] its score, hyp_len[h] = t,
+ * hyp_tokens[h][p] = tokens[p+1][k_p] for p < t, and attn_argmax[h][p] the first index of the maximum of its
+ * attention row attn[p][k_p] (NaN above every number, as torch's max(0)); positions p >= t hold -1.  hyp_tokens,
+ * attn_argmax: int64 [B, n_best, T]; hyp_len int64, hyp_scores float32: [B, n_best].  One warp per sentence; no
+ * atomics, no synchronisation, no allocation: graph-capturable.  QD_ERR_INVALID_ARG: NULL or misaligned pointers
+ * (origins, step_scores, attn, hyp_tokens and attn_argmax may be NULL when steps = 0), beam outside [1, QD_BEAM_MAX], n_best outside
+ * [1, QD_BEAM_FINISH_MAX_NBEST], negative batch, steps or src_len, src_len 0 with steps > 0, (steps+1)*beam past
+ * 2^32, sizes past 64-bit indexing, outputs overlapping the inputs or each other.  batch 0 does nothing. */
+#define QD_BEAM_FINISH_MAX_NBEST 16
+int qd_beam_finish(const int64_t* tokens, const int64_t* origins, const float* step_scores, const float* attn,
+                   int64_t steps, int64_t batch, int beam, int64_t src_len, int64_t eos, int n_best,
+                   int64_t* hyp_tokens, int64_t* hyp_len, float* hyp_scores, int64_t* attn_argmax, qd_stream_t stream);
+
+/* ---- multi-bleu.perl's corpus statistics (perl_scripts/multi-bleu.perl) on int32 word ids -------------------------
+ * Hypothesis s is hyp_words[hyp_offsets[s] .. hyp_offsets[s+1]); reference r is ref_words[ref_offsets[r] ..
+ * ref_offsets[r+1]); sentence s has the references ref_first[s] .. ref_first[s] + ref_count[s] - 1 (0, 1 or several).
+ * Offsets need not start at 0.  Only word equality matters.  stats: int64 [n_sent, QD_BLEU_STATS], per sentence
+ * hyp_len, the closest reference length (smaller |diff| wins, a tie takes the shorter, starting from (diff, length) =
+ * (9999, 9999): so 9999 with no reference, and a reference more than 9999 words from the hypothesis is never taken), correct[1..4] and total[1..4]:
+ * total[n] = max(0, hyp_len - n + 1), correct[n] = the sum over the distinct n-grams g of the hypothesis of
+ * min(count_hyp(g), max_r count_ref_r(g)), comparing word tuples exactly (no hashing).  Device arrays, read by the
+ * kernel without a host synchronisation: an offset outside [0, n_words] is clamped into it, a span that ends before
+ * it starts is empty, and a reference range outside [0, n_refs) gives the sentence no reference.  Any length is
+ * exact; a sentence whose words fit in shared memory is staged there.  No atomics, no synchronisation, no allocation:
+ * graph-capturable.  QD_ERR_INVALID_ARG: negative counts, NULL pointers (word arrays may be NULL when their count is
+ * 0), misaligned pointers (words 4 bytes, the rest 8), stats overlapping an input.  n_sent 0 does nothing. */
+#define QD_BLEU_STATS 10
+int qd_bleu_stats(const int32_t* hyp_words, int64_t n_hyp_words, const int64_t* hyp_offsets, int64_t n_sent,
+                  const int32_t* ref_words, int64_t n_ref_words, const int64_t* ref_offsets, int64_t n_refs,
+                  const int64_t* ref_first, const int64_t* ref_count, int64_t* stats, qd_stream_t stream);
+/* totals[c] = sum over s of stats[s][c], c < QD_BLEU_STATS: the 10 corpus integers (exact, one CTA, fixed order).
+ * n_sent 0 writes zeros.  QD_ERR_INVALID_ARG: n_sent < 0, NULL or misaligned (8 bytes) pointers, totals overlapping
+ * stats. */
+int qd_bleu_fold(const int64_t* stats, int64_t n_sent, int64_t* totals, qd_stream_t stream);
+
 /* ---- next row f2: Huffman-coded storage (the model helpers/functions.py:226-262 only sizes) ----------
  * Canonical code over uint8 symbols, codes of 1..QD_HUFFMAN_MAX_LENGTH bits (built on the host: codec.py).
  * Stream: a tensor's symbols are cut into chunks of QD_HUFFMAN_CHUNK; each chunk's codes are written MSB-first

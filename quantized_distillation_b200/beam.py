@@ -8,10 +8,13 @@ one index_select per state tensor reorders the decoder, and done() is the loop's
 
     BatchBeam(batch, beam, n_best, bos, eos, pad, max_len, device)
     beam_search(model, src, src_lengths, beam_size=5, n_best=1, max_sent_length=100, *, bos, eos, pad, global_scorer=None)
+    beam_search_on_device(...)       the same search; the hypotheses stay on the device (BatchBeam.finish_on_device)
 
 There is no CPU implementation: without a CUDA device the calls raise RuntimeError.
 """
 from __future__ import annotations
+
+from typing import NamedTuple
 
 import torch
 import torch.nn as nn
@@ -128,6 +131,38 @@ class BatchBeam:
             attns.append(ats)
         return hyps, scores, attns
 
+    def finish_on_device(self) -> "DeviceHypotheses":
+        """finish() on the device, in one qd_beam_finish launch: the same hypotheses, lengths and scores (the n_best
+        first entries of sortFinished, the `minimum` quirk included), and for each hypothesis position the index that
+        `.max(0)` of finish()'s attention row returns, in place of the row.  No host synchronisation and no copy of the
+        histories.  n_best above QD_BEAM_FINISH_MAX_NBEST is refused (ValueError).  NaN scores rank first here;
+        Python's sort gives them no defined order."""
+        T, K, B, nb = self.steps, self.K, self.B, self.n_best
+        dev = self.device
+        hyp_tokens = torch.empty(B, nb, T, dtype=torch.int64, device=dev)
+        hyp_len = torch.empty(B, nb, dtype=torch.int64, device=dev)
+        hyp_scores = torch.empty(B, nb, dtype=torch.float32, device=dev)
+        attn_argmax = torch.empty(B, nb, T, dtype=torch.int64, device=dev)
+        attn = self.attn if T else None
+        if attn is not None and attn.dtype != torch.float32:
+            attn = attn.float()                  # exact: the same first maximum
+        with torch.cuda.device(dev):
+            N.check(N.lib().qd_beam_finish(
+                N.ptr(self.tokens), N.ptr(self.origins), N.ptr(self.step_scores), N.ptr(attn), T, B, K,
+                attn.shape[3] if attn is not None else 0, self.eos, nb, N.ptr(hyp_tokens), N.ptr(hyp_len),
+                N.ptr(hyp_scores), N.ptr(attn_argmax), N.stream_ptr(dev)))
+        return DeviceHypotheses(hyp_tokens, hyp_len, hyp_scores, attn_argmax)
+
+
+class DeviceHypotheses(NamedTuple):
+    """The n_best hypotheses of B sentences on the device (BatchBeam.finish_on_device), in sortFinished order.
+    tokens, attn_argmax: int64 [B, n_best, T]; lengths: int64 [B, n_best]; scores: float32 [B, n_best].  Positions at
+    and past a hypothesis's length hold -1."""
+    tokens: torch.Tensor
+    lengths: torch.Tensor
+    scores: torch.Tensor
+    attn_argmax: torch.Tensor
+
 
 def _generator_linear(gen):
     """The Linear of a Sequential(Linear or PackedLinear, LogSoftmax) generator."""
@@ -139,16 +174,8 @@ def _generator_linear(gen):
     return gen[0]
 
 
-@torch.no_grad()
-def beam_search(model, src, src_lengths, beam_size=5, n_best=1, max_sent_length=100, *, bos, eos, pad, global_scorer=None):
-    """Translator.translateBatch (onmt/Translator.py:90-193) without copy attention, global scorer or gold scores, for a
-    model that follows onmt's protocol: model.encoder(src, lengths) -> (enc_states, context [S, B, H]);
-    model.decoder.init_decoder_state(src, context, enc_states) -> a state with repeat_beam_size_times and `_all`
-    tensors [a, K*B, d]; model.decoder(inp [1, K*B, 1], context, state) -> (out [1, K*B, H], state, attn with
-    attn["std"] [1, K*B, S]); model.generator = Sequential(Linear or PackedLinear, LogSoftmax).  Each step runs the
-    decoder, the generator's Linear and one qd_beam_step on the logits, then reorders every state tensor with one
-    index_select.  Returns (hyps, scores, attn) per sentence, as BatchBeam.finish.  A global scorer (GNMT) is refused:
-    the reference ships it commented out (Translator.py:112)."""
+def _search(model, src, src_lengths, beam_size, n_best, max_sent_length, bos, eos, pad, global_scorer) -> BatchBeam:
+    """translateBatch's loop (onmt/Translator.py:90-193) up to the finished BatchBeam; see beam_search."""
     if global_scorer is not None:
         raise ValueError("a global scorer is not supported")
     if getattr(model.decoder, "_copy", False) or getattr(model.decoder, "copy_attn", False):
@@ -170,4 +197,26 @@ def beam_search(model, src, src_lengths, beam_size=5, n_best=1, max_sent_length=
         flat_origin = beam.advance(logits, attn["std"].squeeze(0), normalized=False)
         for e in state._all:
             e.copy_(e.index_select(1, flat_origin))
-    return beam.finish()
+    return beam
+
+
+@torch.no_grad()
+def beam_search(model, src, src_lengths, beam_size=5, n_best=1, max_sent_length=100, *, bos, eos, pad, global_scorer=None):
+    """Translator.translateBatch (onmt/Translator.py:90-193) without copy attention, global scorer or gold scores, for a
+    model that follows onmt's protocol: model.encoder(src, lengths) -> (enc_states, context [S, B, H]);
+    model.decoder.init_decoder_state(src, context, enc_states) -> a state with repeat_beam_size_times and `_all`
+    tensors [a, K*B, d]; model.decoder(inp [1, K*B, 1], context, state) -> (out [1, K*B, H], state, attn with
+    attn["std"] [1, K*B, S]); model.generator = Sequential(Linear or PackedLinear, LogSoftmax).  Each step runs the
+    decoder, the generator's Linear and one qd_beam_step on the logits, then reorders every state tensor with one
+    index_select.  Returns (hyps, scores, attn) per sentence, as BatchBeam.finish.  A global scorer (GNMT) is refused:
+    the reference ships it commented out (Translator.py:112)."""
+    return _search(model, src, src_lengths, beam_size, n_best, max_sent_length, bos, eos, pad, global_scorer).finish()
+
+
+@torch.no_grad()
+def beam_search_on_device(model, src, src_lengths, beam_size=5, n_best=1, max_sent_length=100, *, bos, eos, pad,
+                          global_scorer=None) -> DeviceHypotheses:
+    """beam_search with BatchBeam.finish_on_device in place of finish: the same search, and the n_best hypotheses of
+    every sentence as device tensors, with no host loop and no copy of the histories."""
+    return _search(model, src, src_lengths, beam_size, n_best, max_sent_length, bos, eos, pad,
+                   global_scorer).finish_on_device()

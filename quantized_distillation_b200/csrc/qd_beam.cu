@@ -218,6 +218,94 @@ __global__ void __launch_bounds__(kMergeWarps * 32) beam_merge_kernel(MergeArgs 
     }
 }
 
+struct FinishArgs {
+    const int64_t* tokens;                   // [T+1, K, B]
+    const int64_t* origins;                  // [T, K, B]
+    const float* step_scores;                // [T, K, B]
+    const float* attn;                       // [T, K, B, S]
+    int64_t* hyp_tokens;                     // [B, n_best, T]
+    int64_t* hyp_len;                        // [B, n_best]
+    float* hyp_scores;                       // [B, n_best]
+    int64_t* attn_argmax;                    // [B, n_best, T]
+    int64_t T, B, S, eos;
+    int K, n_best;
+};
+
+// (value, index) of the first maximum: a larger value wins, an equal one the lower index; NaN is above every number
+// (the first NaN wins, as torch.max); index -1 is no candidate
+__device__ __forceinline__ bool first_max_beats(float v, int64_t i, float bv, int64_t bi) {
+    if (i < 0) return false;
+    if (bi < 0) return true;
+    if (v != v) return bv == bv || i < bi;
+    if (bv != bv) return false;
+    return v > bv || (v == bv && i < bi);
+}
+
+// one warp per sentence: the finished list of sortFinished(minimum=n_best) (Beam.py:108-121) is virtual, entry
+// i < T*K being (t, k) = (i / K + 1, i % K) when tokens[t][k] is eos, entry T*K + p (p < pads) the top beam of the last
+// step.  Round j selects the largest (key_order(score), -i) below round j-1's: the stable sort on -score, ties in
+// list order.  Then the hypothesis is walked back through origins (Beam.getHyp), the warp taking each row's argmax.
+__global__ void __launch_bounds__(kMergeWarps * 32) beam_finish_kernel(FinishArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int K = a.K;
+    const int64_t B = a.B, T = a.T, TK = T * K;
+    for (int64_t b = (int64_t)blockIdx.x * kMergeWarps + (threadIdx.x >> 5); b < B; b += (int64_t)gridDim.x * kMergeWarps) {
+        unsigned nf = 0;
+        for (int64_t i = lane; i < TK; i += 32) nf += __ldg(a.tokens + (i + K) * B + b) == a.eos;
+        nf = __reduce_add_sync(0xFFFFFFFFu, nf);
+        const int64_t pads = nf < (unsigned)a.n_best ? a.n_best - nf : 0;
+        const float last0 = T ? __ldg(a.step_scores + (T - 1) * K * B + b) : 0.f;
+        unsigned long long prev = ~0ull;
+        for (int j = 0; j < a.n_best; ++j) {
+            unsigned long long best = 0;
+            for (int64_t i = lane; i < TK + pads; i += 32) {
+                float sc;
+                if (i < TK) {
+                    if (__ldg(a.tokens + (i + K) * B + b) != a.eos) continue;
+                    sc = __ldg(a.step_scores + i * B + b);
+                } else {
+                    sc = last0;
+                }
+                const unsigned long long key = ((unsigned long long)key_order(sc) << 32) | (0xFFFFFFFFu - (uint32_t)i);
+                if (key < prev && key > best) best = key;
+            }
+            prev = warp_max(best);
+            const int64_t i = 0xFFFFFFFFu - (uint32_t)prev;
+            const int64_t t = i < TK ? i / K + 1 : T;
+            int64_t k = i < TK ? i % K : 0;
+            const int64_t h = b * a.n_best + j;
+            if (lane == 0) {
+                a.hyp_scores[h] = i < TK ? __ldg(a.step_scores + i * B + b) : last0;
+                a.hyp_len[h] = t;
+            }
+            int64_t* out_tok = a.hyp_tokens + h * T;
+            int64_t* out_arg = a.attn_argmax + h * T;
+            for (int64_t p = t + lane; p < T; p += 32) out_tok[p] = -1, out_arg[p] = -1;
+            for (int64_t p = t - 1; p >= 0; --p) {
+                const int64_t row = (p * K + k) * B + b;
+                const float* at = a.attn + row * a.S;
+                float bv = 0.f;
+                int64_t bi = -1;
+                for (int64_t c = lane; c < a.S; c += 32) {
+                    const float v = __ldg(at + c);
+                    if (first_max_beats(v, c, bv, bi)) bv = v, bi = c;
+                }
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) {
+                    const float ov = __shfl_xor_sync(0xFFFFFFFFu, bv, o);
+                    const int64_t oi = __shfl_xor_sync(0xFFFFFFFFu, bi, o);
+                    if (first_max_beats(ov, oi, bv, bi)) bv = ov, bi = oi;
+                }
+                if (lane == 0) {
+                    out_tok[p] = __ldg(a.tokens + row + K * B);      // tokens[p + 1][k][b]
+                    out_arg[p] = bi;
+                }
+                k = __ldg(a.origins + row);
+            }
+        }
+    }
+}
+
 bool overlap(const void* a, size_t na, const void* b, size_t nb) {
     const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
     return a != nullptr && b != nullptr && na > 0 && nb > 0 && pa < pb + nb && pb < pa + na;
@@ -288,6 +376,50 @@ extern "C" int qd_beam_step(const float* out, int normalize, int64_t batch, int 
     ma.n_finished = n_finished, ma.eos_top = eos_top, ma.B = batch, ma.eos = eos, ma.K = beam, ma.first = ra.first;
     const int64_t merge_blocks = (batch + kMergeWarps - 1) / kMergeWarps;
     beam_merge_kernel<<<(unsigned)(merge_blocks < kBeamMaxGrid ? merge_blocks : kBeamMaxGrid), kMergeWarps * 32, 0, st>>>(ma);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+extern "C" int qd_beam_finish(const int64_t* tokens, const int64_t* origins, const float* step_scores, const float* attn,
+                              int64_t steps, int64_t batch, int beam, int64_t src_len, int64_t eos, int n_best,
+                              int64_t* hyp_tokens, int64_t* hyp_len, float* hyp_scores, int64_t* attn_argmax,
+                              qd_stream_t stream) {
+    if (beam < 1 || beam > QD_BEAM_MAX) return fail(QD_ERR_INVALID_ARG, "beam must be in [1, %d] (beam=%d)", QD_BEAM_MAX, beam);
+    if (n_best < 1 || n_best > QD_BEAM_FINISH_MAX_NBEST)
+        return fail(QD_ERR_INVALID_ARG, "n_best must be in [1, %d] (n_best=%d)", QD_BEAM_FINISH_MAX_NBEST, n_best);
+    if (batch < 0 || steps < 0 || src_len < 0)
+        return fail(QD_ERR_INVALID_ARG, "batch, steps and src_len must be >= 0 (batch=%lld steps=%lld src_len=%lld)",
+                    (long long)batch, (long long)steps, (long long)src_len);
+    if (steps > 0 && src_len < 1) return fail(QD_ERR_INVALID_ARG, "src_len must be >= 1 when steps > 0");
+    if ((steps + 1) * beam + n_best >= (int64_t)UINT32_MAX) return fail(QD_ERR_INVALID_ARG, "steps * beam must be below 2^32");
+    if (batch > 0 && (steps + 1) * beam > INT64_MAX / 8 / batch / (src_len > 0 ? src_len : 1))
+        return fail(QD_ERR_INVALID_ARG, "steps * beam * batch * src_len overflows 64-bit indexing");
+    if (batch == 0) return QD_OK;
+    if (tokens == nullptr || hyp_len == nullptr || hyp_scores == nullptr ||
+        (steps > 0 && (origins == nullptr || step_scores == nullptr || attn == nullptr || hyp_tokens == nullptr ||
+                       attn_argmax == nullptr)))
+        return fail(QD_ERR_INVALID_ARG, "NULL argument");
+    if (misaligned(tokens, 8) || misaligned(origins, 8) || misaligned(step_scores, 4) || misaligned(attn, 4) ||
+        misaligned(hyp_tokens, 8) || misaligned(hyp_len, 8) || misaligned(hyp_scores, 4) || misaligned(attn_argmax, 8))
+        return fail(QD_ERR_INVALID_ARG, "misaligned argument (int64 arrays 8 bytes, float arrays 4 bytes)");
+    const int64_t R = batch * beam, H = batch * n_best;
+    const void* ins[4] = {tokens, origins, step_scores, attn};
+    const size_t in_bytes[4] = {(size_t)((steps + 1) * R) * 8, (size_t)(steps * R) * 8, (size_t)(steps * R) * 4,
+                                (size_t)(steps * R * src_len) * 4};
+    const void* outs[4] = {hyp_tokens, hyp_len, hyp_scores, attn_argmax};
+    const size_t out_bytes[4] = {(size_t)(H * steps) * 8, (size_t)H * 8, (size_t)H * 4, (size_t)(H * steps) * 8};
+    for (int i = 0; i < 4; ++i) {
+        for (int j = 0; j < 4; ++j)
+            if (overlap(outs[i], out_bytes[i], ins[j], in_bytes[j])) return fail(QD_ERR_INVALID_ARG, "outputs must not overlap the inputs");
+        for (int j = 0; j < i; ++j)
+            if (overlap(outs[i], out_bytes[i], outs[j], out_bytes[j])) return fail(QD_ERR_INVALID_ARG, "outputs must not overlap each other");
+    }
+    FinishArgs fa{};
+    fa.tokens = tokens, fa.origins = origins, fa.step_scores = step_scores, fa.attn = attn;
+    fa.hyp_tokens = hyp_tokens, fa.hyp_len = hyp_len, fa.hyp_scores = hyp_scores, fa.attn_argmax = attn_argmax;
+    fa.T = steps, fa.B = batch, fa.S = src_len, fa.eos = eos, fa.K = beam, fa.n_best = n_best;
+    const int64_t blocks = (batch + kMergeWarps - 1) / kMergeWarps;
+    beam_finish_kernel<<<(unsigned)(blocks < kBeamMaxGrid ? blocks : kBeamMaxGrid), kMergeWarps * 32, 0, as_stream(stream)>>>(fa);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }
