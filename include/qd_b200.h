@@ -345,6 +345,44 @@ int qd_nmt_loss_bwd(const float* logits, const float* teacher_logits, const int6
                     const float* grad_loss, int64_t rows, int64_t V, int64_t padding_idx, float w, float* grad_logits,
                     qd_stream_t stream);
 
+/* ---- the core of onmt's GlobalAttention, "dot" and "general" (onmt/modules/GlobalAttention.py:108-188) ------------
+ * Between linear_in and linear_out: align = softmax_s(q . h_s) over all S source positions (no mask), c = sum_s
+ * align_s h_s, concat = [c | input].  Batch entry n has T query rows; row (n, t) attends to n.  q, input, grad_q:
+ * float32 [N, T, H] (row n*T + t), C order.  align, grad_align, concat, grad_concat: float32 [T, N, S] / [T, N, 2H]
+ * (row t*N + n), C order: the reference's output order.  The context is read at context[n*sN + s*sS + h] (unit stride
+ * along H): sN = S*H, sS = H for a contiguous [N, S, H]; sN = H, sS = N*H for the transpose of a contiguous [S, N, H],
+ * as onmt's decoders pass it; grad_context is written in the same layout.  Any 4-byte alignment: every load is scalar.
+ * Arithmetic: float32, one IEEE rounding per operation (no FMA).  A score is a sum over h = l + 32j per lane l, in j
+ * order, then a butterfly over the 32 lanes; the softmax takes the row maximum m, l = sum_s expf(x_s - m) (per lane in
+ * s order, then a butterfly) and align = expf(x - m) / l; c[h] and grad_q[h] are sums over s in order; grad_context
+ * sums over n's rows in t order.  All of it depends on (S, H) alone: a row's forward gives the same bits alone or in
+ * any batch, and both calls give the same bits on every run.  Error: a float32 sum of k terms in these orders is within
+ * (ceil(k/32) + 6) * 2^-24 * sum|terms| of the exact one (the sum of a weighted context: (k + 2) * 2^-24 * sum|terms|);
+ * align_s carries in addition a relative 2^-24 |x_s - m| from the rounding of x_s - m before the exponential, and any
+ * operation with a subnormal result up to 2^-149 more.  The tests allow twice these bounds, propagated through the
+ * chain to first order (oracle/attention_oracle.py, core_bounds).
+ * Neither call allocates or synchronises: graph-capturable.  Rows 0 (N = 0 or T = 0) do nothing.
+ * QD_ERR_INVALID_ARG: kind not QD_ATTN_DOT / QD_ATTN_GENERAL (dot reads the query from input: q must be NULL or input),
+ * negative sizes, S or H 0 with rows, negative strides, strides that make two (n, s) rows overlap, sizes or the
+ * context's extent past 64-bit indexing, NULL or misaligned pointers, outputs overlapping the inputs or each other. */
+#define QD_ATTN_DOT 0
+#define QD_ATTN_GENERAL 1
+int qd_attn_fwd(int kind, const float* q, const float* input, const float* context, int64_t ctx_batch_stride,
+                int64_t ctx_src_stride, int64_t N, int64_t T, int64_t S, int64_t H, float* align, float* concat,
+                qd_stream_t stream);
+/* The backward's workspace: R*S floats (R = N*T), 0 without rows. */
+size_t qd_attn_workspace_bytes(int64_t rows, int64_t S);
+/* gc = grad_concat[:, :H]; ga_s = gc . h_s + grad_align_s (grad_align may be NULL: zero); gs = align (ga - sum_s
+ * align ga); grad_q = sum_s gs_s h_s; grad_context[n, s] = sum over the rows r of n of (align_{r,s} gc_r +
+ * gs_{r,s} q_r), no atomics.  The gradient of input is grad_concat[:, H:] itself: no work here.  align and q as given
+ * to or read by qd_attn_fwd (for dot, q is the input).  Two launches.  workspace: >= qd_attn_workspace_bytes(N*T, S)
+ * bytes, 4-byte aligned, else QD_ERR_WORKSPACE.  Checks as the forward's; grad_q, grad_context and the workspace must
+ * not overlap the inputs or each other. */
+int qd_attn_bwd(const float* grad_concat, const float* grad_align, const float* align, const float* q,
+                const float* context, int64_t ctx_batch_stride, int64_t ctx_src_stride, int64_t N, int64_t T, int64_t S,
+                int64_t H, float* grad_q, float* grad_context, void* workspace, size_t workspace_bytes,
+                qd_stream_t stream);
+
 /* ---- one beam search step of B sentences (onmt/Beam.py:55-106, Beam.advance; Translator.translateBatch) ----------
  * Rows follow onmt's beam-major decoder batch: row r = k*B + b is beam k of sentence b (K = beam).  out: float32
  * [K*B, V], C order, any 4-byte alignment.  With normalize = 0 it holds log-probabilities lp; with normalize = 1 the

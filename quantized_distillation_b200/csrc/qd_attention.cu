@@ -1,0 +1,321 @@
+// qd_attention.cu -- the core of onmt's GlobalAttention for the "dot" and "general" scores
+// (onmt/modules/GlobalAttention.py:108-188): score -> softmax over the source -> weighted context -> [c | input].  The
+// query projection linear_in and the output linear_out + tanh stay GEMMs outside.
+//
+// Rows: batch entry n has T query rows; q and input are n-major ([N, T, H], row n*T + t), align and concat are t-major
+// ([T, N, .], row t*N + n), the order the reference returns them.  Row (n, t) attends to the context slab of n, read at
+// context + n*sN + s*sS + h: the contiguous [N, S, H] and the transposed view of a contiguous [S, N, H] alike.
+//
+// Forward (qd_attn_fwd): one 256-thread CTA per tile of up to kAtTile rows of one n, three phases:
+//   1. scores: warp w owns the source positions s = w + 8k, lane l the elements h = l + 32j; per row a lane-strided
+//      float32 sum and a butterfly over the warp.  The raw scores go to align.
+//   2. softmax: warp t owns row t of the tile; max, then sum of expf(x - max) (lane-strided, butterfly), then
+//      align = expf(x - max) / sum in place.
+//   3. context: thread j owns h = j + 256k and sums align_s * h_s over s in order; it writes c and copies input beside.
+// The slab is read from HBM once per tile in phase 1; phase 3 reads it again from L2 (at most S*H*4 bytes per tile).
+//
+// Backward: qd_attn_bwd_rows runs the same three phases on grad_concat (ga = gc . h_s + grad_align, then
+// gs = align (ga - sum_s align ga) into the workspace, then grad_q = sum_s gs h_s); qd_attn_bwd_context gives each CTA
+// kAtSChunk source positions of one n and sums a_{r,s} gc_r + gs_{r,s} q_r over that n's rows in the order t = 0..T-1.
+//
+// Which thread owns which element, and every summation order, depend only on (S, H): a row's forward bits are the
+// same alone or in any batch; all loads are scalar, so the alignment of a view changes nothing either.
+#include <cmath>
+
+#include "qd_launch.h"
+
+using namespace qd;
+
+namespace {
+
+constexpr int kAtThreads = 256;
+constexpr int kAtWarps = kAtThreads / 32;
+constexpr int kAtTile = 8;          // query rows of one batch entry per CTA (phase 2 gives each a warp)
+constexpr int kAtSChunk = 8;        // source positions per CTA of the context gradient
+constexpr int64_t kAtMaxGrid = 1 << 20, kAtMaxGridY = 65535;
+static_assert(kAtTile <= kAtWarps, "phase 2 gives each row of a tile its own warp");
+
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+
+// out[t*os + s] = v_t . h_s (+ add[t*os + s]) for the nt rows v_t = v + t*vs of a tile and every s < S
+__device__ __forceinline__ void tile_dots(const float* __restrict__ ctx, int64_t sS, int64_t S, int64_t H,
+                                          const float* __restrict__ v, int64_t vs, int nt, const float* __restrict__ add,
+                                          float* out, int64_t os) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int64_t s = warp; s < S; s += kAtWarps) {
+        const float* hs = ctx + s * sS;
+        float acc[kAtTile];
+#pragma unroll
+        for (int t = 0; t < kAtTile; ++t) acc[t] = 0.f;
+#pragma unroll 4
+        for (int64_t j = lane; j < H; j += 32) {
+            const float x = __ldg(hs + j);
+#pragma unroll
+            for (int t = 0; t < kAtTile; ++t)
+                if (t < nt) acc[t] = __fadd_rn(acc[t], __fmul_rn(__ldg(v + t * vs + j), x));
+        }
+#pragma unroll
+        for (int t = 0; t < kAtTile; ++t) {
+            if (t < nt) {
+                float d = warp_sum(acc[t]);
+                if (lane == 0) {
+                    if (add != nullptr) d = __fadd_rn(d, __ldg(add + t * os + s));
+                    out[t * os + s] = d;
+                }
+            }
+        }
+    }
+}
+
+// out[t*os + h] = sum_s p[t*ps + s] h_s[h] for the nt rows of a tile, s in order
+__device__ __forceinline__ void tile_weighted_sum(const float* __restrict__ ctx, int64_t sS, int64_t S, int64_t H,
+                                                  const float* p, int64_t ps, int nt, float* __restrict__ out, int64_t os) {
+    for (int64_t h = threadIdx.x; h < H; h += kAtThreads) {
+        float acc[kAtTile];
+#pragma unroll
+        for (int t = 0; t < kAtTile; ++t) acc[t] = 0.f;
+#pragma unroll 4
+        for (int64_t s = 0; s < S; ++s) {
+            const float x = __ldg(ctx + s * sS + h);
+#pragma unroll
+            for (int t = 0; t < kAtTile; ++t)
+                if (t < nt) acc[t] = __fadd_rn(acc[t], __fmul_rn(p[t * ps + s], x));
+        }
+#pragma unroll
+        for (int t = 0; t < kAtTile; ++t)
+            if (t < nt) out[t * os + h] = acc[t];
+    }
+}
+
+struct AtShape {
+    const float* ctx;
+    int64_t sN, sS, N, T, S, H;
+};
+
+struct AtFwdArgs {
+    AtShape g;
+    const float* q;       // [N, T, H]
+    const float* input;   // [N, T, H]
+    float* align;         // [T, N, S]
+    float* concat;        // [T, N, 2H]
+};
+
+__global__ void __launch_bounds__(kAtThreads) attn_fwd_kernel(AtFwdArgs a) {
+    const AtShape g = a.g;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int64_t n = blockIdx.x; n < g.N; n += gridDim.x)
+    for (int64_t t0 = (int64_t)blockIdx.y * kAtTile; t0 < g.T; t0 += (int64_t)gridDim.y * kAtTile) {
+        const int nt = (int)min((int64_t)kAtTile, g.T - t0);
+        const float* ctx = g.ctx + n * g.sN;
+        const int64_t in_row = (n * g.T + t0) * g.H, out_row = t0 * g.N + n;
+        float* al = a.align + out_row * g.S;
+        const int64_t as = g.N * g.S;
+        tile_dots(ctx, g.sS, g.S, g.H, a.q + in_row, g.H, nt, nullptr, al, as);
+        __syncthreads();
+        if (warp < nt) {
+            float* row = al + warp * as;
+            float m = -INFINITY;
+            for (int64_t s = lane; s < g.S; s += 32) m = fmaxf(m, row[s]);
+            m = warp_max(m);
+            float l = 0.f;
+            for (int64_t s = lane; s < g.S; s += 32) l = __fadd_rn(l, expf(__fsub_rn(row[s], m)));
+            l = warp_sum(l);
+            for (int64_t s = lane; s < g.S; s += 32) row[s] = __fdiv_rn(expf(__fsub_rn(row[s], m)), l);
+        }
+        __syncthreads();
+        float* cc = a.concat + out_row * 2 * g.H;
+        const int64_t cs = g.N * 2 * g.H;
+        tile_weighted_sum(ctx, g.sS, g.S, g.H, al, as, nt, cc, cs);
+        for (int64_t h = threadIdx.x; h < g.H; h += kAtThreads)
+            for (int t = 0; t < nt; ++t) cc[t * cs + g.H + h] = __ldg(a.input + in_row + t * g.H + h);
+    }
+}
+
+struct AtBwdArgs {
+    AtShape g;
+    const float* grad_concat;   // [T, N, 2H]
+    const float* grad_align;    // [T, N, S] or NULL
+    const float* align;         // [T, N, S]
+    const float* q;             // [N, T, H]
+    float* gs;                  // workspace [T, N, S]
+    float* grad_q;              // [N, T, H]
+    float* grad_ctx;            // the context's layout
+};
+
+__global__ void __launch_bounds__(kAtThreads) attn_bwd_rows_kernel(AtBwdArgs a) {
+    const AtShape g = a.g;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int64_t n = blockIdx.x; n < g.N; n += gridDim.x)
+    for (int64_t t0 = (int64_t)blockIdx.y * kAtTile; t0 < g.T; t0 += (int64_t)gridDim.y * kAtTile) {
+        const int nt = (int)min((int64_t)kAtTile, g.T - t0);
+        const float* ctx = g.ctx + n * g.sN;
+        const int64_t in_row = (n * g.T + t0) * g.H, out_row = t0 * g.N + n;
+        const int64_t as = g.N * g.S;
+        float* gs = a.gs + out_row * g.S;
+        tile_dots(ctx, g.sS, g.S, g.H, a.grad_concat + out_row * 2 * g.H, g.N * 2 * g.H, nt,
+                  a.grad_align != nullptr ? a.grad_align + out_row * g.S : nullptr, gs, as);
+        __syncthreads();
+        if (warp < nt) {
+            const float* al = a.align + out_row * g.S + warp * as;
+            float* row = gs + warp * as;
+            float d = 0.f;
+            for (int64_t s = lane; s < g.S; s += 32) d = __fadd_rn(d, __fmul_rn(__ldg(al + s), row[s]));
+            d = warp_sum(d);
+            for (int64_t s = lane; s < g.S; s += 32) row[s] = __fmul_rn(__ldg(al + s), __fsub_rn(row[s], d));
+        }
+        __syncthreads();
+        tile_weighted_sum(ctx, g.sS, g.S, g.H, gs, as, nt, a.grad_q + in_row, g.H);
+    }
+}
+
+__global__ void __launch_bounds__(kAtThreads) attn_bwd_context_kernel(AtBwdArgs a) {
+    const AtShape g = a.g;
+    for (int64_t n = blockIdx.x; n < g.N; n += gridDim.x)
+    for (int64_t s0 = (int64_t)blockIdx.y * kAtSChunk; s0 < g.S; s0 += (int64_t)gridDim.y * kAtSChunk) {
+        const int ns = (int)min((int64_t)kAtSChunk, g.S - s0);
+        for (int64_t h = threadIdx.x; h < g.H; h += kAtThreads) {
+            float acc[kAtSChunk];
+#pragma unroll
+            for (int j = 0; j < kAtSChunk; ++j) acc[j] = 0.f;
+            for (int64_t t = 0; t < g.T; ++t) {
+                const int64_t r = t * g.N + n;
+                const float gc = __ldg(a.grad_concat + r * 2 * g.H + h), qv = __ldg(a.q + (n * g.T + t) * g.H + h);
+                const float* al = a.align + r * g.S + s0;
+                const float* gs = a.gs + r * g.S + s0;
+#pragma unroll
+                for (int j = 0; j < kAtSChunk; ++j)
+                    if (j < ns) acc[j] = __fadd_rn(acc[j], __fadd_rn(__fmul_rn(__ldg(al + j), gc), __fmul_rn(__ldg(gs + j), qv)));
+            }
+#pragma unroll
+            for (int j = 0; j < kAtSChunk; ++j)
+                if (j < ns) a.grad_ctx[n * g.sN + (s0 + j) * g.sS + h] = acc[j];
+        }
+    }
+}
+
+bool overlap(const void* a, size_t na, const void* b, size_t nb) {
+    const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
+    return a != nullptr && b != nullptr && na > 0 && nb > 0 && pa < pb + nb && pb < pa + na;
+}
+
+bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) != 0; }
+
+// checks of the sizes and the context layout both calls share; R = N*T.  span: bytes from context to its last element
+int check_shape(const float* ctx, int64_t sN, int64_t sS, int64_t N, int64_t T, int64_t S, int64_t H, int64_t* R,
+                size_t* span) {
+    if (N < 0 || T < 0 || S < 0 || H < 0) return fail(QD_ERR_INVALID_ARG, "sizes must be >= 0 (N=%lld T=%lld S=%lld H=%lld)",
+                                                      (long long)N, (long long)T, (long long)S, (long long)H);
+    if (T > 0 && N > INT64_MAX / T) return fail(QD_ERR_INVALID_ARG, "N * T overflows 64-bit indexing");
+    *R = N * T;
+    *span = 0;
+    if (*R == 0) return QD_OK;
+    if (S == 0 || H == 0) return fail(QD_ERR_INVALID_ARG, "S and H must be >= 1 when there are rows (S=%lld H=%lld)",
+                                      (long long)S, (long long)H);
+    if (sN < 0 || sS < 0) return fail(QD_ERR_INVALID_ARG, "context strides must be >= 0");
+    const int64_t lim = INT64_MAX / 8;
+    if (*R > lim / S || *R > lim / (2 * H)) return fail(QD_ERR_INVALID_ARG, "rows * S or rows * 2H overflows 64-bit indexing");
+    if ((N > 1 && sN > (lim - H) / (N - 1)) || (S > 1 && sS > (lim - H) / (S - 1)) ||
+        (N - 1) * sN > lim - H - (S - 1) * sS)
+        return fail(QD_ERR_INVALID_ARG, "the context's extent overflows 64-bit indexing");
+    // the (batch, source) rows of H elements must not overlap: the smaller stride covers a row, the larger its run
+    int64_t lo = sS, clo = S, hi = sN, chi = N;
+    if (sN < sS || (sN == sS && N < S)) lo = sN, clo = N, hi = sS, chi = S;
+    if ((clo > 1 && lo < H) || (chi > 1 && hi < (clo - 1) * lo + H))
+        return fail(QD_ERR_INVALID_ARG, "context strides (batch %lld, source %lld) make rows of %lld elements overlap",
+                    (long long)sN, (long long)sS, (long long)H);
+    if (ctx == nullptr) return fail(QD_ERR_INVALID_ARG, "NULL context");
+    *span = (size_t)((N - 1) * sN + (S - 1) * sS + H) * sizeof(float);
+    return QD_OK;
+}
+
+// blockIdx.x walks the batch entries, blockIdx.y the tiles (or source chunks) of one; both loop past the grid
+dim3 grid_of(int64_t N, int64_t tiles) {
+    return dim3((unsigned)(N < kAtMaxGrid ? N : kAtMaxGrid), (unsigned)(tiles < kAtMaxGridY ? tiles : kAtMaxGridY));
+}
+
+}  // namespace
+
+extern "C" size_t qd_attn_workspace_bytes(int64_t rows, int64_t S) {
+    return rows > 0 && S > 0 ? (size_t)rows * (size_t)S * sizeof(float) : 0;
+}
+
+extern "C" int qd_attn_fwd(int kind, const float* q, const float* input, const float* context, int64_t ctx_batch_stride,
+                           int64_t ctx_src_stride, int64_t N, int64_t T, int64_t S, int64_t H, float* align, float* concat,
+                           qd_stream_t stream) {
+    if (kind != QD_ATTN_DOT && kind != QD_ATTN_GENERAL) return fail(QD_ERR_INVALID_ARG, "kind must be QD_ATTN_DOT or QD_ATTN_GENERAL");
+    if (kind == QD_ATTN_DOT && q != nullptr && q != input) return fail(QD_ERR_INVALID_ARG, "dot attention reads its query from input: q must be NULL");
+    int64_t R;
+    size_t span;
+    int rc = check_shape(context, ctx_batch_stride, ctx_src_stride, N, T, S, H, &R, &span);
+    if (rc) return rc;
+    if (R == 0) return QD_OK;
+    if (kind == QD_ATTN_DOT) q = input;
+    if (q == nullptr || input == nullptr || align == nullptr || concat == nullptr) return fail(QD_ERR_INVALID_ARG, "NULL argument");
+    if (misaligned(q) || misaligned(input) || misaligned(context) || misaligned(align) || misaligned(concat))
+        return fail(QD_ERR_INVALID_ARG, "float arrays must be 4-byte aligned");
+    const size_t row_bytes = (size_t)(R * H) * sizeof(float), al_bytes = (size_t)(R * S) * sizeof(float);
+    if (overlap(align, al_bytes, concat, 2 * row_bytes)) return fail(QD_ERR_INVALID_ARG, "align and concat must not overlap");
+    const float* outs[2] = {align, concat};
+    const size_t out_bytes[2] = {al_bytes, 2 * row_bytes};
+    for (int i = 0; i < 2; ++i)
+        if (overlap(outs[i], out_bytes[i], q, row_bytes) || overlap(outs[i], out_bytes[i], input, row_bytes) ||
+            overlap(outs[i], out_bytes[i], context, span))
+            return fail(QD_ERR_INVALID_ARG, "outputs must not overlap the inputs");
+    AtFwdArgs a{};
+    a.g = AtShape{context, ctx_batch_stride, ctx_src_stride, N, T, S, H};
+    a.q = q, a.input = input, a.align = align, a.concat = concat;
+    attn_fwd_kernel<<<grid_of(N, (T + kAtTile - 1) / kAtTile), kAtThreads, 0, as_stream(stream)>>>(a);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
+
+extern "C" int qd_attn_bwd(const float* grad_concat, const float* grad_align, const float* align, const float* q,
+                           const float* context, int64_t ctx_batch_stride, int64_t ctx_src_stride, int64_t N, int64_t T,
+                           int64_t S, int64_t H, float* grad_q, float* grad_context, void* workspace, size_t workspace_bytes,
+                           qd_stream_t stream) {
+    int64_t R;
+    size_t span;
+    int rc = check_shape(context, ctx_batch_stride, ctx_src_stride, N, T, S, H, &R, &span);
+    if (rc) return rc;
+    if (R == 0) return QD_OK;
+    if (grad_concat == nullptr || align == nullptr || q == nullptr || grad_q == nullptr || grad_context == nullptr)
+        return fail(QD_ERR_INVALID_ARG, "NULL argument");
+    if (misaligned(grad_concat) || misaligned(grad_align) || misaligned(align) || misaligned(q) || misaligned(context) ||
+        misaligned(grad_q) || misaligned(grad_context))
+        return fail(QD_ERR_INVALID_ARG, "float arrays must be 4-byte aligned");
+    const size_t need = qd_attn_workspace_bytes(R, S);
+    if (workspace == nullptr || workspace_bytes < need || misaligned(workspace))
+        return fail(QD_ERR_WORKSPACE, "workspace must be 4-byte aligned and hold qd_attn_workspace_bytes(%lld, %lld) = %zu bytes",
+                    (long long)R, (long long)S, need);
+    const size_t row_bytes = (size_t)(R * H) * sizeof(float), al_bytes = (size_t)(R * S) * sizeof(float);
+    const void* outs[3] = {grad_q, grad_context, workspace};
+    const size_t out_bytes[3] = {row_bytes, span, need};
+    for (int i = 0; i < 3; ++i) {
+        if (overlap(outs[i], out_bytes[i], grad_concat, 2 * row_bytes) || overlap(outs[i], out_bytes[i], grad_align, al_bytes) ||
+            overlap(outs[i], out_bytes[i], align, al_bytes) || overlap(outs[i], out_bytes[i], q, row_bytes) ||
+            overlap(outs[i], out_bytes[i], context, span))
+            return fail(QD_ERR_INVALID_ARG, "outputs and workspace must not overlap the inputs");
+        for (int j = 0; j < i; ++j)
+            if (overlap(outs[i], out_bytes[i], outs[j], out_bytes[j]))
+                return fail(QD_ERR_INVALID_ARG, "outputs and workspace must not overlap each other");
+    }
+    AtBwdArgs a{};
+    a.g = AtShape{context, ctx_batch_stride, ctx_src_stride, N, T, S, H};
+    a.grad_concat = grad_concat, a.grad_align = grad_align, a.align = align, a.q = q;
+    a.gs = static_cast<float*>(workspace), a.grad_q = grad_q, a.grad_ctx = grad_context;
+    cudaStream_t st = as_stream(stream);
+    attn_bwd_rows_kernel<<<grid_of(N, (T + kAtTile - 1) / kAtTile), kAtThreads, 0, st>>>(a);
+    attn_bwd_context_kernel<<<grid_of(N, (S + kAtSChunk - 1) / kAtSChunk), kAtThreads, 0, st>>>(a);
+    QD_CUDA(cudaGetLastError());
+    return QD_OK;
+}
