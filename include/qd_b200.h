@@ -383,6 +383,39 @@ int qd_attn_bwd(const float* grad_concat, const float* grad_align, const float* 
                 int64_t H, float* grad_q, float* grad_context, void* workspace, size_t workspace_bytes,
                 qd_stream_t stream);
 
+/* ---- the SRU recurrence of onmt's SRU layers (onmt/modules/SRU.py:71-347, sru_fwd / sru_bwd / sru_bi_fwd /
+ * sru_bi_bwd) ----------------------------------------------------------------------------------------------------
+ * Columns col = b*(dir*d) + j, dir = 2 when bidirectional, else 1; ncols = batch*dir*d.  u: float32 [len, batch,
+ * dir*d, k], u = x_2d.mm(weight), the k values of a column adjacent; x (k = 3 only: the layer's input before
+ * rnn_dropout, the highway term), h, c, grad_h, grad_x: [len, batch, dir*d]; init, mask_h, grad_last, grad_init:
+ * [batch, dir*d]; bias, grad_bias: [bias1 (dir*d) | bias2 (dir*d)].  A bidirectional column with j >= d runs
+ * backwards in time.  With g1 = sigmoid(u1 + bias1[j]), g2 = sigmoid(u2 + bias2[j]), sigmoid(v) = 1 / (1 + expf(-v)):
+ *   c_t = (c_{t-1} - u0) g1 + u0 (c_{-1} = init),  h_t = (act(c_t) mask_h - x') g2 + x',
+ * act = identity / tanhf / relu for activation 0 / 1 / 2, x' = u3 for k = 4 and x for k = 3.  The backward is the
+ * reference's: grad_u, grad_x (k = 3) and grad_init for every column, grad_bias summed over the batch in b order (a
+ * second launch over the workspace's [2, batch, dir*d] partials; no atomics).  Float32 in the reference's expressions
+ * and order, no FMA contraction: bit-identical to the reference's kernels compiled with -fmad=false.  One thread
+ * runs one column's loop over time, so a column's bits do not depend on batch, launch or run.  init, mask_h and
+ * grad_last may be NULL (zeros, ones, zeros); grad_init may be NULL (not written).  Any 4-byte alignment.  Neither
+ * call allocates or synchronises: graph-capturable.
+ * QD_ERR_INVALID_ARG: len, batch or d < 1; k not 3 or 4; bidirectional not 0 / 1; activation not 0, 1 or 2; x (or
+ * grad_x) NULL with k = 3 or given with k = 4; sizes past 64-bit indexing; NULL or misaligned pointers; outputs
+ * overlapping the inputs or each other.  QD_ERR_WORKSPACE: a missing, short or misaligned workspace.  Nothing is
+ * written on a refusal. */
+#define QD_SRU_IDENTITY 0
+#define QD_SRU_TANH 1
+#define QD_SRU_RELU 2
+int qd_sru_fwd(const float* u, const float* x, const float* bias, const float* init, const float* mask_h, int64_t len,
+               int64_t batch, int64_t d, int k, int bidirectional, int activation, float* h, float* c,
+               qd_stream_t stream);
+/* The backward's workspace: 2*batch*dir*d floats. */
+size_t qd_sru_workspace_bytes(int64_t batch, int64_t d, int bidirectional);
+/* c as written by qd_sru_fwd on the same u, x, bias, init, mask_h.  Two launches. */
+int qd_sru_bwd(const float* u, const float* x, const float* bias, const float* init, const float* mask_h,
+               const float* c, const float* grad_h, const float* grad_last, int64_t len, int64_t batch, int64_t d,
+               int k, int bidirectional, int activation, float* grad_u, float* grad_x, float* grad_bias,
+               float* grad_init, void* workspace, size_t workspace_bytes, qd_stream_t stream);
+
 /* ---- one beam search step of B sentences (onmt/Beam.py:55-106, Beam.advance; Translator.translateBatch) ----------
  * Rows follow onmt's beam-major decoder batch: row r = k*B + b is beam k of sentence b (K = beam).  out: float32
  * [K*B, V], C order, any 4-byte alignment.  With normalize = 0 it holds log-probabilities lp; with normalize = 1 the

@@ -159,5 +159,16 @@ for K, B, V in ((1, 3, 1), (2, 1, 5), (5, 7, 1025), (16, 2, 10_004)):
         bb.advance(buf[1:].view(K * B, V), torch.rand(K * B, 4, device="cuda"), normalized)
         bb.tokens[t + 1, 0, 0] = V - 1
     bb.done()
+# SRU recurrence, forward and backward: k = 3 and 4 (the float4 path and, at an offset view, the scalar one), both
+# directions, len 1 and longer than the load ring, one column and several CTAs
+from quantized_distillation_b200.sru import sru_compute  # noqa: E402
+for L, B, d, k, bi, off in ((1, 1, 1, 4, False, 0), (7, 3, 5, 3, True, 0), (9, 2, 70, 4, True, 1), (5, 4, 40, 3, False, 1)):
+    D = d * (2 if bi else 1)
+    xin = torch.randn(L, B, D if k == 3 else 3, device="cuda", requires_grad=True)
+    ubuf = torch.randn(L * B * D * k + off, device="cuda")
+    u = ubuf[off:].view(L * B, D * k).detach().requires_grad_(True)
+    init = torch.randn(B, D, device="cuda", requires_grad=True)
+    h, last = sru_compute(u, xin, torch.randn(2 * D, device="cuda"), d, bi, 1, init=init, mask_h=torch.rand(B, D, device="cuda"))
+    (h.sum() + last.sum()).backward()
 torch.cuda.synchronize()
 print("sanitize probe ok")
