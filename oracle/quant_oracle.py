@@ -281,6 +281,23 @@ def nonuniform_fwd(x, points, bucket_size, rule="nearest", subtract_mean=False, 
     return q, idx, st
 
 
+def dequantize_levels(idx, alpha, beta, bucket_size, s=None, points=None) -> np.ndarray:
+    """q of stored levels: unit * alpha + beta of the element's bucket, one float32 rounding per op, where unit is
+    idx / (s-1) (uniform, quant_functions.py:191) or points[idx] (non-uniform, :278-289), then the inverse scaling's
+    mul_ and add_ (:142-143).  Any bucket, ragged last row included; no mean is added (the stored models have
+    none), so a -0.0 stays -0.0.  The flat float32 array of idx.size elements."""
+    i = np.asarray(idx).reshape(-1).astype(np.int64)
+    _, row_len, _ = bucket_geometry(i.size, bucket_size)
+    if points is None:
+        unit = (i.astype(F32) / F32(s - 1)).astype(F32)
+    else:
+        unit = np.asarray(points, dtype=F32).reshape(-1)[i]
+    row = np.arange(i.size, dtype=np.int64) // row_len
+    a = np.asarray(alpha, dtype=F32).reshape(-1)[row]
+    b = np.asarray(beta, dtype=F32).reshape(-1)[row]
+    return ((unit * a).astype(F32) + b).astype(F32)
+
+
 # --------------------------------------------------------------------------
 # a8: gradient w.r.t. the centroids (quant_functions.py:471-506)
 # --------------------------------------------------------------------------
