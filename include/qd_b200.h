@@ -416,6 +416,68 @@ int qd_sru_bwd(const float* u, const float* x, const float* bias, const float* i
                int k, int bidirectional, int activation, float* grad_u, float* grad_x, float* grad_bias,
                float* grad_init, void* workspace, size_t workspace_bytes, qd_stream_t stream);
 
+/* ---- the core of onmt's MultiHeadedAttention (onmt/modules/MultiHeadedAttn.py:44-110, between the projections and
+ * the residual) ------------------------------------------------------------------------------------------------------
+ * D = heads*dh.  q, out, grad_out, grad_q: float32 [B, Lq, D]; k, v, grad_k, grad_v: [B, Lk, D], C order, the
+ * projections' own layout: head hd of row (b, t) is q[(b*Lq + t)*D + hd*dh + j].  probs: [B, heads, Lq, Lk]; top,
+ * grad_top: [B, Lq, Lk]; keep: uint8 [B*heads, Lq, Lk] (0 or 1), all C order.  mask: uint8 (or bool) [B, Lq, Lk] read at
+ * mask[b*sB + t*sQ + s*sK] (strides in elements, >= 0: the stride-0 expanded padding masks are read in place), nonzero
+ * = masked; NULL for none.  Per (b, head, t), with x_s = fl(q . k_s) / fl(sqrt(dh)), -inf where masked:
+ *   p = softmax_s(x) (an all-masked row is NaN, as torch's),  p' = p keep scale (keep NULL: p' = p),
+ *   out[b, t, hd] = sum_s p'_s v_s,  top = p of head 0.
+ * Arithmetic: float32, one IEEE rounding per operation (no FMA).  A dot product over dh is a sum over j = l + 32i per
+ * lane l, in i order, then a butterfly over the 32 lanes; the softmax takes the row maximum m, l = sum_s expf(x_s - m)
+ * (per lane in s order, then a butterfly), p = expf(x - m) / l; out and grad_q are sums over s in order, grad_k and
+ * grad_v over t in order.  All of it depends on (Lk, dh) alone: a row gives the same bits alone or in any batch, and
+ * every call the same bits on every run.  Error: a float32 sum of k terms in these orders is within (ceil(k/32) + 6) *
+ * 2^-24 * sum|terms| (lane sums) or (k + 2) * 2^-24 * sum|terms| (ordered sums) of the exact one, and each operation
+ * with a subnormal result up to 2^-149 more.  The tests allow twice these bounds, propagated through the chain to
+ * first order (oracle/mha_oracle.py, core_bounds).
+ * Neither call allocates or synchronises: graph-capturable.
+ * QD_ERR_INVALID_ARG: B, Lq, Lk, heads or dh < 1; negative mask strides; sizes or the mask's extent past 64-bit
+ * indexing; a non-finite keep_scale with keep; NULL or misaligned (4-byte) float pointers; outputs (and the workspace)
+ * overlapping the inputs or each other.  QD_ERR_WORKSPACE: a missing, short or misaligned workspace.  Nothing is
+ * written on a refusal. */
+int qd_mha_fwd(const float* q, const float* k, const float* v, const uint8_t* mask, int64_t mask_batch_stride,
+               int64_t mask_query_stride, int64_t mask_key_stride, const uint8_t* keep, float keep_scale, int64_t B,
+               int64_t Lq, int64_t Lk, int64_t heads, int64_t dh, float* out, float* probs, float* top,
+               qd_stream_t stream);
+/* The backward's workspace: B*heads*Lq*Lk floats (dS). */
+size_t qd_mha_workspace_bytes(int64_t B, int64_t heads, int64_t Lq, int64_t Lk);
+/* The reference's two softmax calls have equal values, so their gradients add: G_s = fl(grad_out . v_s) keep scale
+ * (+ grad_top_s on head 0; grad_top may be NULL), dS = p (G - sum_s p G) / fl(sqrt(dh)), 0 where masked (masked_fill's
+ * backward: an all-masked row gives grad_q 0 and no share of grad_k), grad_q = sum_s dS_s k_s; grad_k[s] = sum_t
+ * dS_{t,s} q_t and grad_v[s] = sum_t p'_{t,s} grad_out_t, no atomics.  probs as written by qd_mha_fwd on the same q, k,
+ * v, mask, keep.  Two launches: one owns query rows (dS into the workspace, grad_q), one owns keys (grad_k, grad_v). */
+int qd_mha_bwd(const float* grad_out, const float* grad_top, const float* q, const float* k, const float* v,
+               const float* probs, const uint8_t* mask, int64_t mask_batch_stride, int64_t mask_query_stride,
+               int64_t mask_key_stride, const uint8_t* keep, float keep_scale, int64_t B, int64_t Lq, int64_t Lk,
+               int64_t heads, int64_t dh, float* grad_q, float* grad_k, float* grad_v, void* workspace,
+               size_t workspace_bytes, qd_stream_t stream);
+
+/* ---- onmt's own LayerNorm (onmt/modules/UtilClass.py:24-46), not torch's ------------------------------------------
+ * Rows of width d: x, residual, y, grad_y, grad_x: float32 [rows, d]; a_2, b_2, grad_a_2, grad_b_2: [d], C order.
+ * z = fl(x + residual) (residual NULL: z = x), mu = sum z / d, sd = sqrt(sum (z - mu)^2 / (d - 1)) (unbiased),
+ *   y = fl(fl(fl(z - mu) / fl(sd + eps)) a_2) + b_2;   d = 1: y = z, as the reference returns z unchanged.
+ * One warp per row; sums over j = l + 32i per lane l, in i order, then a butterfly: a row's bits depend on d alone.
+ * The backward recomputes z, mu and sd in the same order (the same bits) and writes
+ *   grad_x = (g - mean g) / (sd + eps) + k (z - mu),  g = grad_y a_2,  k = -(sum g (z - mu) / (sd + eps)^2) / ((d-1) sd),
+ * which is also the residual's gradient; grad_a_2 = sum over rows of grad_y xhat and grad_b_2 = sum of grad_y, each per
+ * column over chunks of 32 rows in row order into the workspace, then over the chunks in order by a second launch; no
+ * atomics.  d = 1: grad_x = grad_y, grad_a_2 = grad_b_2 = 0.  A constant row (sd = 0) gives a NaN gradient, as the
+ * reference's std backward does.  Error bounds as stated for the attention core, propagated through this chain
+ * (oracle/mha_oracle.py, layer_norm_bounds).  Neither call allocates or synchronises: graph-capturable.
+ * QD_ERR_INVALID_ARG: rows < 0, d < 1, rows * d past 64-bit indexing, non-finite eps, NULL or misaligned pointers
+ * (residual may be NULL), outputs overlapping the inputs or each other.  QD_ERR_WORKSPACE: a missing, short or
+ * misaligned workspace.  Nothing is written on a refusal. */
+int qd_onmt_layernorm_fwd(const float* x, const float* residual, const float* a_2, const float* b_2, int64_t rows,
+                          int64_t d, float eps, float* y, qd_stream_t stream);
+/* The backward's workspace: 2 * ceil(rows / 32) * d floats; 0 when d = 1 or rows = 0. */
+size_t qd_onmt_layernorm_workspace_bytes(int64_t rows, int64_t d);
+int qd_onmt_layernorm_bwd(const float* grad_y, const float* x, const float* residual, const float* a_2, int64_t rows,
+                          int64_t d, float eps, float* grad_x, float* grad_a_2, float* grad_b_2, void* workspace,
+                          size_t workspace_bytes, qd_stream_t stream);
+
 /* ---- one beam search step of B sentences (onmt/Beam.py:55-106, Beam.advance; Translator.translateBatch) ----------
  * Rows follow onmt's beam-major decoder batch: row r = k*B + b is beam k of sentence b (K = beam).  out: float32
  * [K*B, V], C order, any 4-byte alignment.  With normalize = 0 it holds log-probabilities lp; with normalize = 1 the

@@ -73,6 +73,13 @@ SIGNATURES = {
     "qd_sru_fwd": (C.c_int, [_p, _p, _p, _p, _p, _i64, _i64, _i64, _i32, _i32, _i32, _p, _p, _p]),
     "qd_sru_workspace_bytes": (_sz, [_i64, _i64, _i32]),
     "qd_sru_bwd": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i32, _i32, _i32, _p, _p, _p, _p, _p, _sz, _p]),
+    "qd_mha_fwd": (C.c_int, [_p, _p, _p, _p, _i64, _i64, _i64, _p, _f32, _i64, _i64, _i64, _i64, _i64, _p, _p, _p, _p]),
+    "qd_mha_workspace_bytes": (_sz, [_i64, _i64, _i64, _i64]),
+    "qd_mha_bwd": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _p, _f32, _i64, _i64, _i64, _i64, _i64, _p, _p, _p,
+                             _p, _sz, _p]),
+    "qd_onmt_layernorm_fwd": (C.c_int, [_p, _p, _p, _p, _i64, _i64, _f32, _p, _p]),
+    "qd_onmt_layernorm_workspace_bytes": (_sz, [_i64, _i64]),
+    "qd_onmt_layernorm_bwd": (C.c_int, [_p, _p, _p, _p, _i64, _i64, _f32, _p, _p, _p, _p, _sz, _p]),
     "qd_beam_workspace_bytes": (_sz, [_i64, _i32]),
     "qd_beam_step": (C.c_int, [_p, _i32, _i64, _i32, _i64, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
     "qd_beam_finish": (C.c_int, [_p, _p, _p, _p, _i64, _i64, _i32, _i64, _i64, _i32, _p, _p, _p, _p, _p]),

@@ -8,7 +8,7 @@ import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-SOURCES = [os.path.join(HERE, "csrc", f) for f in ("qd_launch.cu", "qd_quant.cu", "qd_codec.cu", "qd_recurrent.cu", "qd_nmt_loss.cu", "qd_attention.cu", "qd_sru.cu", "qd_beam.cu", "qd_bleu.cu", "qd_plans.cu", "qd_stats.cu",
+SOURCES = [os.path.join(HERE, "csrc", f) for f in ("qd_launch.cu", "qd_quant.cu", "qd_codec.cu", "qd_recurrent.cu", "qd_nmt_loss.cu", "qd_attention.cu", "qd_sru.cu", "qd_mha.cu", "qd_beam.cu", "qd_bleu.cu", "qd_plans.cu", "qd_stats.cu",
                                                    "qd_host.cu")]
 HEADERS = [os.path.join(HERE, "csrc", f) for f in ("qd_launch.h", "qd_common.cuh", "qd_rowops.cuh", "qd_warp_path.cuh", "qd_block_path.cuh",
                                                    "qd_staged_path.cuh", "qd_abs_path.cuh", "qd_select.cuh", "qd_grid_path.cuh", "qd_points_grad.cuh", "qd_plan.cuh", "qd_huffman.cuh",
