@@ -187,6 +187,13 @@ def ptr(t):
     return None if t is None else t.data_ptr()
 
 
+def check_float_cuda(t, what, dims=None):
+    """ValueError unless t is a float32 CUDA tensor (of `dims` dimensions when given): these ops have no CPU path."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or (dims is not None and t.dim() != dims):
+        shape = "" if dims is None else f"{dims}-D "
+        raise ValueError(f"{what} must be a {shape}float32 CUDA tensor (no CPU implementation)")
+
+
 def stream_ptr(device=None):
     return torch.cuda.current_stream(device).cuda_stream
 

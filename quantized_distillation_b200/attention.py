@@ -70,11 +70,6 @@ class _AttentionCore(torch.autograd.Function):
         return grad_q, grad_input, grad_context, None
 
 
-def _check_tensor(t, what, dims):
-    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or t.dim() != dims:
-        raise ValueError(f"{what} must be a {dims}-D float32 CUDA tensor (no CPU implementation)")
-
-
 def attention_core(q, input, context, kind):
     """(align, concat) of the attention core for queries q and decoder outputs input [N, T, H] (q is input for dot)
     against context [N, S, H] (any strides; the transposed view of a contiguous [S, N, H] is read in place).
@@ -83,9 +78,9 @@ def attention_core(q, input, context, kind):
     N.require_cuda()
     if kind not in (ATTN_DOT, ATTN_GENERAL):
         raise ValueError("kind must be ATTN_DOT or ATTN_GENERAL")
-    _check_tensor(input, "input", 3)
-    _check_tensor(context, "context", 3)
-    _check_tensor(q, "q", 3)
+    N.check_float_cuda(input, "input", 3)
+    N.check_float_cuda(context, "context", 3)
+    N.check_float_cuda(q, "q", 3)
     if kind == ATTN_DOT and q is not input:
         raise ValueError("dot attention takes the input itself as its query")
     if q.shape != input.shape or context.shape[0] != input.shape[0] or context.shape[2] != input.shape[2]:
@@ -135,13 +130,13 @@ class GlobalAttention(nn.Module):
         [N, S] for one step, else contiguous [T, N, H] and [T, N, S], as the reference."""
         if coverage is not None:
             raise NotImplementedError("coverage attention is not implemented")
-        _check_tensor(context, "context", 3)
+        N.check_float_cuda(context, "context", 3)
         if not isinstance(input, torch.Tensor) or input.dim() not in (2, 3):
             raise ValueError("input must be [N, H] or [N, T, H]")
         one_step = input.dim() == 2
         if one_step:
             input = input.unsqueeze(1)
-        _check_tensor(input, "input", 3)
+        N.check_float_cuda(input, "input", 3)
         if input.shape[0] != context.shape[0] or input.shape[2] != self.dim or context.shape[2] != self.dim:
             raise ValueError(f"input {tuple(input.shape)} and context {tuple(context.shape)} do not match dim {self.dim}")
         input = input.contiguous()

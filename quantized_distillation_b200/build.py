@@ -12,7 +12,7 @@ SOURCES = [os.path.join(HERE, "csrc", f) for f in ("qd_launch.cu", "qd_quant.cu"
                                                    "qd_host.cu")]
 HEADERS = [os.path.join(HERE, "csrc", f) for f in ("qd_launch.h", "qd_common.cuh", "qd_rowops.cuh", "qd_warp_path.cuh", "qd_block_path.cuh",
                                                    "qd_staged_path.cuh", "qd_abs_path.cuh", "qd_select.cuh", "qd_grid_path.cuh", "qd_points_grad.cuh", "qd_plan.cuh", "qd_huffman.cuh",
-                                                   "qd_packed_walk.cuh", "qd_lse.cuh")]
+                                                   "qd_packed_walk.cuh", "qd_lse.cuh", "qd_attn_tile.cuh")]
 HEADERS.append(os.path.join(ROOT, "include", "qd_b200.h"))
 OUT = os.path.join(HERE, "libqd_b200.so")
 

@@ -7,10 +7,10 @@
 // context + n*sN + s*sS + h: the contiguous [N, S, H] and the transposed view of a contiguous [S, N, H] alike.
 //
 // Forward (qd_attn_fwd): one 256-thread CTA per tile of up to kAtTile rows of one n, three phases:
-//   1. scores: warp w owns the source positions s = w + 8k, lane l the elements h = l + 32j; per row a lane-strided
-//      float32 sum and a butterfly over the warp.  The raw scores go to align.
-//   2. softmax: warp t owns row t of the tile; max, then sum of expf(x - max) (lane-strided, butterfly), then
-//      align = expf(x - max) / sum in place.
+//   1. scores (qd_attn_tile.cuh's tile_dots): warp w owns the source positions s = w + 8k, lane l the elements
+//      h = l + 32j; per row a lane-strided float32 sum and a butterfly over the warp.  The raw scores go to align.
+//   2. softmax (softmax_row): warp t owns row t of the tile; max, then sum of expf(x - max) (lane-strided, butterfly),
+//      then align = expf(x - max) / sum in place.
 //   3. context: thread j owns h = j + 256k and sums align_s * h_s over s in order; it writes c and copies input beside.
 // The slab is read from HBM once per tile in phase 1; phase 3 reads it again from L2 (at most S*H*4 bytes per tile).
 //
@@ -22,6 +22,7 @@
 // same alone or in any batch; all loads are scalar, so the alignment of a view changes nothing either.
 #include <cmath>
 
+#include "qd_attn_tile.cuh"
 #include "qd_launch.h"
 
 using namespace qd;
@@ -32,50 +33,7 @@ constexpr int kAtThreads = 256;
 constexpr int kAtWarps = kAtThreads / 32;
 constexpr int kAtTile = 8;          // query rows of one batch entry per CTA (phase 2 gives each a warp)
 constexpr int kAtSChunk = 8;        // source positions per CTA of the context gradient
-constexpr int64_t kAtMaxGrid = 1 << 20, kAtMaxGridY = 65535;
 static_assert(kAtTile <= kAtWarps, "phase 2 gives each row of a tile its own warp");
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-
-// out[t*os + s] = v_t . h_s (+ add[t*os + s]) for the nt rows v_t = v + t*vs of a tile and every s < S
-__device__ __forceinline__ void tile_dots(const float* __restrict__ ctx, int64_t sS, int64_t S, int64_t H,
-                                          const float* __restrict__ v, int64_t vs, int nt, const float* __restrict__ add,
-                                          float* out, int64_t os) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int64_t s = warp; s < S; s += kAtWarps) {
-        const float* hs = ctx + s * sS;
-        float acc[kAtTile];
-#pragma unroll
-        for (int t = 0; t < kAtTile; ++t) acc[t] = 0.f;
-#pragma unroll 4
-        for (int64_t j = lane; j < H; j += 32) {
-            const float x = __ldg(hs + j);
-#pragma unroll
-            for (int t = 0; t < kAtTile; ++t)
-                if (t < nt) acc[t] = __fadd_rn(acc[t], __fmul_rn(__ldg(v + t * vs + j), x));
-        }
-#pragma unroll
-        for (int t = 0; t < kAtTile; ++t) {
-            if (t < nt) {
-                float d = warp_sum(acc[t]);
-                if (lane == 0) {
-                    if (add != nullptr) d = __fadd_rn(d, __ldg(add + t * os + s));
-                    out[t * os + s] = d;
-                }
-            }
-        }
-    }
-}
 
 // out[t*os + h] = sum_s p[t*ps + s] h_s[h] for the nt rows of a tile, s in order
 __device__ __forceinline__ void tile_weighted_sum(const float* __restrict__ ctx, int64_t sS, int64_t S, int64_t H,
@@ -120,17 +78,12 @@ __global__ void __launch_bounds__(kAtThreads) attn_fwd_kernel(AtFwdArgs a) {
         const int64_t in_row = (n * g.T + t0) * g.H, out_row = t0 * g.N + n;
         float* al = a.align + out_row * g.S;
         const int64_t as = g.N * g.S;
-        tile_dots(ctx, g.sS, g.S, g.H, a.q + in_row, g.H, nt, nullptr, al, as);
+        attn::tile_dots<kAtTile, kAtWarps, 4>(a.q + in_row, g.H, ctx, g.sS, g.S, g.H, nt,
+                                              [&](int t, int64_t s, float d) { al[t * as + s] = d; });
         __syncthreads();
         if (warp < nt) {
             float* row = al + warp * as;
-            float m = -INFINITY;
-            for (int64_t s = lane; s < g.S; s += 32) m = fmaxf(m, row[s]);
-            m = warp_max(m);
-            float l = 0.f;
-            for (int64_t s = lane; s < g.S; s += 32) l = __fadd_rn(l, expf(__fsub_rn(row[s], m)));
-            l = warp_sum(l);
-            for (int64_t s = lane; s < g.S; s += 32) row[s] = __fdiv_rn(expf(__fsub_rn(row[s], m)), l);
+            attn::softmax_row(row, g.S, lane, [&](int64_t s, float y) { row[s] = y; });
         }
         __syncthreads();
         float* cc = a.concat + out_row * 2 * g.H;
@@ -162,15 +115,19 @@ __global__ void __launch_bounds__(kAtThreads) attn_bwd_rows_kernel(AtBwdArgs a) 
         const int64_t in_row = (n * g.T + t0) * g.H, out_row = t0 * g.N + n;
         const int64_t as = g.N * g.S;
         float* gs = a.gs + out_row * g.S;
-        tile_dots(ctx, g.sS, g.S, g.H, a.grad_concat + out_row * 2 * g.H, g.N * 2 * g.H, nt,
-                  a.grad_align != nullptr ? a.grad_align + out_row * g.S : nullptr, gs, as);
+        const float* ga = a.grad_align != nullptr ? a.grad_align + out_row * g.S : nullptr;
+        attn::tile_dots<kAtTile, kAtWarps, 4>(a.grad_concat + out_row * 2 * g.H, g.N * 2 * g.H, ctx, g.sS, g.S, g.H, nt,
+                                              [&](int t, int64_t s, float d) {
+                                                  if (ga != nullptr) d = __fadd_rn(d, __ldg(ga + t * as + s));
+                                                  gs[t * as + s] = d;
+                                              });
         __syncthreads();
         if (warp < nt) {
             const float* al = a.align + out_row * g.S + warp * as;
             float* row = gs + warp * as;
             float d = 0.f;
             for (int64_t s = lane; s < g.S; s += 32) d = __fadd_rn(d, __fmul_rn(__ldg(al + s), row[s]));
-            d = warp_sum(d);
+            d = attn::warp_sum(d);
             for (int64_t s = lane; s < g.S; s += 32) row[s] = __fmul_rn(__ldg(al + s), __fsub_rn(row[s], d));
         }
         __syncthreads();
@@ -203,13 +160,6 @@ __global__ void __launch_bounds__(kAtThreads) attn_bwd_context_kernel(AtBwdArgs 
     }
 }
 
-bool overlap(const void* a, size_t na, const void* b, size_t nb) {
-    const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
-    return a != nullptr && b != nullptr && na > 0 && nb > 0 && pa < pb + nb && pb < pa + na;
-}
-
-bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) != 0; }
-
 // checks of the sizes and the context layout both calls share; R = N*T.  span: bytes from context to its last element
 int check_shape(const float* ctx, int64_t sN, int64_t sS, int64_t N, int64_t T, int64_t S, int64_t H, int64_t* R,
                 size_t* span) {
@@ -238,11 +188,6 @@ int check_shape(const float* ctx, int64_t sN, int64_t sS, int64_t N, int64_t T, 
     return QD_OK;
 }
 
-// blockIdx.x walks the batch entries, blockIdx.y the tiles (or source chunks) of one; both loop past the grid
-dim3 grid_of(int64_t N, int64_t tiles) {
-    return dim3((unsigned)(N < kAtMaxGrid ? N : kAtMaxGrid), (unsigned)(tiles < kAtMaxGridY ? tiles : kAtMaxGridY));
-}
-
 }  // namespace
 
 extern "C" size_t qd_attn_workspace_bytes(int64_t rows, int64_t S) {
@@ -261,20 +206,16 @@ extern "C" int qd_attn_fwd(int kind, const float* q, const float* input, const f
     if (R == 0) return QD_OK;
     if (kind == QD_ATTN_DOT) q = input;
     if (q == nullptr || input == nullptr || align == nullptr || concat == nullptr) return fail(QD_ERR_INVALID_ARG, "NULL argument");
-    if (misaligned(q) || misaligned(input) || misaligned(context) || misaligned(align) || misaligned(concat))
+    if (misaligned(q, 4) || misaligned(input, 4) || misaligned(context, 4) || misaligned(align, 4) || misaligned(concat, 4))
         return fail(QD_ERR_INVALID_ARG, "float arrays must be 4-byte aligned");
     const size_t row_bytes = (size_t)(R * H) * sizeof(float), al_bytes = (size_t)(R * S) * sizeof(float);
-    if (overlap(align, al_bytes, concat, 2 * row_bytes)) return fail(QD_ERR_INVALID_ARG, "align and concat must not overlap");
-    const float* outs[2] = {align, concat};
-    const size_t out_bytes[2] = {al_bytes, 2 * row_bytes};
-    for (int i = 0; i < 2; ++i)
-        if (overlap(outs[i], out_bytes[i], q, row_bytes) || overlap(outs[i], out_bytes[i], input, row_bytes) ||
-            overlap(outs[i], out_bytes[i], context, span))
-            return fail(QD_ERR_INVALID_ARG, "outputs must not overlap the inputs");
+    rc = check_disjoint({{q, row_bytes}, {input, row_bytes}, {context, span}}, {{align, al_bytes}, {concat, 2 * row_bytes}});
+    if (rc) return rc;
     AtFwdArgs a{};
     a.g = AtShape{context, ctx_batch_stride, ctx_src_stride, N, T, S, H};
     a.q = q, a.input = input, a.align = align, a.concat = concat;
-    attn_fwd_kernel<<<grid_of(N, (T + kAtTile - 1) / kAtTile), kAtThreads, 0, as_stream(stream)>>>(a);
+    // blockIdx.x walks the batch entries, blockIdx.y the tiles (or source chunks) of one; both loop past the grid
+    attn_fwd_kernel<<<grid_2d(N, (T + kAtTile - 1) / kAtTile), kAtThreads, 0, as_stream(stream)>>>(a);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }
@@ -290,32 +231,23 @@ extern "C" int qd_attn_bwd(const float* grad_concat, const float* grad_align, co
     if (R == 0) return QD_OK;
     if (grad_concat == nullptr || align == nullptr || q == nullptr || grad_q == nullptr || grad_context == nullptr)
         return fail(QD_ERR_INVALID_ARG, "NULL argument");
-    if (misaligned(grad_concat) || misaligned(grad_align) || misaligned(align) || misaligned(q) || misaligned(context) ||
-        misaligned(grad_q) || misaligned(grad_context))
+    if (misaligned(grad_concat, 4) || misaligned(grad_align, 4) || misaligned(align, 4) || misaligned(q, 4) ||
+        misaligned(context, 4) || misaligned(grad_q, 4) || misaligned(grad_context, 4))
         return fail(QD_ERR_INVALID_ARG, "float arrays must be 4-byte aligned");
     const size_t need = qd_attn_workspace_bytes(R, S);
-    if (workspace == nullptr || workspace_bytes < need || misaligned(workspace))
-        return fail(QD_ERR_WORKSPACE, "workspace must be 4-byte aligned and hold qd_attn_workspace_bytes(%lld, %lld) = %zu bytes",
-                    (long long)R, (long long)S, need);
+    rc = check_workspace(workspace, workspace_bytes, need, 4, "qd_attn_workspace_bytes(N * T, S)");
+    if (rc) return rc;
     const size_t row_bytes = (size_t)(R * H) * sizeof(float), al_bytes = (size_t)(R * S) * sizeof(float);
-    const void* outs[3] = {grad_q, grad_context, workspace};
-    const size_t out_bytes[3] = {row_bytes, span, need};
-    for (int i = 0; i < 3; ++i) {
-        if (overlap(outs[i], out_bytes[i], grad_concat, 2 * row_bytes) || overlap(outs[i], out_bytes[i], grad_align, al_bytes) ||
-            overlap(outs[i], out_bytes[i], align, al_bytes) || overlap(outs[i], out_bytes[i], q, row_bytes) ||
-            overlap(outs[i], out_bytes[i], context, span))
-            return fail(QD_ERR_INVALID_ARG, "outputs and workspace must not overlap the inputs");
-        for (int j = 0; j < i; ++j)
-            if (overlap(outs[i], out_bytes[i], outs[j], out_bytes[j]))
-                return fail(QD_ERR_INVALID_ARG, "outputs and workspace must not overlap each other");
-    }
+    rc = check_disjoint({{grad_concat, 2 * row_bytes}, {grad_align, al_bytes}, {align, al_bytes}, {q, row_bytes}, {context, span}},
+                        {{grad_q, row_bytes}, {grad_context, span}, {workspace, need}});
+    if (rc) return rc;
     AtBwdArgs a{};
     a.g = AtShape{context, ctx_batch_stride, ctx_src_stride, N, T, S, H};
     a.grad_concat = grad_concat, a.grad_align = grad_align, a.align = align, a.q = q;
     a.gs = static_cast<float*>(workspace), a.grad_q = grad_q, a.grad_ctx = grad_context;
     cudaStream_t st = as_stream(stream);
-    attn_bwd_rows_kernel<<<grid_of(N, (T + kAtTile - 1) / kAtTile), kAtThreads, 0, st>>>(a);
-    attn_bwd_context_kernel<<<grid_of(N, (S + kAtSChunk - 1) / kAtSChunk), kAtThreads, 0, st>>>(a);
+    attn_bwd_rows_kernel<<<grid_2d(N, (T + kAtTile - 1) / kAtTile), kAtThreads, 0, st>>>(a);
+    attn_bwd_context_kernel<<<grid_2d(N, (S + kAtSChunk - 1) / kAtSChunk), kAtThreads, 0, st>>>(a);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }

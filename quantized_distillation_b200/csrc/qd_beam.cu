@@ -30,7 +30,6 @@ namespace {
 constexpr int kRowThreads = kLseThreads;     // a row's lse must be walked exactly as the NMT loss walks it
 constexpr int kRowWarps = kRowThreads / 32;
 constexpr int kMergeWarps = 4;
-constexpr int kBeamMaxGrid = 1 << 20;        // rows or sentences beyond it loop inside the CTAs
 constexpr float kEosRowKey = -1e20f;         // Beam.py:75, beamLk[i] = -1e20 on a float32 tensor
 
 struct Cand {                                // workspace: [K*B rows][K], each row's K best, best first
@@ -306,13 +305,6 @@ __global__ void __launch_bounds__(kMergeWarps * 32) beam_finish_kernel(FinishArg
     }
 }
 
-bool overlap(const void* a, size_t na, const void* b, size_t nb) {
-    const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
-    return a != nullptr && b != nullptr && na > 0 && nb > 0 && pa < pb + nb && pb < pa + na;
-}
-
-bool misaligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; }
-
 template <int KC>
 void launch_rows(const RowArgs& a, bool normalize, unsigned grid, cudaStream_t st) {
     if (normalize) beam_row_kernel<KC, true><<<grid, kRowThreads, 0, st>>>(a);
@@ -345,26 +337,19 @@ extern "C" int qd_beam_step(const float* out, int normalize, int64_t batch, int 
         misaligned(flat_origin, 8) || misaligned(tokens, 8) || misaligned(n_finished, 4))
         return fail(QD_ERR_INVALID_ARG, "misaligned argument (out, scores, n_finished 4 bytes; token and origin arrays 8 bytes)");
     const size_t need = qd_beam_workspace_bytes(batch, beam);
-    if (workspace == nullptr || workspace_bytes < need || misaligned(workspace, 16))
-        return fail(QD_ERR_WORKSPACE, "workspace must be 16-byte aligned and hold qd_beam_workspace_bytes(%lld, %d) = %zu bytes",
-                    (long long)batch, beam, need);
+    int rc = check_workspace(workspace, workspace_bytes, need, 16, "qd_beam_workspace_bytes(batch, beam)");
+    if (rc) return rc;
     const int64_t R = batch * beam;
-    const void* ins[2] = {out, last_tokens};
-    const size_t in_bytes[2] = {(size_t)(R * V) * sizeof(float), (size_t)R * sizeof(int64_t)};
-    const void* outs[7] = {scores, origin, flat_origin, tokens, n_finished, eos_top, workspace};
-    const size_t out_bytes[7] = {(size_t)R * sizeof(float), (size_t)R * sizeof(int64_t), (size_t)R * sizeof(int64_t),
-                                 (size_t)R * sizeof(int64_t), (size_t)batch * sizeof(int32_t), (size_t)batch, need};
-    for (int i = 0; i < 7; ++i) {
-        for (int j = 0; j < 2; ++j)
-            if (overlap(outs[i], out_bytes[i], ins[j], in_bytes[j])) return fail(QD_ERR_INVALID_ARG, "outputs must not overlap the inputs");
-        for (int j = 0; j < i; ++j)
-            if (overlap(outs[i], out_bytes[i], outs[j], out_bytes[j])) return fail(QD_ERR_INVALID_ARG, "outputs must not overlap each other");
-    }
+    const size_t ids = (size_t)R * sizeof(int64_t);
+    rc = check_disjoint({{out, (size_t)(R * V) * sizeof(float)}, {last_tokens, ids}},
+                        {{scores, (size_t)R * sizeof(float)}, {origin, ids}, {flat_origin, ids}, {tokens, ids},
+                         {n_finished, (size_t)batch * sizeof(int32_t)}, {eos_top, (size_t)batch}, {workspace, need}});
+    if (rc) return rc;
     RowArgs ra{};
     ra.out = out, ra.scores = scores, ra.last_tokens = last_tokens, ra.cand = static_cast<Cand*>(workspace);
     ra.B = batch, ra.V = V, ra.eos = eos, ra.K = beam, ra.first = first_step != 0;
     const int64_t rows = first_step ? batch : R;
-    const unsigned grid = (unsigned)(rows < kBeamMaxGrid ? rows : kBeamMaxGrid);
+    const unsigned grid = clamp_grid(rows);
     cudaStream_t st = as_stream(stream);
     if (beam == 1) launch_rows<1>(ra, normalize, grid, st);
     else if (beam == 2) launch_rows<2>(ra, normalize, grid, st);
@@ -375,7 +360,7 @@ extern "C" int qd_beam_step(const float* out, int normalize, int64_t batch, int 
     ma.cand = ra.cand, ma.scores = scores, ma.origin = origin, ma.flat_origin = flat_origin, ma.tokens = tokens;
     ma.n_finished = n_finished, ma.eos_top = eos_top, ma.B = batch, ma.eos = eos, ma.K = beam, ma.first = ra.first;
     const int64_t merge_blocks = (batch + kMergeWarps - 1) / kMergeWarps;
-    beam_merge_kernel<<<(unsigned)(merge_blocks < kBeamMaxGrid ? merge_blocks : kBeamMaxGrid), kMergeWarps * 32, 0, st>>>(ma);
+    beam_merge_kernel<<<clamp_grid(merge_blocks), kMergeWarps * 32, 0, st>>>(ma);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }
@@ -403,23 +388,17 @@ extern "C" int qd_beam_finish(const int64_t* tokens, const int64_t* origins, con
         misaligned(hyp_tokens, 8) || misaligned(hyp_len, 8) || misaligned(hyp_scores, 4) || misaligned(attn_argmax, 8))
         return fail(QD_ERR_INVALID_ARG, "misaligned argument (int64 arrays 8 bytes, float arrays 4 bytes)");
     const int64_t R = batch * beam, H = batch * n_best;
-    const void* ins[4] = {tokens, origins, step_scores, attn};
-    const size_t in_bytes[4] = {(size_t)((steps + 1) * R) * 8, (size_t)(steps * R) * 8, (size_t)(steps * R) * 4,
-                                (size_t)(steps * R * src_len) * 4};
-    const void* outs[4] = {hyp_tokens, hyp_len, hyp_scores, attn_argmax};
-    const size_t out_bytes[4] = {(size_t)(H * steps) * 8, (size_t)H * 8, (size_t)H * 4, (size_t)(H * steps) * 8};
-    for (int i = 0; i < 4; ++i) {
-        for (int j = 0; j < 4; ++j)
-            if (overlap(outs[i], out_bytes[i], ins[j], in_bytes[j])) return fail(QD_ERR_INVALID_ARG, "outputs must not overlap the inputs");
-        for (int j = 0; j < i; ++j)
-            if (overlap(outs[i], out_bytes[i], outs[j], out_bytes[j])) return fail(QD_ERR_INVALID_ARG, "outputs must not overlap each other");
-    }
+    const int rc = check_disjoint({{tokens, (size_t)((steps + 1) * R) * 8}, {origins, (size_t)(steps * R) * 8},
+                                   {step_scores, (size_t)(steps * R) * 4}, {attn, (size_t)(steps * R * src_len) * 4}},
+                                  {{hyp_tokens, (size_t)(H * steps) * 8}, {hyp_len, (size_t)H * 8}, {hyp_scores, (size_t)H * 4},
+                                   {attn_argmax, (size_t)(H * steps) * 8}});
+    if (rc) return rc;
     FinishArgs fa{};
     fa.tokens = tokens, fa.origins = origins, fa.step_scores = step_scores, fa.attn = attn;
     fa.hyp_tokens = hyp_tokens, fa.hyp_len = hyp_len, fa.hyp_scores = hyp_scores, fa.attn_argmax = attn_argmax;
     fa.T = steps, fa.B = batch, fa.S = src_len, fa.eos = eos, fa.K = beam, fa.n_best = n_best;
     const int64_t blocks = (batch + kMergeWarps - 1) / kMergeWarps;
-    beam_finish_kernel<<<(unsigned)(blocks < kBeamMaxGrid ? blocks : kBeamMaxGrid), kMergeWarps * 32, 0, as_stream(stream)>>>(fa);
+    beam_finish_kernel<<<clamp_grid(blocks), kMergeWarps * 32, 0, as_stream(stream)>>>(fa);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }

@@ -21,7 +21,6 @@ namespace {
 constexpr int kStatsWarps = 4;
 constexpr int kStageWords = 2048;            // per warp: 8 KB, 32 KB per CTA
 constexpr int kFoldThreads = 256;
-constexpr int kBleuMaxGrid = 1 << 20;        // sentences beyond it loop inside the CTAs
 constexpr int64_t kNoReference = 9999;       // multi-bleu's ($closest_diff, $closest_length) start
 
 struct StatsArgs {
@@ -150,13 +149,6 @@ __global__ void __launch_bounds__(kFoldThreads) bleu_fold_kernel(const int64_t* 
     }
 }
 
-bool overlap(const void* a, size_t na, const void* b, size_t nb) {
-    const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
-    return a != nullptr && b != nullptr && na > 0 && nb > 0 && pa < pb + nb && pb < pa + na;
-}
-
-bool misaligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; }
-
 }  // namespace
 
 extern "C" int qd_bleu_stats(const int32_t* hyp_words, int64_t n_hyp_words, const int64_t* hyp_offsets, int64_t n_sent,
@@ -175,18 +167,17 @@ extern "C" int qd_bleu_stats(const int32_t* hyp_words, int64_t n_hyp_words, cons
     if (misaligned(hyp_words, 4) || misaligned(ref_words, 4) || misaligned(hyp_offsets, 8) || misaligned(ref_offsets, 8) ||
         misaligned(ref_first, 8) || misaligned(ref_count, 8) || misaligned(stats, 8))
         return fail(QD_ERR_INVALID_ARG, "misaligned argument (word arrays 4 bytes, offsets, spans and stats 8 bytes)");
-    const void* ins[6] = {hyp_words, hyp_offsets, ref_words, ref_offsets, ref_first, ref_count};
-    const size_t in_bytes[6] = {(size_t)n_hyp_words * 4, (size_t)(n_sent + 1) * 8, (size_t)n_ref_words * 4,
-                                (size_t)(n_refs + 1) * 8, (size_t)n_sent * 8, (size_t)n_sent * 8};
-    for (int j = 0; j < 6; ++j)
-        if (overlap(stats, (size_t)n_sent * QD_BLEU_STATS * 8, ins[j], in_bytes[j]))
-            return fail(QD_ERR_INVALID_ARG, "stats must not overlap the inputs");
+    const int rc = check_disjoint({{hyp_words, (size_t)n_hyp_words * 4}, {hyp_offsets, (size_t)(n_sent + 1) * 8},
+                                   {ref_words, (size_t)n_ref_words * 4}, {ref_offsets, (size_t)(n_refs + 1) * 8},
+                                   {ref_first, (size_t)n_sent * 8}, {ref_count, (size_t)n_sent * 8}},
+                                  {{stats, (size_t)n_sent * QD_BLEU_STATS * 8}});
+    if (rc) return rc;
     StatsArgs sa{};
     sa.hyp_words = hyp_words, sa.hyp_offsets = hyp_offsets, sa.ref_words = ref_words, sa.ref_offsets = ref_offsets;
     sa.ref_first = ref_first, sa.ref_count = ref_count, sa.stats = stats;
     sa.n_hyp_words = n_hyp_words, sa.n_sent = n_sent, sa.n_ref_words = n_ref_words, sa.n_refs = n_refs;
     const int64_t blocks = (n_sent + kStatsWarps - 1) / kStatsWarps;
-    bleu_stats_kernel<<<(unsigned)(blocks < kBleuMaxGrid ? blocks : kBleuMaxGrid), kStatsWarps * 32, 0, as_stream(stream)>>>(sa);
+    bleu_stats_kernel<<<clamp_grid(blocks), kStatsWarps * 32, 0, as_stream(stream)>>>(sa);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }
@@ -196,8 +187,8 @@ extern "C" int qd_bleu_fold(const int64_t* stats, int64_t n_sent, int64_t* total
     if (n_sent > INT64_MAX / 16 / QD_BLEU_STATS) return fail(QD_ERR_INVALID_ARG, "n_sent past 64-bit indexing");
     if (totals == nullptr || (n_sent > 0 && stats == nullptr)) return fail(QD_ERR_INVALID_ARG, "NULL argument");
     if (misaligned(stats, 8) || misaligned(totals, 8)) return fail(QD_ERR_INVALID_ARG, "misaligned argument (8 bytes)");
-    if (overlap(totals, QD_BLEU_STATS * 8, stats, (size_t)n_sent * QD_BLEU_STATS * 8))
-        return fail(QD_ERR_INVALID_ARG, "totals must not overlap stats");
+    const int rc = check_disjoint({{stats, (size_t)n_sent * QD_BLEU_STATS * 8}}, {{totals, QD_BLEU_STATS * 8}});
+    if (rc) return rc;
     bleu_fold_kernel<<<1, kFoldThreads, 0, as_stream(stream)>>>(stats, n_sent, totals);
     QD_CUDA(cudaGetLastError());
     return QD_OK;

@@ -1,10 +1,12 @@
 // qd_launch.h -- host layer shared by every translation unit of libqd_b200.so (state in qd_launch.cu): the
-// per-thread error message, device properties and grid sizing.  Host code only.
+// per-thread error message, device properties, grid sizing and the argument checks of the C entry points.  Host code
+// only.
 #pragma once
 #include <cuda_runtime.h>
 
 #include <cstddef>
 #include <cstdint>
+#include <initializer_list>
 #include <type_traits>
 
 #include "qd_b200.h"
@@ -40,6 +42,45 @@ int opt_in_smem(const void* kernel, size_t smem, size_t* opted);
 
 inline cudaStream_t as_stream(qd_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// Grids of kernels that loop past their grid: at most kMaxGrid CTAs along x, 65535 along y.
+constexpr int64_t kMaxGrid = 1 << 20;
+inline unsigned clamp_grid(int64_t ctas) { return (unsigned)(ctas < kMaxGrid ? ctas : kMaxGrid); }
+inline dim3 grid_2d(int64_t x, int64_t y) { return dim3(clamp_grid(x), (unsigned)(y < 65535 ? y : 65535)); }
+
+// ---- argument checks of the C entry points: each returns before any CUDA call ----
+// [a, a + na) and [b, b + nb) share a byte; a NULL pointer or an empty range overlaps nothing
+inline bool overlap(const void* a, size_t na, const void* b, size_t nb) {
+    const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
+    return a != nullptr && b != nullptr && na > 0 && nb > 0 && pa < pb + nb && pb < pa + na;
+}
+// p is not a multiple of `bytes` (a power of two); NULL is aligned
+inline bool misaligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; }
+
+struct Span {
+    const void* p;
+    size_t bytes;
+};
+
+// QD_ERR_INVALID_ARG unless every output is disjoint from every input and from every earlier output; outputs are
+// checked in order, each against the inputs first
+inline int check_disjoint(std::initializer_list<Span> in, std::initializer_list<Span> out) {
+    for (const Span* o = out.begin(); o != out.end(); ++o) {
+        for (const Span& i : in)
+            if (overlap(o->p, o->bytes, i.p, i.bytes)) return fail(QD_ERR_INVALID_ARG, "outputs must not overlap the inputs");
+        for (const Span* e = out.begin(); e != o; ++e)
+            if (overlap(o->p, o->bytes, e->p, e->bytes)) return fail(QD_ERR_INVALID_ARG, "outputs must not overlap each other");
+    }
+    return QD_OK;
+}
+
+// QD_ERR_WORKSPACE unless ws is non-NULL, `align`-byte aligned and holds `need` bytes.  `query` names the size query
+// that returns need.
+inline int check_workspace(const void* ws, size_t bytes, size_t need, uintptr_t align, const char* query) {
+    if (ws == nullptr || bytes < need || misaligned(ws, align))
+        return fail(QD_ERR_WORKSPACE, "workspace must be %d-byte aligned and hold %s = %zu bytes", (int)align, query, need);
+    return QD_OK;
+}
 
 // Calls f(std::integral_constant<int, R>{}) with the registers per lane of the warp-row kernels for rows of
 // `row_len` floats: R = 2 up to 256, 4 up to 512, 8 above.  MAX_R = 4 leaves R = 8 uninstantiated.

@@ -7,7 +7,7 @@
 // workspace are [B, h, Lq, Lk] (bh = b*h + hd), keep [B*h, Lq, Lk], top [B, Lq, Lk], out [B, Lq, D].
 //
 // Forward (qd_mha_fwd): one 256-thread CTA per (b, head, tile of up to kMhTile query rows), three phases:
-//   1. scores: warp w owns keys s = w + 8k, lane l the elements j = l + 32i; a lane-strided float32 sum and a
+//   1. scores (qd_attn_tile.cuh's tile_dots): warp w owns keys s = w + 8k, lane l the elements j = l + 32i; a lane-strided float32 sum and a
 //      butterfly over the warp, then x = sum / sqrt(dh), or -inf where the mask is set.  The scores go to probs.
 //   2. softmax: warp t owns row t; max, sum of expf(x - max) (lane-strided, butterfly), then p = expf(x - max) / sum in
 //      place; head 0 copies its row to top.  An all-masked row is -inf - -inf = NaN throughout, as torch's softmax.
@@ -26,6 +26,7 @@
 // alone or in any batch; all loads are scalar, so the alignment of a view changes nothing either.
 #include <cmath>
 
+#include "qd_attn_tile.cuh"
 #include "qd_launch.h"
 
 using namespace qd;
@@ -37,20 +38,7 @@ constexpr int kMhWarps = kMhThreads / 32;
 constexpr int kMhTile = 8;           // query rows of one (b, head) per CTA (phase 2 gives each a warp)
 constexpr int kMhKChunk = 8;         // keys per CTA of the key-side gradients
 constexpr int kLnChunk = 32;         // rows per CTA of the layer norm's backward (one partial per chunk and column)
-constexpr int64_t kMhMaxGrid = 1 << 20, kMhMaxGridY = 65535;
 static_assert(kMhTile <= kMhWarps, "phase 2 gives each row of a tile its own warp");
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
 
 struct MhArgs {
     const float* q;           // [B, Lq, D]
@@ -80,33 +68,6 @@ __device__ __forceinline__ float dropped(const MhArgs& a, float p, int64_t idx) 
     return a.keep == nullptr ? p : __fmul_rn(__fmul_rn(p, (float)a.keep[idx]), a.scale);
 }
 
-// out[t*Lk + s] = u_t . w_s over the nt rows u_t = u + t*D of a tile and every key w_s = w + s*D, then fin(t, s, dot)
-template <class F>
-__device__ __forceinline__ void tile_dots(const MhArgs& a, const float* __restrict__ u, const float* __restrict__ w, int nt,
-                                          F&& fin) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int64_t s = warp; s < a.Lk; s += kMhWarps) {
-        const float* ws = w + s * a.D;
-        float acc[kMhTile];
-#pragma unroll
-        for (int t = 0; t < kMhTile; ++t) acc[t] = 0.f;
-#pragma unroll 2
-        for (int64_t j = lane; j < a.dh; j += 32) {
-            const float x = __ldg(ws + j);
-#pragma unroll
-            for (int t = 0; t < kMhTile; ++t)
-                if (t < nt) acc[t] = __fadd_rn(acc[t], __fmul_rn(__ldg(u + t * a.D + j), x));
-        }
-#pragma unroll
-        for (int t = 0; t < kMhTile; ++t) {
-            if (t < nt) {
-                const float d = warp_sum(acc[t]);
-                if (lane == 0) fin(t, s, d);
-            }
-        }
-    }
-}
-
 __global__ void __launch_bounds__(kMhThreads) mha_fwd_kernel(MhArgs a) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int64_t bh = blockIdx.x; bh < a.B * a.h; bh += gridDim.x)
@@ -115,18 +76,21 @@ __global__ void __launch_bounds__(kMhThreads) mha_fwd_kernel(MhArgs a) {
         const int nt = (int)min((int64_t)kMhTile, a.Lq - t0);
         const int64_t row = b * a.Lq + t0, col = hd * a.dh;
         float* P = a.probs + (bh * a.Lq + t0) * a.Lk;
-        tile_dots(a, a.q + row * a.D + col, a.k + b * a.Lk * a.D + col, nt, [&](int t, int64_t s, float d) {
-            P[t * a.Lk + s] = masked(a, b, t0 + t, s) ? -INFINITY : __fdiv_rn(d, a.rdh);
-        });
+        attn::tile_dots<kMhTile, kMhWarps, 2>(a.q + row * a.D + col, a.D, a.k + b * a.Lk * a.D + col, a.D, a.Lk, a.dh, nt,
+                                              [&](int t, int64_t s, float d) {
+                                                  P[t * a.Lk + s] = masked(a, b, t0 + t, s) ? -INFINITY : __fdiv_rn(d, a.rdh);
+                                              });
         __syncthreads();
         if (warp < nt) {
             float* p = P + warp * a.Lk;
+            // attn::softmax_row with a store that also writes top schedules this kernel differently, and measured
+            // slower at Lk = 100, so the row is written out here
             float m = -INFINITY;
             for (int64_t s = lane; s < a.Lk; s += 32) m = fmaxf(m, p[s]);
-            m = warp_max(m);
+            m = attn::warp_fmax(m);
             float l = 0.f;
             for (int64_t s = lane; s < a.Lk; s += 32) l = __fadd_rn(l, expf(__fsub_rn(p[s], m)));
-            l = warp_sum(l);
+            l = attn::warp_sum(l);
             float* top = hd == 0 ? a.top + (row + warp) * a.Lk : nullptr;
             for (int64_t s = lane; s < a.Lk; s += 32) {
                 const float y = __fdiv_rn(expf(__fsub_rn(p[s], m)), l);
@@ -157,8 +121,8 @@ __global__ void __launch_bounds__(kMhThreads) mha_bwd_rows_kernel(MhArgs a) {
         const int64_t row = b * a.Lq + t0, col = hd * a.dh, pk = (bh * a.Lq + t0) * a.Lk;
         float* W = a.ds + pk;
         const float* gt = (hd == 0 && a.grad_top != nullptr) ? a.grad_top + row * a.Lk : nullptr;
-        tile_dots(a, a.grad_out + row * a.D + col, a.v + b * a.Lk * a.D + col, nt,
-                  [&](int t, int64_t s, float d) { W[t * a.Lk + s] = d; });
+        attn::tile_dots<kMhTile, kMhWarps, 2>(a.grad_out + row * a.D + col, a.D, a.v + b * a.Lk * a.D + col, a.D, a.Lk, a.dh,
+                                              nt, [&](int t, int64_t s, float d) { W[t * a.Lk + s] = d; });
         __syncthreads();
         if (warp < nt) {
             const float* p = a.probs + pk + warp * a.Lk;
@@ -170,7 +134,7 @@ __global__ void __launch_bounds__(kMhThreads) mha_bwd_rows_kernel(MhArgs a) {
                 w[s] = g;
                 d = __fadd_rn(d, __fmul_rn(__ldg(p + s), g));
             }
-            d = warp_sum(d);
+            d = attn::warp_sum(d);
             for (int64_t s = lane; s < a.Lk; s += 32)
                 w[s] = masked(a, b, t0 + warp, s) ? 0.f : __fdiv_rn(__fmul_rn(__ldg(p + s), __fsub_rn(w[s], d)), a.rdh);
         }
@@ -233,13 +197,13 @@ __device__ __forceinline__ void ln_stats(const LnArgs& a, int64_t r, float& mu, 
     const int64_t base = r * a.d;
     float s = 0.f;
     for (int64_t j = lane; j < a.d; j += 32) s = __fadd_rn(s, ln_z(a, base + j));
-    mu = __fdiv_rn(warp_sum(s), (float)a.d);
+    mu = __fdiv_rn(attn::warp_sum(s), (float)a.d);
     float q = 0.f;
     for (int64_t j = lane; j < a.d; j += 32) {
         const float c = __fsub_rn(ln_z(a, base + j), mu);
         q = __fadd_rn(q, __fmul_rn(c, c));
     }
-    sd = __fsqrt_rn(__fdiv_rn(warp_sum(q), (float)(a.d - 1)));
+    sd = __fsqrt_rn(__fdiv_rn(attn::warp_sum(q), (float)(a.d - 1)));
     den = __fadd_rn(sd, a.eps);
 }
 
@@ -281,8 +245,8 @@ __global__ void __launch_bounds__(kMhThreads) ln_bwd_kernel(LnArgs a) {
                 sg = __fadd_rn(sg, g);
                 sgc = __fadd_rn(sgc, __fmul_rn(g, __fsub_rn(ln_z(a, base + j), mu)));
             }
-            const float mg = __fdiv_rn(warp_sum(sg), (float)a.d);
-            const float kc = -__fdiv_rn(__fdiv_rn(warp_sum(sgc), __fmul_rn(den, den)), __fmul_rn((float)(a.d - 1), sd));
+            const float mg = __fdiv_rn(attn::warp_sum(sg), (float)a.d);
+            const float kc = -__fdiv_rn(__fdiv_rn(attn::warp_sum(sgc), __fmul_rn(den, den)), __fmul_rn((float)(a.d - 1), sd));
             for (int64_t j = lane; j < a.d; j += 32) {
                 const float g = __fmul_rn(__ldg(a.grad_y + base + j), __ldg(a.a2 + j));
                 const float c = __fsub_rn(ln_z(a, base + j), mu);
@@ -322,31 +286,6 @@ __global__ void __launch_bounds__(kMhThreads) ln_param_kernel(LnArgs a) {
     }
 }
 
-bool overlap(const void* a, size_t na, const void* b, size_t nb) {
-    const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
-    return a != nullptr && b != nullptr && na > 0 && nb > 0 && pa < pb + nb && pb < pa + na;
-}
-
-bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) != 0; }
-
-struct Span {
-    const void* p;
-    size_t bytes;
-};
-
-// every output must be disjoint from every input and from every other output
-int check_disjoint(const Span* in, int nin, const Span* out, int nout) {
-    for (int i = 0; i < nout; ++i) {
-        for (int j = 0; j < nin; ++j)
-            if (overlap(out[i].p, out[i].bytes, in[j].p, in[j].bytes))
-                return fail(QD_ERR_INVALID_ARG, "outputs and workspace must not overlap the inputs");
-        for (int j = 0; j < i; ++j)
-            if (overlap(out[i].p, out[i].bytes, out[j].p, out[j].bytes))
-                return fail(QD_ERR_INVALID_ARG, "outputs and workspace must not overlap each other");
-    }
-    return QD_OK;
-}
-
 // checks of the sizes and the mask both attention calls share; fills the sizes of a and the mask's byte span
 int check_mha(const float* q, const float* k, const float* v, const uint8_t* mask, int64_t mB, int64_t mQ, int64_t mK,
               int64_t B, int64_t Lq, int64_t Lk, int64_t heads, int64_t dh, MhArgs* a, size_t* mask_span) {
@@ -371,11 +310,6 @@ int check_mha(const float* q, const float* k, const float* v, const uint8_t* mas
     return QD_OK;
 }
 
-// blockIdx.x walks the (b, head) pairs, blockIdx.y the tiles (or key chunks) of one; both loop past the grid
-dim3 grid_of(int64_t bh, int64_t tiles) {
-    return dim3((unsigned)(bh < kMhMaxGrid ? bh : kMhMaxGrid), (unsigned)(tiles < kMhMaxGridY ? tiles : kMhMaxGridY));
-}
-
 int check_ln(const float* x, const float* a2, int64_t rows, int64_t d, float eps, LnArgs* a) {
     if (rows < 0 || d < 1) return fail(QD_ERR_INVALID_ARG, "rows must be >= 0 and d >= 1 (rows=%lld d=%lld)", (long long)rows, (long long)d);
     if (rows > INT64_MAX / 16 / d) return fail(QD_ERR_INVALID_ARG, "rows * d overflows 64-bit indexing");
@@ -385,8 +319,6 @@ int check_ln(const float* x, const float* a2, int64_t rows, int64_t d, float eps
     a->chunks = (rows + kLnChunk - 1) / kLnChunk;
     return QD_OK;
 }
-
-int ln_grid(int64_t ctas) { return (int)(ctas < kMhMaxGrid ? ctas : kMhMaxGrid); }
 
 }  // namespace
 
@@ -404,16 +336,15 @@ extern "C" int qd_mha_fwd(const float* q, const float* k, const float* v, const 
     if (rc) return rc;
     if (keep != nullptr && !std::isfinite(keep_scale)) return fail(QD_ERR_INVALID_ARG, "keep_scale must be finite");
     if (out == nullptr || probs == nullptr || top == nullptr) return fail(QD_ERR_INVALID_ARG, "NULL out, probs or top");
-    if (misaligned(q) || misaligned(k) || misaligned(v) || misaligned(out) || misaligned(probs) || misaligned(top))
+    if (misaligned(q, 4) || misaligned(k, 4) || misaligned(v, 4) || misaligned(out, 4) || misaligned(probs, 4) || misaligned(top, 4))
         return fail(QD_ERR_INVALID_ARG, "float arrays must be 4-byte aligned");
     const size_t qb = (size_t)(B * Lq * a.D) * sizeof(float), kb = (size_t)(B * Lk * a.D) * sizeof(float);
     const size_t pn = (size_t)(B * heads * Lq * Lk), tb = (size_t)(B * Lq * Lk) * sizeof(float);
-    const Span in[] = {{q, qb}, {k, kb}, {v, kb}, {mask, mspan}, {keep, pn}};
-    const Span outs[] = {{out, qb}, {probs, pn * sizeof(float)}, {top, tb}};
-    rc = check_disjoint(in, 5, outs, 3);
+    rc = check_disjoint({{q, qb}, {k, kb}, {v, kb}, {mask, mspan}, {keep, pn}}, {{out, qb}, {probs, pn * sizeof(float)}, {top, tb}});
     if (rc) return rc;
     a.keep = keep, a.scale = keep_scale, a.out = out, a.probs = probs, a.top = top;
-    mha_fwd_kernel<<<grid_of(B * heads, (Lq + kMhTile - 1) / kMhTile), kMhThreads, 0, as_stream(stream)>>>(a);
+    // blockIdx.x walks the (b, head) pairs, blockIdx.y the tiles (or key chunks) of one; both loop past the grid
+    mha_fwd_kernel<<<grid_2d(B * heads, (Lq + kMhTile - 1) / kMhTile), kMhThreads, 0, as_stream(stream)>>>(a);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }
@@ -430,24 +361,22 @@ extern "C" int qd_mha_bwd(const float* grad_out, const float* grad_top, const fl
     if (keep != nullptr && !std::isfinite(keep_scale)) return fail(QD_ERR_INVALID_ARG, "keep_scale must be finite");
     if (grad_out == nullptr || probs == nullptr || grad_q == nullptr || grad_k == nullptr || grad_v == nullptr)
         return fail(QD_ERR_INVALID_ARG, "NULL grad_out, probs, grad_q, grad_k or grad_v");
-    if (misaligned(grad_out) || misaligned(grad_top) || misaligned(q) || misaligned(k) || misaligned(v) ||
-        misaligned(probs) || misaligned(grad_q) || misaligned(grad_k) || misaligned(grad_v))
+    if (misaligned(grad_out, 4) || misaligned(grad_top, 4) || misaligned(q, 4) || misaligned(k, 4) || misaligned(v, 4) ||
+        misaligned(probs, 4) || misaligned(grad_q, 4) || misaligned(grad_k, 4) || misaligned(grad_v, 4))
         return fail(QD_ERR_INVALID_ARG, "float arrays must be 4-byte aligned");
     const size_t need = qd_mha_workspace_bytes(B, heads, Lq, Lk);
-    if (workspace == nullptr || workspace_bytes < need || misaligned(workspace))
-        return fail(QD_ERR_WORKSPACE, "workspace must be 4-byte aligned and hold qd_mha_workspace_bytes = %zu bytes", need);
+    rc = check_workspace(workspace, workspace_bytes, need, 4, "qd_mha_workspace_bytes(B, heads, Lq, Lk)");
+    if (rc) return rc;
     const size_t qb = (size_t)(B * Lq * a.D) * sizeof(float), kb = (size_t)(B * Lk * a.D) * sizeof(float);
     const size_t pn = (size_t)(B * heads * Lq * Lk), tb = (size_t)(B * Lq * Lk) * sizeof(float);
-    const Span in[] = {{grad_out, qb}, {grad_top, tb}, {q, qb}, {k, kb}, {v, kb}, {probs, pn * sizeof(float)},
-                       {mask, mspan}, {keep, pn}};
-    const Span outs[] = {{grad_q, qb}, {grad_k, kb}, {grad_v, kb}, {workspace, need}};
-    rc = check_disjoint(in, 8, outs, 4);
+    rc = check_disjoint({{grad_out, qb}, {grad_top, tb}, {q, qb}, {k, kb}, {v, kb}, {probs, pn * sizeof(float)}, {mask, mspan}, {keep, pn}},
+                        {{grad_q, qb}, {grad_k, kb}, {grad_v, kb}, {workspace, need}});
     if (rc) return rc;
     a.grad_out = grad_out, a.grad_top = grad_top, a.probs = const_cast<float*>(probs), a.keep = keep, a.scale = keep_scale;
     a.ds = static_cast<float*>(workspace), a.grad_q = grad_q, a.grad_k = grad_k, a.grad_v = grad_v;
     cudaStream_t st = as_stream(stream);
-    mha_bwd_rows_kernel<<<grid_of(B * heads, (Lq + kMhTile - 1) / kMhTile), kMhThreads, 0, st>>>(a);
-    mha_bwd_keys_kernel<<<grid_of(B * heads, (Lk + kMhKChunk - 1) / kMhKChunk), kMhThreads, 0, st>>>(a);
+    mha_bwd_rows_kernel<<<grid_2d(B * heads, (Lq + kMhTile - 1) / kMhTile), kMhThreads, 0, st>>>(a);
+    mha_bwd_keys_kernel<<<grid_2d(B * heads, (Lk + kMhKChunk - 1) / kMhKChunk), kMhThreads, 0, st>>>(a);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }
@@ -462,16 +391,14 @@ extern "C" int qd_onmt_layernorm_fwd(const float* x, const float* residual, cons
     int rc = check_ln(x, a_2, rows, d, eps, &a);
     if (rc) return rc;
     if (b_2 == nullptr || y == nullptr) return fail(QD_ERR_INVALID_ARG, "NULL b_2 or y");
-    if (misaligned(x) || misaligned(residual) || misaligned(a_2) || misaligned(b_2) || misaligned(y))
+    if (misaligned(x, 4) || misaligned(residual, 4) || misaligned(a_2, 4) || misaligned(b_2, 4) || misaligned(y, 4))
         return fail(QD_ERR_INVALID_ARG, "float arrays must be 4-byte aligned");
     const size_t xb = (size_t)(rows * d) * sizeof(float), pb = (size_t)d * sizeof(float);
-    const Span in[] = {{x, xb}, {residual, xb}, {a_2, pb}, {b_2, pb}};
-    const Span outs[] = {{y, xb}};
-    rc = check_disjoint(in, 4, outs, 1);
+    rc = check_disjoint({{x, xb}, {residual, xb}, {a_2, pb}, {b_2, pb}}, {{y, xb}});
     if (rc) return rc;
     if (rows == 0) return QD_OK;
     a.res = residual, a.b2 = b_2, a.y = y;
-    ln_fwd_kernel<<<ln_grid((rows + kMhWarps - 1) / kMhWarps), kMhThreads, 0, as_stream(stream)>>>(a);
+    ln_fwd_kernel<<<clamp_grid((rows + kMhWarps - 1) / kMhWarps), kMhThreads, 0, as_stream(stream)>>>(a);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }
@@ -485,21 +412,23 @@ extern "C" int qd_onmt_layernorm_bwd(const float* grad_y, const float* x, const 
     if (rc) return rc;
     if (grad_y == nullptr || grad_x == nullptr || grad_a_2 == nullptr || grad_b_2 == nullptr)
         return fail(QD_ERR_INVALID_ARG, "NULL grad_y, grad_x, grad_a_2 or grad_b_2");
-    if (misaligned(grad_y) || misaligned(x) || misaligned(residual) || misaligned(a_2) || misaligned(grad_x) || misaligned(grad_a_2) || misaligned(grad_b_2))
+    if (misaligned(grad_y, 4) || misaligned(x, 4) || misaligned(residual, 4) || misaligned(a_2, 4) || misaligned(grad_x, 4) ||
+        misaligned(grad_a_2, 4) || misaligned(grad_b_2, 4))
         return fail(QD_ERR_INVALID_ARG, "float arrays must be 4-byte aligned");
     const size_t need = qd_onmt_layernorm_workspace_bytes(rows, d);
-    if ((need > 0 && workspace == nullptr) || workspace_bytes < need || misaligned(workspace))
-        return fail(QD_ERR_WORKSPACE, "workspace must be 4-byte aligned and hold qd_onmt_layernorm_workspace_bytes = %zu bytes", need);
+    if (need > 0 || workspace != nullptr) {   // d = 1 or rows = 0 takes a NULL workspace, but no misaligned one
+        rc = check_workspace(workspace, workspace_bytes, need, 4, "qd_onmt_layernorm_workspace_bytes(rows, d)");
+        if (rc) return rc;
+    }
     const size_t xb = (size_t)(rows * d) * sizeof(float), pb = (size_t)d * sizeof(float);
-    const Span in[] = {{grad_y, xb}, {x, xb}, {residual, xb}, {a_2, pb}};
-    const Span outs[] = {{grad_x, xb}, {grad_a_2, pb}, {grad_b_2, pb}, {workspace, need}};
-    rc = check_disjoint(in, 4, outs, 4);
+    rc = check_disjoint({{grad_y, xb}, {x, xb}, {residual, xb}, {a_2, pb}},
+                        {{grad_x, xb}, {grad_a_2, pb}, {grad_b_2, pb}, {workspace, need}});
     if (rc) return rc;
     a.res = residual, a.grad_y = grad_y, a.grad_x = grad_x, a.grad_a2 = grad_a_2, a.grad_b2 = grad_b_2;
     a.partial = static_cast<float*>(workspace);
     cudaStream_t st = as_stream(stream);
-    if (rows > 0) ln_bwd_kernel<<<ln_grid(a.chunks), kMhThreads, 0, st>>>(a);
-    ln_param_kernel<<<ln_grid((2 * d + kMhThreads - 1) / kMhThreads), kMhThreads, 0, st>>>(a);
+    if (rows > 0) ln_bwd_kernel<<<clamp_grid(a.chunks), kMhThreads, 0, st>>>(a);
+    ln_param_kernel<<<clamp_grid((2 * d + kMhThreads - 1) / kMhThreads), kMhThreads, 0, st>>>(a);
     QD_CUDA(cudaGetLastError());
     return QD_OK;
 }

@@ -242,11 +242,6 @@ __global__ void __launch_bounds__(kNlThreads) nmt_loss_bwd_kernel(NlBwdArgs a) {
     }
 }
 
-bool overlap(const void* a, size_t na, const void* b, size_t nb) {
-    const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
-    return a != nullptr && b != nullptr && na > 0 && nb > 0 && pa < pb + nb && pb < pa + na;
-}
-
 // the checks both calls share
 int check_common(const float* logits, const int64_t* target, int64_t R, int64_t V, int64_t padding_idx, float w) {
     if (R < 0 || V < 1) return fail(QD_ERR_INVALID_ARG, "rows must be >= 0 and V >= 1 (rows=%lld V=%lld)", (long long)R, (long long)V);
@@ -254,12 +249,10 @@ int check_common(const float* logits, const int64_t* target, int64_t R, int64_t 
     if (R > INT64_MAX / 4 / V) return fail(QD_ERR_INVALID_ARG, "rows * V overflows 64-bit indexing");
     if (padding_idx < -1 || padding_idx >= V) return fail(QD_ERR_INVALID_ARG, "padding_idx must be -1 (none) or in [0, V)");
     if (!(w >= 0.f && w <= 1.f)) return fail(QD_ERR_INVALID_ARG, "weight_teacher_loss must be in [0, 1]");
-    if ((reinterpret_cast<uintptr_t>(logits) & 3) || (reinterpret_cast<uintptr_t>(target) & 7))
+    if (misaligned(logits, 4) || misaligned(target, 8))
         return fail(QD_ERR_INVALID_ARG, "logits must be 4-byte and target 8-byte aligned");
     return QD_OK;
 }
-
-constexpr int kNlMaxGrid = 1 << 20;   // rows beyond it loop inside the CTAs
 
 }  // namespace
 
@@ -271,23 +264,18 @@ extern "C" int qd_nmt_loss_fwd(const float* logits, const float* teacher_logits,
     int rc = check_common(logits, target, rows, V, padding_idx, w);
     if (rc) return rc;
     if (loss == nullptr || counts == nullptr || (rows > 0 && row_lse == nullptr)) return fail(QD_ERR_INVALID_ARG, "NULL argument");
-    if ((reinterpret_cast<uintptr_t>(teacher_logits) & 3) || (reinterpret_cast<uintptr_t>(row_lse) & 3) ||
-        (reinterpret_cast<uintptr_t>(loss) & 3) || (reinterpret_cast<uintptr_t>(counts) & 7))
+    if (misaligned(teacher_logits, 4) || misaligned(row_lse, 4) || misaligned(loss, 4) || misaligned(counts, 8))
         return fail(QD_ERR_INVALID_ARG, "misaligned output (teacher_logits, row_lse, loss 4 bytes, counts 8 bytes)");
     const size_t need = qd_nmt_loss_workspace_bytes(rows);
-    if (need > 0 && (workspace == nullptr || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 15)))
-        return fail(QD_ERR_WORKSPACE, "workspace must be 16-byte aligned and hold qd_nmt_loss_workspace_bytes(%lld) = %zu bytes",
-                    (long long)rows, need);
-    const size_t in_bytes = (size_t)(rows * V) * sizeof(float);
-    const void* outs[4] = {row_lse, loss, counts, workspace};
-    const size_t out_bytes[4] = {(size_t)rows * 2 * sizeof(float), sizeof(float), 3 * sizeof(int64_t), need};
-    for (int i = 0; i < 4; ++i) {
-        if (overlap(outs[i], out_bytes[i], logits, in_bytes) || overlap(outs[i], out_bytes[i], teacher_logits, in_bytes) ||
-            overlap(outs[i], out_bytes[i], target, (size_t)rows * sizeof(int64_t)))
-            return fail(QD_ERR_INVALID_ARG, "outputs must not overlap the inputs");
-        for (int j = 0; j < i; ++j)
-            if (overlap(outs[i], out_bytes[i], outs[j], out_bytes[j])) return fail(QD_ERR_INVALID_ARG, "outputs must not overlap each other");
+    if (need > 0) {                       // rows = 0 takes any workspace pointer, NULL or not
+        rc = check_workspace(workspace, workspace_bytes, need, 16, "qd_nmt_loss_workspace_bytes(rows)");
+        if (rc) return rc;
     }
+    const size_t in_bytes = (size_t)(rows * V) * sizeof(float);
+    rc = check_disjoint({{logits, in_bytes}, {teacher_logits, in_bytes}, {target, (size_t)rows * sizeof(int64_t)}},
+                        {{row_lse, (size_t)rows * 2 * sizeof(float)}, {loss, sizeof(float)}, {counts, 3 * sizeof(int64_t)},
+                         {workspace, need}});
+    if (rc) return rc;
     NlArgs a{};
     a.zs = logits, a.zt = teacher_logits, a.target = target, a.row_lse = row_lse;
     a.part = static_cast<RowPartial*>(workspace);
@@ -295,7 +283,7 @@ extern "C" int qd_nmt_loss_fwd(const float* logits, const float* teacher_logits,
     a.w = teacher_logits != nullptr ? (double)w : 0.0;
     cudaStream_t st = as_stream(stream);
     if (rows > 0) {
-        const unsigned grid = (unsigned)(rows < kNlMaxGrid ? rows : kNlMaxGrid);
+        const unsigned grid = clamp_grid(rows);
         if (teacher_logits != nullptr) nmt_loss_fwd_kernel<true><<<grid, kNlThreads, 0, st>>>(a);
         else nmt_loss_fwd_kernel<false><<<grid, kNlThreads, 0, st>>>(a);
     }
@@ -311,19 +299,18 @@ extern "C" int qd_nmt_loss_bwd(const float* logits, const float* teacher_logits,
     if (rc) return rc;
     if (rows == 0) return QD_OK;
     if (row_lse == nullptr || grad_loss == nullptr || grad_logits == nullptr) return fail(QD_ERR_INVALID_ARG, "NULL argument");
-    if ((reinterpret_cast<uintptr_t>(teacher_logits) & 3) || (reinterpret_cast<uintptr_t>(row_lse) & 3) ||
-        (reinterpret_cast<uintptr_t>(grad_loss) & 3) || (reinterpret_cast<uintptr_t>(grad_logits) & 3))
+    if (misaligned(teacher_logits, 4) || misaligned(row_lse, 4) || misaligned(grad_loss, 4) || misaligned(grad_logits, 4))
         return fail(QD_ERR_INVALID_ARG, "float arguments must be 4-byte aligned");
     const size_t bytes = (size_t)(rows * V) * sizeof(float);
-    if (overlap(grad_logits, bytes, logits, bytes) || overlap(grad_logits, bytes, teacher_logits, bytes) ||
-        overlap(grad_logits, bytes, target, (size_t)rows * sizeof(int64_t)) ||
-        overlap(grad_logits, bytes, row_lse, (size_t)rows * 2 * sizeof(float)) || overlap(grad_logits, bytes, grad_loss, sizeof(float)))
-        return fail(QD_ERR_INVALID_ARG, "grad_logits must not overlap the inputs");
+    rc = check_disjoint({{logits, bytes}, {teacher_logits, bytes}, {target, (size_t)rows * sizeof(int64_t)},
+                         {row_lse, (size_t)rows * 2 * sizeof(float)}, {grad_loss, sizeof(float)}},
+                        {{grad_logits, bytes}});
+    if (rc) return rc;
     NlBwdArgs a{};
     a.zs = logits, a.zt = teacher_logits, a.target = target, a.row_lse = row_lse, a.grad_loss = grad_loss, a.grad = grad_logits;
     a.R = rows, a.V = V, a.padding_idx = padding_idx;
     a.w = teacher_logits != nullptr ? w : 0.f;
-    const unsigned grid = (unsigned)(rows < kNlMaxGrid ? rows : kNlMaxGrid);
+    const unsigned grid = clamp_grid(rows);
     cudaStream_t st = as_stream(stream);
     if (teacher_logits != nullptr) nmt_loss_bwd_kernel<true><<<grid, kNlThreads, 0, st>>>(a);
     else nmt_loss_bwd_kernel<false><<<grid, kNlThreads, 0, st>>>(a);

@@ -23,7 +23,6 @@ namespace {
 
 constexpr int kSruThreads = 128;
 constexpr int kSruAhead = 4;        // steps whose loads are in flight ahead of the math
-constexpr int64_t kSruMaxGrid = 1 << 20;
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
 __device__ __forceinline__ float reluf_(float x) { return (x > 0.f) ? x : 0.f; }
@@ -182,13 +181,6 @@ __global__ void __launch_bounds__(kSruThreads) sru_bias_kernel(SruArgs a) {
     }
 }
 
-bool overlap(const void* a, size_t na, const void* b, size_t nb) {
-    const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
-    return a != nullptr && b != nullptr && na > 0 && nb > 0 && pa < pb + nb && pb < pa + na;
-}
-
-bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) != 0; }
-
 // checks both calls share; on success fills the sizes of a
 int check_common(const float* u, const float* x, const float* bias, int64_t len, int64_t batch, int64_t d, int k,
                  int bidirectional, int activation, SruArgs* a) {
@@ -209,28 +201,7 @@ int check_common(const float* u, const float* x, const float* bias, int64_t len,
     return QD_OK;
 }
 
-int grid_of(int64_t n) {
-    const int64_t g = (n + kSruThreads - 1) / kSruThreads;
-    return (int)(g < kSruMaxGrid ? g : kSruMaxGrid);
-}
-
-struct Span {
-    const void* p;
-    size_t bytes;
-};
-
-// every output must be disjoint from every input and from every other output
-int check_disjoint(const Span* in, int nin, const Span* out, int nout) {
-    for (int i = 0; i < nout; ++i) {
-        for (int j = 0; j < nin; ++j)
-            if (overlap(out[i].p, out[i].bytes, in[j].p, in[j].bytes))
-                return fail(QD_ERR_INVALID_ARG, "outputs and workspace must not overlap the inputs");
-        for (int j = 0; j < i; ++j)
-            if (overlap(out[i].p, out[i].bytes, out[j].p, out[j].bytes))
-                return fail(QD_ERR_INVALID_ARG, "outputs and workspace must not overlap each other");
-    }
-    return QD_OK;
-}
+unsigned grid_of(int64_t n) { return clamp_grid((n + kSruThreads - 1) / kSruThreads); }
 
 template <class F>
 void with_k(int k, bool v4, F&& f) {
@@ -252,13 +223,12 @@ extern "C" int qd_sru_fwd(const float* u, const float* x, const float* bias, con
     int rc = check_common(u, x, bias, len, batch, d, k, bidirectional, activation, &a);
     if (rc) return rc;
     if (h == nullptr || c == nullptr) return fail(QD_ERR_INVALID_ARG, "NULL h or c");
-    if (misaligned(u) || misaligned(x) || misaligned(bias) || misaligned(init) || misaligned(mask_h) || misaligned(h) ||
-        misaligned(c))
+    if (misaligned(u, 4) || misaligned(x, 4) || misaligned(bias, 4) || misaligned(init, 4) || misaligned(mask_h, 4) ||
+        misaligned(h, 4) || misaligned(c, 4))
         return fail(QD_ERR_INVALID_ARG, "float arrays must be 4-byte aligned");
     const size_t seq = (size_t)(len * a.ncols) * sizeof(float), col = (size_t)a.ncols * sizeof(float);
-    const Span in[] = {{u, seq * k}, {x, seq}, {bias, 2 * (size_t)a.dcols * sizeof(float)}, {init, col}, {mask_h, col}};
-    const Span out[] = {{h, seq}, {c, seq}};
-    rc = check_disjoint(in, 5, out, 2);
+    rc = check_disjoint({{u, seq * k}, {x, seq}, {bias, 2 * (size_t)a.dcols * sizeof(float)}, {init, col}, {mask_h, col}},
+                        {{h, seq}, {c, seq}});
     if (rc) return rc;
     a.u = u, a.x = x, a.bias = bias, a.init = init, a.mask_h = mask_h, a.h = h, a.cout = c;
     cudaStream_t st = as_stream(stream);
@@ -281,19 +251,17 @@ extern "C" int qd_sru_bwd(const float* u, const float* x, const float* bias, con
         return fail(QD_ERR_INVALID_ARG, "NULL c, grad_h, grad_u or grad_bias");
     if (k == 3 && grad_x == nullptr) return fail(QD_ERR_INVALID_ARG, "k = 3 writes grad_x: it must not be NULL");
     if (k == 4 && grad_x != nullptr) return fail(QD_ERR_INVALID_ARG, "k = 4 has no grad_x: it must be NULL");
-    if (misaligned(u) || misaligned(x) || misaligned(bias) || misaligned(init) || misaligned(mask_h) || misaligned(c) ||
-        misaligned(grad_h) || misaligned(grad_last) || misaligned(grad_u) || misaligned(grad_x) ||
-        misaligned(grad_bias) || misaligned(grad_init))
+    if (misaligned(u, 4) || misaligned(x, 4) || misaligned(bias, 4) || misaligned(init, 4) || misaligned(mask_h, 4) ||
+        misaligned(c, 4) || misaligned(grad_h, 4) || misaligned(grad_last, 4) || misaligned(grad_u, 4) ||
+        misaligned(grad_x, 4) || misaligned(grad_bias, 4) || misaligned(grad_init, 4))
         return fail(QD_ERR_INVALID_ARG, "float arrays must be 4-byte aligned");
     const size_t need = qd_sru_workspace_bytes(batch, d, bidirectional);
-    if (workspace == nullptr || workspace_bytes < need || misaligned(workspace))
-        return fail(QD_ERR_WORKSPACE, "workspace must be 4-byte aligned and hold qd_sru_workspace_bytes = %zu bytes", need);
+    rc = check_workspace(workspace, workspace_bytes, need, 4, "qd_sru_workspace_bytes(batch, d, bidirectional)");
+    if (rc) return rc;
     const size_t seq = (size_t)(len * a.ncols) * sizeof(float), col = (size_t)a.ncols * sizeof(float);
     const size_t nb = 2 * (size_t)a.dcols * sizeof(float);
-    const Span in[] = {{u, seq * k}, {x, seq}, {bias, nb}, {init, col}, {mask_h, col}, {c, seq}, {grad_h, seq},
-                       {grad_last, col}};
-    const Span out[] = {{grad_u, seq * k}, {grad_x, seq}, {grad_bias, nb}, {grad_init, col}, {workspace, need}};
-    rc = check_disjoint(in, 8, out, 5);
+    rc = check_disjoint({{u, seq * k}, {x, seq}, {bias, nb}, {init, col}, {mask_h, col}, {c, seq}, {grad_h, seq}, {grad_last, col}},
+                        {{grad_u, seq * k}, {grad_x, seq}, {grad_bias, nb}, {grad_init, col}, {workspace, need}});
     if (rc) return rc;
     a.u = u, a.x = x, a.bias = bias, a.init = init, a.mask_h = mask_h, a.c = c, a.grad_h = grad_h;
     a.grad_last = grad_last, a.grad_u = grad_u, a.grad_x = grad_x, a.grad_init = grad_init;

@@ -23,11 +23,6 @@ from . import _native as N
 IDENTITY, TANH, RELU = 0, 1, 2      # QD_SRU_IDENTITY, QD_SRU_TANH, QD_SRU_RELU
 
 
-def _check_tensor(t, what):
-    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32:
-        raise ValueError(f"{what} must be a float32 CUDA tensor (no CPU implementation)")
-
-
 class _SRUCompute(torch.autograd.Function):
     @staticmethod
     def forward(ctx, u, x, bias, init, mask_h, three_d, d, bidirectional, activation, length, batch, k):
@@ -78,7 +73,7 @@ def sru_compute(u, x, bias, d, bidirectional, activation, init=None, mask_h=None
     Differentiable in u, x (k = 3), bias and init."""
     N.require_cuda()
     for t, what in ((u, "u"), (x, "x"), (bias, "bias")):
-        _check_tensor(t, what)
+        N.check_float_cuda(t, what)
     if x.dim() not in (2, 3):
         raise ValueError("x must be [len, batch, n_in] or [batch, n_in]")
     if activation not in (IDENTITY, TANH, RELU):
@@ -98,7 +93,7 @@ def sru_compute(u, x, bias, d, bidirectional, activation, init=None, mask_h=None
         raise ValueError(f"bias must be [{2 * dir_ * d}], got {tuple(bias.shape)}")
     for t, what in ((init, "init"), (mask_h, "mask_h")):
         if t is not None:
-            _check_tensor(t, what)
+            N.check_float_cuda(t, what)
             if t.numel() != batch * dir_ * d:
                 raise ValueError(f"{what} must hold batch*dir*d = {batch * dir_ * d} values, got {tuple(t.shape)}")
     if any(t is not None and t.device != u.device for t in (x, bias, init, mask_h)):
@@ -145,8 +140,8 @@ class SRUCell(nn.Module):
     def forward(self, input, c0=None):
         if not isinstance(input, torch.Tensor) or input.dim() not in (2, 3):
             raise ValueError("input must be [len, batch, n_in] or [batch, n_in]")
-        _check_tensor(input, "input")
-        _check_tensor(self.weight, "weight")
+        N.check_float_cuda(input, "input")
+        N.check_float_cuda(self.weight, "weight")
         n_in, n_out = self.n_in, self.n_out
         batch = input.size(-2)
         if self.training and self.rnn_dropout > 0:

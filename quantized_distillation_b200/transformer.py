@@ -25,11 +25,6 @@ import torch.nn as nn
 from . import _native as N
 
 
-def _check_tensor(t, what, dims):
-    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or t.dim() != dims:
-        raise ValueError(f"{what} must be a {dims}-D float32 CUDA tensor (no CPU implementation)")
-
-
 def _as_bytes(m):
     """uint8 view of a bool or uint8 tensor, strides kept (a stride-0 expanded mask stays a view)."""
     return m.view(torch.uint8) if m.dtype == torch.bool else m
@@ -88,9 +83,9 @@ def mha_core(q, k, v, heads, mask=None, keep=None, p=0.0):
     out: [B, Lq, D] = sum_s p' v_s per head, unshaped as the reference; top_attn: head 0's probabilities [B, Lq, Lk].
     Differentiable in q, k and v (through both outputs).  The backward saves q, k, v, the probabilities and keep."""
     N.require_cuda()
-    _check_tensor(q, "q", 3)
-    _check_tensor(k, "k", 3)
-    _check_tensor(v, "v", 3)
+    N.check_float_cuda(q, "q", 3)
+    N.check_float_cuda(k, "k", 3)
+    N.check_float_cuda(v, "v", 3)
     if not isinstance(heads, int) or heads < 1:
         raise ValueError("heads must be a positive int")
     B, Lq, D = q.shape
@@ -160,14 +155,14 @@ def onmt_layer_norm(x, a_2, b_2, eps, residual=None):
     (z - mean) / (std + eps) * a_2 + b_2 with the unbiased std; z itself when d = 1.  Differentiable in x, a_2, b_2 and
     residual."""
     N.require_cuda()
-    _check_tensor(x, "x", 2)
-    _check_tensor(a_2, "a_2", 1)
-    _check_tensor(b_2, "b_2", 1)
+    N.check_float_cuda(x, "x", 2)
+    N.check_float_cuda(a_2, "a_2", 1)
+    N.check_float_cuda(b_2, "b_2", 1)
     d = x.shape[1]
     if a_2.shape[0] != d or b_2.shape[0] != d:
         raise ValueError(f"a_2 {tuple(a_2.shape)} and b_2 {tuple(b_2.shape)} must have the width {d} of x")
     if residual is not None:
-        _check_tensor(residual, "residual", 2)
+        N.check_float_cuda(residual, "residual", 2)
         if residual.shape != x.shape:
             raise ValueError(f"residual {tuple(residual.shape)} must have the shape of x {tuple(x.shape)}")
         residual = residual.contiguous()
@@ -238,7 +233,7 @@ class MultiHeadedAttention(nn.Module):
 
     def forward(self, key, value, query, mask=None):
         for t, what in ((key, "key"), (value, "value"), (query, "query")):
-            _check_tensor(t, what, 3)
+            N.check_float_cuda(t, what, 3)
         B, Lk, d = key.shape
         if value.shape != key.shape or query.shape[0] != B or query.shape[2] != d or d != self.model_dim:
             raise ValueError(f"key {tuple(key.shape)}, value {tuple(value.shape)} and query {tuple(query.shape)} do not "

@@ -443,7 +443,7 @@ def test_c_abi_refusals(N):
     bad = [dict(kind=2), dict(kind=-1), dict(kind=0), dict(n=-1), dict(s=-1), dict(h=-1), dict(t=-1), dict(s=0), dict(h=0),
            dict(sN=-1), dict(sS=2), dict(sN=H, sS=H), dict(sS=1 << 62), dict(ip=0), dict(cp=0), dict(ap=0), dict(op=0),
            dict(ap=N.ptr(align) + 2), dict(cp=N.ptr(ctx) + 1), dict(ap=N.ptr(concat)), dict(op=N.ptr(inp)),
-           dict(ap=N.ptr(ctx))]
+           dict(ap=N.ptr(ctx)), dict(ap=N.ptr(align) + 2, op=N.ptr(inp)), dict(ip=0, cp=N.ptr(ctx) + 1)]
     for kw in bad:
         assert fwd(**kw) == N.QD_ERR_INVALID_ARG, kw
     gc = torch.randn(T, Nb, 2 * H, device="cuda")
@@ -460,6 +460,8 @@ def test_c_abi_refusals(N):
     assert bwd() == N.QD_OK
     assert bwd(wn=need - 1) == N.QD_ERR_WORKSPACE
     assert bwd(wp=0) == N.QD_ERR_WORKSPACE
+    assert bwd(wp=0, gq_=N.ptr(gctx)) == N.QD_ERR_WORKSPACE
+    assert bwd(wn=need - 1, gp=0) == N.QD_ERR_INVALID_ARG
     for kw in (dict(gp=0), dict(gq_=0), dict(gctx_=N.ptr(ctx)), dict(gq_=N.ptr(gctx)), dict(wp=N.ptr(gq)), dict(sS=2),
                dict(gq_=N.ptr(gq) + 2)):
         assert bwd(**kw) == N.QD_ERR_INVALID_ARG, kw

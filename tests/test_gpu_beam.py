@@ -268,10 +268,14 @@ def test_c_abi_refusals(N):
            dict(last=p(st.last) + 4), dict(origin=p(st.origin) + 4), dict(flat=p(st.flat) + 4), dict(tokens=p(st.tokens) + 4),
            dict(n_fin=p(st.n_fin) + 2), dict(tokens=p(st.origin)), dict(flat=p(st.tokens) + 8), dict(scores=p(st.out) + 64),
            dict(origin=p(st.last)), dict(ws=p(st.out)), dict(n_fin=p(st.scores)), dict(eos_top=p(st.n_fin) + 1),
-           dict(ws=p(st.origin)), dict(batch=1 << 62)]
+           dict(ws=p(st.origin)), dict(batch=1 << 62), dict(out=p(st.out) + 2, ws=None), dict(scores=None, n_fin=p(st.n_fin) + 2),
+           dict(last=p(st.last) + 4, tokens=p(st.origin))]
     for kw in bad:
         assert call(**kw) == N.QD_ERR_INVALID_ARG, kw
-    for kw in (dict(ws=None), dict(ws_bytes=need - 1), dict(ws=p(st.ws) + 8)):
+    # a batch past the workspace query's range (which then returns 0) still needs a workspace
+    assert lib.qd_beam_workspace_bytes(1 << 53, 1) == 0
+    for kw in (dict(ws=None), dict(ws_bytes=need - 1), dict(ws=p(st.ws) + 8), dict(ws=None, origin=p(st.last)),
+               dict(ws=p(st.ws) + 8, flat=p(st.tokens)), dict(ws=None, batch=1 << 53, beam=1, V=1, eos=0)):
         assert call(**kw) == N.QD_ERR_WORKSPACE, kw
     torch.cuda.synchronize()
     for g, w in zip(st.result(), before):

@@ -314,11 +314,15 @@ def test_c_abi_refusals(N):
     for bad in (dict(zs=None), dict(y=None), dict(lse=None), dict(loss=None), dict(counts=None), dict(R=-1), dict(V=0),
                 dict(pad=-2), dict(pad=V), dict(w=-0.1), dict(w=1.5), dict(w=float("nan")), dict(counts=N.ptr(counts) + 4),
                 dict(zs=N.ptr(zs) + 2), dict(lse=N.ptr(zs)), dict(loss=N.ptr(zt) + 4), dict(counts=N.ptr(y)),
-                dict(lse=N.ptr(ws)), dict(R=1 << 62, V=1 << 10)):
+                dict(lse=N.ptr(ws)), dict(R=1 << 62, V=1 << 10), dict(zs=N.ptr(zs) + 2, lse=N.ptr(zs)),
+                dict(loss=None, counts=N.ptr(counts) + 4), dict(counts=N.ptr(counts) + 4, ws=None)):
         assert fwd(**bad) == N.QD_ERR_INVALID_ARG, bad
         assert L.qd_last_error().decode()
-    for bad in (dict(ws=None), dict(wsb=ws.numel() - 1), dict(ws=N.ptr(ws) + 8)):
+    for bad in (dict(ws=None), dict(wsb=ws.numel() - 1), dict(ws=N.ptr(ws) + 8), dict(ws=None, lse=N.ptr(zs)),
+                dict(ws=N.ptr(ws) + 8, counts=N.ptr(y))):
         assert fwd(**bad) == N.QD_ERR_WORKSPACE, bad
+    # rows = 0 needs no workspace and takes any pointer for it
+    assert fwd(R=0, zs=None, y=None, lse=None, ws=N.ptr(ws) + 1, wsb=0) == N.QD_OK
     torch.cuda.synchronize()
     gd = torch.ones((), device="cuda")
     grad = torch.empty(R, V, device="cuda")
@@ -329,7 +333,8 @@ def test_c_abi_refusals(N):
         return L.qd_nmt_loss_bwd(*a.values(), N.stream_ptr())
     assert bwd() == N.QD_OK and bwd(R=0, zs=None, y=None) == N.QD_OK
     for bad in (dict(zs=None), dict(y=None), dict(lse=None), dict(g=None), dict(out=None), dict(V=0), dict(pad=V),
-                dict(w=2.0), dict(out=N.ptr(zs)), dict(out=N.ptr(zt) + 4), dict(out=N.ptr(grad) + 2)):
+                dict(w=2.0), dict(out=N.ptr(zs)), dict(out=N.ptr(zt) + 4), dict(out=N.ptr(grad) + 2),
+                dict(out=N.ptr(zs) + 2), dict(g=None, lse=N.ptr(row_lse) + 2)):
         assert bwd(**bad) == N.QD_ERR_INVALID_ARG, bad
     torch.cuda.synchronize()
 

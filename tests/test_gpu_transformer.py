@@ -615,7 +615,8 @@ def test_c_abi_refusals(N):
     assert fwd() == N.QD_OK
     for kw in ({"B": 0}, {"Lq": 0}, {"Lk": -1}, {"h": 0}, {"dh": 0}, {"q": None}, {"out": None}, {"top": None},
                {"q": N.ptr(q) + 2}, {"out": N.ptr(out.t) + 1}, {"out": N.ptr(q)}, {"probs": N.ptr(out.t)},
-               {"mask": N.ptr(q), "sb": -1}, {"keep": N.ptr(k), "scale": float("inf")}, {"Lk": 1 << 62}):
+               {"mask": N.ptr(q), "sb": -1}, {"keep": N.ptr(k), "scale": float("inf")}, {"Lk": 1 << 62},
+               {"q": N.ptr(q) + 2, "out": N.ptr(q)}, {"out": None, "probs": N.ptr(out.t) + 1}):
         out.buf.fill_(NAN)
         assert fwd(**kw) == N.QD_ERR_INVALID_ARG, kw
         assert torch.isnan(out.buf).all(), kw
@@ -635,7 +636,9 @@ def test_c_abi_refusals(N):
                    ({"ws": N.ptr(ws) + 1}, N.QD_ERR_WORKSPACE), ({"go": None}, N.QD_ERR_INVALID_ARG),
                    ({"probs": None}, N.QD_ERR_INVALID_ARG), ({"gq": N.ptr(q)}, N.QD_ERR_INVALID_ARG),
                    ({"gk": N.ptr(gq.t)}, N.QD_ERR_INVALID_ARG), ({"ws": N.ptr(probs.t)}, N.QD_ERR_INVALID_ARG),
-                   ({"gt": N.ptr(q) + 1}, N.QD_ERR_INVALID_ARG), ({"B": 0}, N.QD_ERR_INVALID_ARG)):
+                   ({"gt": N.ptr(q) + 1}, N.QD_ERR_INVALID_ARG), ({"B": 0}, N.QD_ERR_INVALID_ARG),
+                   ({"ws": None, "gq": N.ptr(q)}, N.QD_ERR_WORKSPACE), ({"ws": N.ptr(ws) + 1, "go": None}, N.QD_ERR_INVALID_ARG),
+                   ({"nws": ws.numel() - 1, "gt": N.ptr(q) + 1}, N.QD_ERR_INVALID_ARG)):
         gq.buf.fill_(NAN)
         assert bwd(**kw) == rc, kw
         assert torch.isnan(gq.buf).all(), kw
@@ -663,6 +666,14 @@ def test_c_abi_refusals(N):
         gx.buf.fill_(NAN)
         assert L.qd_onmt_layernorm_bwd(*a, s) == rc, (i, val)
         assert torch.isnan(gx.buf).all()
+    # d = 1 needs no workspace: NULL is accepted, a misaligned pointer is not
+    d1 = list(base)
+    d1[5], d1[10], d1[11] = 1, None, 0
+    assert L.qd_onmt_layernorm_bwd(*d1, s) == N.QD_OK
+    d1[10] = N.ptr(lws) + 1
+    assert L.qd_onmt_layernorm_bwd(*d1, s) == N.QD_ERR_WORKSPACE
+    d1[10], d1[7] = None, N.ptr(x)
+    assert L.qd_onmt_layernorm_bwd(*d1, s) == N.QD_ERR_INVALID_ARG
 
 
 def test_python_refusals(N):
