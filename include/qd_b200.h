@@ -383,6 +383,53 @@ int qd_attn_bwd(const float* grad_concat, const float* grad_align, const float* 
                 int64_t H, float* grad_q, float* grad_context, void* workspace, size_t workspace_bytes,
                 qd_stream_t stream);
 
+/* ---- the core of onmt's GlobalAttention, "mlp" (Bahdanau; onmt/modules/GlobalAttention.py:93-106, 108-188) --------
+ * Between linear_query / linear_context and linear_out: score[n, t, s] = sum_h v_h tanhf(wq[n, t, h] + uh[n, s, h]),
+ * align = softmax_s(score) over all S source positions (no mask), c = sum_s align_s h_s, concat = [c | input].
+ * wq = linear_query(input) (bias included), input, grad_wq: float32 [N, T, H] (row n*T + t), C order.  uh =
+ * linear_context(context) is read at uh[n*uN + s*uS + h] and the context at context[n*sN + s*sS + h], each through
+ * its own two strides with unit stride along H, under the rules of the context of qd_attn_fwd (the transposed view of
+ * a contiguous [S, N, H] and a contiguous [N, S, H] alike); grad_uh and grad_context are written in the layouts of uh
+ * and the context.  v, grad_v: float32 [H].  align, grad_align, concat, grad_concat: t-major [T, N, S] / [T, N, 2H],
+ * exactly as qd_attn_fwd's.  Any 4-byte alignment: every load is scalar.  No limit on H.
+ * Arithmetic: float32, one IEEE rounding per operation (no FMA), tanhf of the CUDA math library (not tanh.approx).
+ * A score is a sum over h = l + 32j per lane l, in j order, of fl(v_h e), e = tanhf(fl(wq + uh)), then a butterfly
+ * over the 32 lanes; the softmax, c and the gradient of the scores are qd_attn_fwd's / qd_attn_bwd's.  The backward
+ * recomputes e (it is never stored) and with gs = align (ga - sum_s align ga), ga = gc . h_s + grad_align, forms the
+ * terms d = fl(gs fl(v_h fl(1 - fl(e e)))):  grad_wq[t, h] = sum_s d, s in order;  grad_uh[s, h] = sum_t d, t in
+ * order;  grad_context[s, h] = sum_t align_{t,s} gc_t[h], t in order;  grad_v[h] = sum over (n, t, s) of fl(gs e):
+ * one partial per (n, chunk of 8 source positions), t in order and s in order within t, then the partials summed
+ * n-major, chunk 0 first.  No atomics.  Everything but grad_v depends on (S, H) alone: a row's forward gives the same
+ * bits alone or in any batch; every call gives the same bits on every run, grad_v included.
+ * Error: tanhf is within 2 ulp (CUDA Math API documentation, single-precision maximum ulp errors), so with the
+ * rounding of wq + uh, |e - tanh(wq + uh)| <= 2^-22 |e| + 2^-24 (1 - e^2) |wq + uh| (+ 2^-149 where the sum is
+ * subnormal); a score is within (ceil(H/32) + 6) * 2^-24 * sum_h |v_h e| + sum_h |v_h| * that; a float32 sum of k
+ * terms in the orders above is within (ceil(k/32) + 6) * 2^-24 * sum|terms| (lane sums) or (k + 2) * 2^-24 *
+ * sum|terms| (ordered sums; for grad_v k = 8T + N*ceil(S/8)), each term of the backward carries 2 |gs v_h e| times
+ * e's error and 3 * 2^-24 |gs v_h| more, align_s the relative 2^-24 |x_s - m| of qd_attn_fwd, and any operation with
+ * a subnormal result up to 2^-149 more.  The tests allow twice these bounds, propagated through the chain to first
+ * order (oracle/attention_mlp_oracle.py, mlp_core_bounds).
+ * Neither call allocates or synchronises: graph-capturable.  Rows 0 (N = 0 or T = 0) do nothing.
+ * QD_ERR_INVALID_ARG: negative sizes, S or H 0 with rows, negative strides or strides that make two (n, s) rows of
+ * uh or of the context overlap, sizes or either extent past 64-bit indexing, NULL or misaligned pointers, outputs
+ * overlapping the inputs or each other.  Nothing is written on a refusal. */
+int qd_attn_mlp_fwd(const float* wq, const float* uh, int64_t uh_batch_stride, int64_t uh_src_stride, const float* v,
+                    const float* input, const float* context, int64_t ctx_batch_stride, int64_t ctx_src_stride,
+                    int64_t N, int64_t T, int64_t S, int64_t H, float* align, float* concat, qd_stream_t stream);
+/* The backward's workspace: N*T*S floats (gs) + N*ceil(S/8)*H floats (the grad_v partials); 0 without rows. */
+size_t qd_attn_mlp_workspace_bytes(int64_t N, int64_t T, int64_t S, int64_t H);
+/* The gradients above; grad_align may be NULL (zero).  The gradient of input is grad_concat[:, H:] plus linear_query's
+ * backward of grad_wq: no work here.  align as written by qd_attn_mlp_fwd on the same wq, uh, v and context.  Three
+ * launches: rows (gs, grad_wq), sources (grad_uh, grad_context, the grad_v partials), the grad_v fold.  workspace:
+ * >= qd_attn_mlp_workspace_bytes(N, T, S, H) bytes, 4-byte aligned, else QD_ERR_WORKSPACE.  Checks as the forward's;
+ * grad_wq, grad_uh, grad_v, grad_context and the workspace must not overlap the inputs or each other.  Nothing is
+ * written on a refusal. */
+int qd_attn_mlp_bwd(const float* grad_concat, const float* grad_align, const float* align, const float* wq,
+                    const float* uh, int64_t uh_batch_stride, int64_t uh_src_stride, const float* v,
+                    const float* context, int64_t ctx_batch_stride, int64_t ctx_src_stride, int64_t N, int64_t T,
+                    int64_t S, int64_t H, float* grad_wq, float* grad_uh, float* grad_v, float* grad_context,
+                    void* workspace, size_t workspace_bytes, qd_stream_t stream);
+
 /* ---- the SRU recurrence of onmt's SRU layers (onmt/modules/SRU.py:71-347, sru_fwd / sru_bwd / sru_bi_fwd /
  * sru_bi_bwd) ----------------------------------------------------------------------------------------------------
  * Columns col = b*(dir*d) + j, dir = 2 when bidirectional, else 1; ncols = batch*dir*d.  u: float32 [len, batch,

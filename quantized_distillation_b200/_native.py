@@ -70,6 +70,10 @@ SIGNATURES = {
     "qd_attn_fwd": (C.c_int, [_i32, _p, _p, _p, _i64, _i64, _i64, _i64, _i64, _i64, _p, _p, _p]),
     "qd_attn_workspace_bytes": (_sz, [_i64, _i64]),
     "qd_attn_bwd": (C.c_int, [_p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _i64, _i64, _p, _p, _p, _sz, _p]),
+    "qd_attn_mlp_fwd": (C.c_int, [_p, _p, _i64, _i64, _p, _p, _p, _i64, _i64, _i64, _i64, _i64, _i64, _p, _p, _p]),
+    "qd_attn_mlp_workspace_bytes": (_sz, [_i64, _i64, _i64, _i64]),
+    "qd_attn_mlp_bwd": (C.c_int, [_p, _p, _p, _p, _p, _i64, _i64, _p, _p, _i64, _i64, _i64, _i64, _i64, _i64, _p, _p, _p, _p,
+                                  _p, _sz, _p]),
     "qd_sru_fwd": (C.c_int, [_p, _p, _p, _p, _p, _i64, _i64, _i64, _i32, _i32, _i32, _p, _p, _p]),
     "qd_sru_workspace_bytes": (_sz, [_i64, _i64, _i32]),
     "qd_sru_bwd": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i32, _i32, _i32, _p, _p, _p, _p, _p, _sz, _p]),

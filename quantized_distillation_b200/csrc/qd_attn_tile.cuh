@@ -3,7 +3,8 @@
 //   1. tile_dots: warp w owns the keys s = w + WARPS*k, lane l the elements j = l + 32i; per row a lane-strided float32
 //      sum and a butterfly over the warp.
 //   2. softmax_row: one warp per row; max, sum of expf(x - max) (lane-strided, butterfly), then expf(x - max) / sum.
-//      qd_mha.cu writes the same row out itself (see there).
+//      qd_mha.cu writes the same row out itself (see there).  softmax_row_bwd is its backward, as global attention's
+//      two backward row kernels take it.
 // The max is fmaxf, which drops a NaN operand.  qd_common.cuh's warp_max propagates NaN and would change the results
 // of rows with NaN scores, so the reductions are defined here and these files do not include qd_common.cuh.
 #pragma once
@@ -66,6 +67,15 @@ __device__ __forceinline__ void softmax_row(const float* row, int64_t n, int lan
     for (int64_t s = lane; s < n; s += 32) l = __fadd_rn(l, expf(__fsub_rn(row[s], m)));
     l = warp_sum(l);
     for (int64_t s = lane; s < n; s += 32) store(s, __fdiv_rn(expf(__fsub_rn(row[s], m)), l));
+}
+
+// The softmax's backward of one row, by the calling warp: row[s] <- p[s] (row[s] - sum_s p[s] row[s]) for the n
+// probabilities p, the sum per lane in s order, then a butterfly.
+__device__ __forceinline__ void softmax_row_bwd(const float* p, float* row, int64_t n, int lane) {
+    float d = 0.f;
+    for (int64_t s = lane; s < n; s += 32) d = __fadd_rn(d, __fmul_rn(__ldg(p + s), row[s]));
+    d = warp_sum(d);
+    for (int64_t s = lane; s < n; s += 32) row[s] = __fmul_rn(__ldg(p + s), __fsub_rn(row[s], d));
 }
 
 }  // namespace attn

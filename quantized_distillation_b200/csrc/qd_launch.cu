@@ -105,7 +105,7 @@ int opt_in_smem(const void* kernel, size_t smem, size_t* opted) {
 
 using namespace qd;
 
-extern "C" int qd_version(void) { return 110; }
+extern "C" int qd_version(void) { return 111; }
 extern "C" const char* qd_last_error(void) { return g_err; }
 
 extern "C" int qd_device_info(int* sm_count, int* cc_major, int* cc_minor) {

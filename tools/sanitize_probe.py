@@ -170,5 +170,15 @@ for L, B, d, k, bi, off in ((1, 1, 1, 4, False, 0), (7, 3, 5, 3, True, 0), (9, 2
     init = torch.randn(B, D, device="cuda", requires_grad=True)
     h, last = sru_compute(u, xin, torch.randn(2 * D, device="cuda"), d, bi, 1, init=init, mask_h=torch.rand(B, D, device="cuda"))
     (h.sum() + last.sum()).backward()
+# "mlp" global attention, forward and backward: one row and partial and full row tiles, S = 1 and past one source
+# chunk, H = 1 and past one CTA, the transposed bank and contiguous [N, S, H] slabs, at offset (unaligned) views
+from quantized_distillation_b200.attention import mlp_attention_core  # noqa: E402
+for Nb, T, S, H, off in ((1, 1, 1, 1, 0), (3, 5, 9, 40, 1), (2, 9, 17, 300, 0), (4, 1, 33, 550, 1)):
+    wq, inp = (torch.randn(Nb * T * H + off, device="cuda")[off:].view(Nb, T, H).requires_grad_(True) for _ in range(2))
+    uh = torch.randn(S * Nb * H + off, device="cuda")[off:].view(S, Nb, H).transpose(0, 1).requires_grad_(True)
+    ctx = torch.randn(Nb, S, H, device="cuda", requires_grad=True)
+    v = torch.randn(H, device="cuda", requires_grad=True)
+    align, concat = mlp_attention_core(wq, uh, v, inp, ctx)
+    (concat.sum() + (align * align).sum()).backward()
 torch.cuda.synchronize()
 print("sanitize probe ok")
